@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py - depth frames/s of the plane-sweep DPV hot path (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--config c1..c5] [--impl engine|reference|reference-gpu]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--config c1..c5] [--impl engine|reference|reference-gpu] [--dump-outputs DIR]
 
 Workloads = BASELINE.json configs (SURVEY 8d). `--config` picks one; the default c2 is the configuration the metric is
 quoted on (the driver's BENCH / SCALE runs use it), the others write the same JSON line for their shape:
@@ -11,7 +11,13 @@ quoted on (the driver's BENCH / SCALE runs use it), the others write the same JS
   c4  1248x376 (the reference CNN rejects 1242x375), 128 KITTI planes, full KVNet streaming, frame chunks sharded over ranks
   c5  1920x1080, 256 planes, 8 source views, first-window KVNET.forward (the 1/2/4/8-GPU throughput sweep)
 One step = one depth frame (c1: one cost volume). Synthetic seeded frames / poses / random-init weights of the reference
-architecture (no datasets or checkpoints offline).
+architecture (no datasets or checkpoints offline): with the same arguments every run sees the same inputs.
+
+--dump-outputs DIR: after the timed steps, the arrays the last timed step computed (what a caller of that path receives) are
+         written as DIR/<name>.npy (float32); an array of more than S = 3 * 2^20 elements (a full-resolution DPV) is stored as
+         a fixed sample of S elements: flat index i * size // S + r_i, r_i < size // S drawn by numpy.random.RandomState(1234)
+         (one element per stratum, a cost of O(S)). Two builds run with the same arguments can then be compared output for
+         output. Engine runs only (--impl engine).
 
 value  : whole-job frames/s with the inputs already resident in HBM (engine C ABI, device pointers).
 e2e    : the same metric through the public Python surface with pinned HOST buffers inside the timed region, every step:
@@ -19,15 +25,15 @@ e2e    : the same metric through the public Python surface with pinned HOST buff
          c3/c4 stream ONE decoded uint8 frame per step into the resident FrameWindow (mdataloader mirror, SURVEY f-4),
          run the reference-named inference step (test_utils.test_KVNet.test: forward + DPV propagation) and read back the
          depth map and the confidence map (export_res mirror, f-2).
-roofline: the dominant kernel family (conv_h2_kernel, tcgen05 kind::f16 on split-fp16 pairs) timed with CUDA events around
+roofline: the dominant kernel family (conv_wg_kernel, wgmma on split-fp16 pairs) timed with CUDA events around
          every launch on the launching stream, in eager frames with ONE frame in flight run right after the timed region;
          the frames/s of that same regime is reported next to it (roofline.regime). achieved = algorithmic fp32 FLOPs /
-         kernel time against the measured bf16 tensor peak (MEASURED_PEAKS.json; the kernel issues 3 f16 MMAs per
+         kernel time against the bf16 tensor peak (MEASURED_PEAKS.json, else the H100 SXM data sheet; the kernel issues 3 f16 MMAs per
          product: its MMA rate is 3x the algorithmic rate). The geometry kernels' HBM fractions are listed in config.hbm_kernels.
-cpu_baseline / --impl reference: the UNMODIFIED reference (baseline/_ref, copied by baseline/fetch_reference.py) through its
+cpu_baseline / --impl reference: the UNMODIFIED reference (oracle/_ref, copied by build(); $NRGBD_REFERENCE_CODE overrides) through its
          own models.KVNET.KVNET.forward / test_utils.test_KVNet.test on the host cores (the 4-line .cuda() shim of SURVEY
-         8c; kind "reference"); oracle/torch_port.py (kind "port") only when baseline/_ref is absent.
---impl reference-gpu: the same unmodified reference, unshimmed, eager ATen/cuDNN on the same B200 (SURVEY 8d ii), with
+         8c; kind "reference"); oracle/torch_port.py (kind "port") only when that copy is absent.
+--impl reference-gpu: the same unmodified reference, unshimmed, eager ATen/cuDNN on the same GPU (SURVEY 8d ii), with
          cudnn.benchmark as test_KVNet.py:10 sets it; also records its TF32-default vs fp32 deviation (the noise floor
          the reference itself has on this GPU).
 
@@ -50,7 +56,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
-REF_CODE = os.path.join(ROOT, 'baseline', '_ref', 'code')
+REF_CODE = os.environ.get('NRGBD_REFERENCE_CODE') or os.path.join(ROOT, 'oracle', '_ref', 'code')   # unmodified reference, see oracle/fetch_reference.py
 
 SCANNET = dict(fx=585.0, fy=585.0, cx=320.0, cy=240.0, d=(0.1, 5.0))          # DSO/cam_info_7scenes.mat, test_KVNet.py ScanNet planes
 CONFIGS = {
@@ -66,7 +72,7 @@ CONFIGS = {
     'c4': dict(kind='stream', H=376, W=1248, D=128, V=4, r=2, intr=dict(fx=721.5377, fy=721.5377, cx=624.0, cy=188.0, d=(1.0, 60.0)), n_stream=12, inflight=2,
                workload='kitti1248x376_d128_v4_full_kvnet_stream (BASELINE.json configs[3]; 1242x375 is rejected by the reference CNN; SURVEY C4)',
                metric='depth frames/sec at 1248x376x128-plane x4-view, full KVNet, streaming'),
-    'c5': dict(kind='first', H=1080, W=1920, D=256, V=8, r=4, intr=dict(fx=1755.0, fy=1755.0, cx=960.0, cy=540.0, d=(0.1, 5.0)), inflight=2,
+    'c5': dict(kind='first', H=1080, W=1920, D=256, V=8, r=4, intr=dict(fx=1755.0, fy=1755.0, cx=960.0, cy=540.0, d=(0.1, 5.0)), inflight=1,
                workload='synthetic1920x1080_d256_v8_dnet_dpv_plus_rnet (BASELINE.json configs[4]; SURVEY C5)',
                metric='depth frames/sec at 1920x1080x256-plane x8-view'),
 }
@@ -78,7 +84,7 @@ def read_peaks():
         j = json.load(open(p))
         return dict(hbm_gbs=j['hbm_gbs'], bf16=j['bf16_tflops'], bf16_sustained=j.get('bf16_tflops_sustained', j['bf16_tflops']),
                     source='measured (MEASURED_PEAKS.json)')
-    return dict(hbm_gbs=6650.0, bf16=1590.0, bf16_sustained=1400.0, source='fallback (B200_PROFILING.md)')
+    return dict(hbm_gbs=3350.0, bf16=989.0, bf16_sustained=989.0, source='H100 SXM data sheet (dense bf16, HBM3), not measured')
 
 
 class ClockSampler(threading.Thread):
@@ -116,15 +122,6 @@ class ClockSampler(threading.Thread):
                 'samples': len(self.rows), 'reasons': sorted(reasons)}
 
 
-def conv_traffic_per_launch():
-    """dram__bytes_read.sum + dram__bytes_write.sum per conv launch (mean over the conv launches of one c2 frame) from the ncu
-    capture of this round's kernels, profiles/r2_conv_dram_traffic.json; None if the file is missing."""
-    try:
-        return float(json.load(open(os.path.join(ROOT, 'profiles', 'r2_conv_dram_traffic.json')))['traffic_bytes_per_launch'])
-    except Exception:
-        return None
-
-
 def make_video(cfg, n_frames, seed):
     from neuralrgbd_b200 import synth
     frames, rng = synth.video(seed, n_frames, cfg['H'], cfg['W'])
@@ -153,7 +150,7 @@ def cam_of(cfg, make_cam, quarter=True):
 
 
 # ==============================================================================================
-# reference arms: the unmodified reference (baseline/_ref) on the host cores / on the same GPU
+# reference arms: the unmodified reference (oracle/_ref) on the host cores / on the same GPU
 # ==============================================================================================
 def pick_cpu_threads():
     """Thread count for the CPU arm: the fastest of {all cores, 64, 32, 16, 8} on a short calibration over the three conv
@@ -185,11 +182,11 @@ def pick_cpu_threads():
 
 
 def reference_runner(cfg, on_gpu):
-    """-> (step(i) -> seconds, description). Drives the unmodified reference (or, without baseline/_ref, the torch port)."""
+    """-> (step(i) -> seconds, description). Drives the unmodified reference (or, without oracle/_ref, the torch port)."""
     import torch
     from neuralrgbd_b200 import arch, synth
     from oracle import planesweep_oracle as O
-    have_ref = os.path.isdir(REF_CODE)
+    have_ref = bool(REF_CODE) and os.path.isdir(REF_CODE)
     scale = 1.0
     crop = None
     if cfg['kind'] != 'sweep' and not on_gpu and cfg['H'] * cfg['W'] * cfg['D'] > 1248 * 376 * 128:
@@ -224,21 +221,21 @@ def reference_runner(cfg, on_gpu):
                     torch.cuda.synchronize()
                 assert torch.isfinite(out).all()
                 return time.perf_counter() - t0
-            return step, 'unmodified reference warping.homography.est_swp_volume_v4 (baseline/_ref)', 'reference', 1.0
+            return step, 'unmodified reference warping.homography.est_swp_volume_v4 (oracle/_ref)', 'reference', 1.0
         from oracle import torch_port as TP
 
         def step(k):
             t0 = time.perf_counter()
             TP.est_swp_volume_v4(torch.from_numpy(c['ref']), torch.from_numpy(c['src']), c['d'], torch.from_numpy(c['R']), torch.from_numpy(c['t']), camn, c['sigma'])
             return time.perf_counter() - t0
-        return step, 'CPU torch port of est_swp_volume_v4 (baseline/_ref absent)', 'port', 1.0
+        return step, 'CPU torch port of est_swp_volume_v4 (oracle/_ref absent)', 'port', 1.0
     r = cfg['r']
     sd = arch.synth_state_dict(5, 64, cfg['D'], r, 64)
     n_frames = 2 * r + 4
     frames, exts = make_video(cfg, n_frames, 7)
     if not have_ref:
         if cfg['kind'] != 'first' or on_gpu:
-            raise RuntimeError('baseline/_ref is not present: only the first-window CPU port is available')
+            raise RuntimeError('oracle/_ref is not present: only the first-window CPU port is available')
         from oracle import torch_port as TP
         P = TP._P(sd)
 
@@ -248,7 +245,7 @@ def reference_runner(cfg, on_gpu):
             t0 = time.perf_counter()
             TP.kvnet_first_window(P, f[-1:], f[None, :-1], poses[None], camn, d, 10.)
             return time.perf_counter() - t0
-        return step, 'CPU torch port of the reference path (oracle/torch_port.py; baseline/_ref absent)', 'port', scale
+        return step, 'CPU torch port of the reference path (oracle/torch_port.py; oracle/_ref absent)', 'port', scale
     sys.path.insert(0, REF_CODE)
     import models.KVNET as m_kvnet                              # reference
     import test_utils.test_KVNet as ref_step                    # reference
@@ -291,7 +288,7 @@ def reference_runner(cfg, on_gpu):
             assert torch.isfinite(out).all()
             state['bv'] = bv
             return time.perf_counter() - t0
-    what = 'unmodified reference (baseline/_ref): models.KVNET.KVNET.forward + resample_vol_cuda through its own test_utils.test_KVNet.test'
+    what = 'unmodified reference (oracle/_ref): models.KVNET.KVNET.forward + resample_vol_cuda through its own test_utils.test_KVNet.test'
     if crop is not None:
         what += ', on a centred %dx%d crop (%.3f of the pixels; frames/s scaled by that factor)' % (cfg['W'], cfg['H'], scale)
     return step, what, 'reference', scale
@@ -404,11 +401,13 @@ def run_sweep(args, cfg):
     e0.record()
     for _ in range(K):
         flush.zero_()
-        Hm.est_swp_volume_v4(ref, src, c['d'], R, t, cam, c['sigma'])
+        cost = Hm.est_swp_volume_v4(ref, src, c['d'], R, t, cam, c['sigma'])
     e1.record()
     barrier()
     launches = int(L.nrgbd_launch_count())
     ms = max_ms(e0.elapsed_time(e1), world, dev)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {'cost_volume': cost})
     # kernel-only time of the sweep (events around each call, no flush in between the event pair)
     ks = []
     for _ in range(10):
@@ -490,7 +489,7 @@ def run_engine(args, cfg):
     model = model.to(dev)
     model.conv_math = args.conv_math
     sharding.broadcast_module(model, src=0)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)          # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)          # > 50 MB L2
     h, w = H_IMG // 4, W_IMG // 4
 
     def barrier():
@@ -561,6 +560,9 @@ def run_engine(args, cfg):
         barrier()
         launches = int(L.nrgbd_launch_count())
         ms_value = max_ms(e0.elapsed_time(e1), world, dev)
+        if args.dump_outputs and rank == 0:
+            last = outs[(Wm + K - 1) % inflight]
+            dump_outputs(args.dump_outputs, {'dmap_cur_refined': last[0], 'dpv_lowres': last[1], 'depth_lowres': last[2]})
 
         def eager_frame(i):
             flush.zero_()
@@ -649,6 +651,14 @@ def run_engine(args, cfg):
         barrier()
         launches = int(L.nrgbd_launch_count())
         ms_value = max_ms(e0.elapsed_time(e1), world, dev)
+        if args.dump_outputs and rank == 0:
+            last = base + K - 1
+            tr = trajs[last % inflight]
+            j = last // inflight
+            out = {'dmap_refined': tr['o_ref'], 'depth_lowres': tr['o_dep'], 'dpv_prior_next': tr['priors'][(j + 1) % 2]}
+            if (j % n_stream) != 0:
+                out.update({'dmap_cur_refined': tr['o_cur'], 'dpv_lowres': tr['o_dpv']})
+            dump_outputs(args.dump_outputs, out)
 
         def eager_frame(i):
             stream_step((1 + i % (n_stream - 1)) * inflight, True)      # chunk 0, a steady-state frame
@@ -791,8 +801,8 @@ def run_engine(args, cfg):
         conv_tflops = conv_flops / (conv_ms * 1e-3) / 1e12 if conv_ms > 0 else 0.0
         sweep_gbs = sw_bytes / (sw_ms * 1e-3) / 1e9 if sw_ms > 0 else 0.0
         peak_tf = peaks['bf16_sustained']       # kernels timed inside a long step -> sustained figure
-        kname = {'f16x3': 'conv_h2_kernel (tcgen05 kind::f16 on split-fp16 operand pairs, halo tile, persistent CTAs; algorithmic fp32 FLOPs, the MMA rate is 3x this)',
-                 'tf32x3': 'conv_tc2_kernel (tcgen05 3xTF32 implicit GEMM; algorithmic fp32 FLOPs, the MMA rate is 3x this)',
+        kname = {'f16x3': 'conv_wg_kernel (wgmma on split-fp16 operand pairs, halo tile; algorithmic fp32 FLOPs, the MMA rate is 3x this)',
+                 'tf32x3': 'conv_wg_kernel (wgmma 3xTF32 implicit GEMM; algorithmic fp32 FLOPs, the MMA rate is 3x this)',
                  'fp32': 'conv_igemm_kernel<128,{32,64}> (fp32 FFMA implicit GEMM)'}[args.conv_math]
         dtype = {'f16x3': 'f32 (split-fp16 pair products: 22-bit significands, fp32 accumulate)', 'tf32x3': 'f32 (3xTF32 error-compensated products, fp32 accumulate)',
                  'fp32': 'f32'}[args.conv_math]
@@ -813,12 +823,10 @@ def run_engine(args, cfg):
             'gpu_launches': launches,
             'clocks': sampler.summary(),
             'roofline': {'bound': 'tensor', 'achieved': conv_tflops, 'peak': peak_tf, 'unit': 'TFLOP/s', 'frac': conv_tflops / peak_tf,
-                         'traffic': conv_traffic_per_launch() if (args.conv_math == 'f16x3' and args.config == 'c2') else None,
+                         'traffic': None,
                          'kernel': kname + ', %d launches/step, avg %.1f us' % (conv_n // P_PROF, 1e3 * conv_ms / max(conv_n, 1)),
                          'regime': {'what': 'CUDA events around every conv launch in %d eager frames, ONE frame in flight, run right after the timed region' % P_PROF,
                                     'frames_per_s_in_this_regime': 1e3 * P_PROF / prof_ms_total, 'frame_ms': prof_ms_total / P_PROF},
-                         'traffic_note': 'bytes per launch: dram__bytes_read.sum + dram__bytes_write.sum, mean over the conv launches of one c2 frame, ncu capture of this '
-                                         "round's kernels (profiles/r2_conv_dram_traffic.json)",
                          'peak_source': peaks['source'] + ', sustained bf16'},
         }
         if args.conv_math in ('f16x3', 'tf32x3'):
@@ -841,6 +849,20 @@ def run_engine(args, cfg):
 
 
 _emit = print
+DUMP_SAMPLE = 3 << 20       # elements: at most five arrays per step, so a dump stays below 64 MB
+
+
+def dump_outputs(dirname, arrays):
+    """Write {name: CUDA tensor} as DIR/<name>.npy (float32). Arrays above DUMP_SAMPLE elements are stored as the fixed seeded
+    sample of DUMP_SAMPLE elements described in the module docstring."""
+    os.makedirs(dirname, exist_ok=True)
+    for name, t in sorted(arrays.items()):
+        a = t.detach().float().cpu().numpy()
+        if a.size > DUMP_SAMPLE:
+            k = np.arange(DUMP_SAMPLE, dtype=np.int64)
+            idx = k * a.size // DUMP_SAMPLE + np.random.RandomState(1234).randint(0, a.size // DUMP_SAMPLE, DUMP_SAMPLE)
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(dirname, name + '.npy'), np.ascontiguousarray(a, np.float32))
 
 
 def main():
@@ -856,8 +878,12 @@ def main():
     ap.add_argument('--dev-bn-unroll', type=int, default=0, help='development: vectors in flight per thread in the BatchNorm pass')
     ap.add_argument('--dev-smem-cap-kb', type=int, default=0, help='development: cap conv_h2 shared memory (co-residency experiment)')
     ap.add_argument('--conv-math', default='f16x3', choices=['fp32', 'tf32x3', 'f16x3'],
-                    help='f16x3: tcgen05 kind::f16 on split-fp16 pairs (default); tf32x3: tcgen05 3xTF32; fp32: exact CUDA-core FFMA implicit GEMM')
+                    help='f16x3: wgmma on split-fp16 pairs (default); tf32x3: wgmma 3xTF32; fp32: exact CUDA-core FFMA implicit GEMM')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='write the outputs of the last timed step to DIR/<name>.npy (float32, at most 64 MB in all)')
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != 'engine':
+        ap.error('--dump-outputs writes the engine\'s outputs: it needs --impl engine')
     cfg = CONFIGS[args.config]
     args.warmup = max(args.warmup, 3) if args.impl == 'engine' else args.warmup
     # stdout carries exactly one JSON line: anything a library prints there meanwhile (e.g. NCCL's version banner with

@@ -1,9 +1,9 @@
-/* nrgbd.h - C ABI of the B200-native plane-sweep DPV engine (libnrgbd.so).
+/* nrgbd.h - C ABI of the H100-native plane-sweep DPV engine (libnrgbd.so).
  *
  * The reference (NVlabs/neuralrgbd) has no FFI / plugin ABI of its own: its boundary is the
  * Python import surface `warping.homography` (free functions) and `models.KVNET.KVNET`
  * (an nn.Module). Each entry point below names the reference call it replaces (paths relative to
- * /root/reference/code); `neuralrgbd_b200/warping/homography.py` and
+ * the reference's code/ directory); `neuralrgbd_b200/warping/homography.py` and
  * `neuralrgbd_b200/models/KVNET.py` bind them through ctypes with the reference's names and
  * argument conventions (see INTEGRATION.md).
  *
@@ -230,7 +230,7 @@ int nrgbd_tap_gather_sum(const float* Q, int N, int D, int H, int W, int Cs, int
 /* y = [relu](x*scale + shift) [+ res] over n_pos positions of Cs channels (C logical). */
 int nrgbd_bn_apply(const float* x, const float* scale, const float* shift, const float* res, int relu,
                    long long n_pos, int Cs, int C, float* y, nrgbd_stream_t stream);
-/* Tensor-core (tcgen05 / TMEM / TMA) variants: 3xTF32 error-compensated products, fp32 accumulate.
+/* Tensor-core (wgmma / TMA) variants: 3xTF32 error-compensated products, fp32 accumulate.
  * Activations and K-major packed weights are passed as their TF32 hi / lo splits
  * (nrgbd_split_tf32, nrgbd_pack_conv_weight_tc -> [taps][Cout_pad][Cin_pad]). Semantics otherwise
  * identical to nrgbd_conv_nhwc / nrgbd_conv_transpose2d_k4s2_nhwc. */
@@ -247,13 +247,13 @@ int nrgbd_conv_transpose2d_k4s2_nhwc_tc(const float* x_hi, const float* x_lo, in
                                         int Cin_pad, int Cs_in, const float* w_hi, const float* w_lo,
                                         const float* bias, int Cout, int Cout_pad, float* y, int Cs_out,
                                         int c_off, int leaky, nrgbd_stream_t stream);
-/* v2 tensor-core kernels: raw fp32 activations (the TF32 split happens in-kernel, operand A is fed
- * from TMEM), pre-split K-major weights. Cout_pad <= 128. Same semantics as the v1 entries. */
-/* Training-mode BatchNorm (+ReLU) of a conv's INPUT, folded into the consuming tcgen05 convolution: x is the RAW output
+/* v2 entries: raw fp32 activations (split into TF32 pairs in stream-ordered scratch right before the GEMM),
+ * pre-split K-major weights. Cout_pad <= 128. Same semantics as the v1 entries. */
+/* Training-mode BatchNorm (+ReLU) of a conv's INPUT, folded into the operand split of the consuming tensor-core convolution: x is the RAW output
  * of the producing conv (psm_submodule.convbn :10-16 = Conv2d + BatchNorm2d, BasicBlock :31-49 conv1 -> bn -> relu -> conv2)
  * and `stats` its per-channel [sum(C) | sum of squares(C)] as written by the conv entry points. The consumer computes
- * scale = gamma / sqrt(var + eps), shift = beta - mean * scale per CTA and applies fmaf(x, scale, shift) (+ReLU) while it
- * converts its operands - the same arithmetic as nrgbd_bn_apply_stats, without that pass over the tensor. Padding stays
+ * scale = gamma / sqrt(var + eps), shift = beta - mean * scale once and applies fmaf(x, scale, shift) (+ReLU) while it
+ * splits its operands - the same arithmetic as nrgbd_bn_apply_stats, without that pass over the tensor. Padding stays
  * zero. running_mean / running_var (optional) get the momentum update once. `stats` must differ from the consumer's own. */
 typedef struct nrgbd_bn_input {
   const double* stats; double count;            /* [2*C] sums of the producing conv; number of positions N*D*H*W */
@@ -275,7 +275,7 @@ int nrgbd_conv_transpose2d_k4s2_nhwc_tc2(const float* x, int N, int Hin, int Win
                                          const float* w_hi, const float* w_lo, const float* bias, int Cout,
                                          int Cout_pad, float* y, int Cs_out, int c_off, int leaky,
                                          nrgbd_stream_t stream);
-/* Second-generation tensor-core path (csrc/conv_f16.cu): tcgen05 kind::f16 on SPLIT-FP16 operand pairs, fp32 accumulate.
+/* Second-generation tensor-core path (csrc/conv_f16.cu): wgmma on SPLIT-FP16 operand pairs, fp32 accumulate.
  * Every fp32 value a is carried as two halves, a = hi + lo * 2^-11 (hi = RN_f16(a), lo = RN_f16((a - hi) * 2^11)), and a
  * product is accumulated as hi*hi + 2^-11 (hi*lo + lo*hi): the 22-bit product of the 3xTF32 path at twice the MMA rate
  * and half the operand bytes. Activations are consumed in pair form (two half tensors with the fp32 tensor's
@@ -331,7 +331,7 @@ int nrgbd_kvnet_set_param(nrgbd_kvnet* e, const char* name, const float* data, l
 int nrgbd_kvnet_set_camera(nrgbd_kvnet* e, int slot, const float* K_host, const float* rays_host, float cx,
                            float cy, double hfov_deg, double vfov_deg);
 int nrgbd_kvnet_set_planes(nrgbd_kvnet* e, const float* d_host, int D);   /* float32(d_candi) */
-int nrgbd_kvnet_set_option(nrgbd_kvnet* e, const char* key, int value);   /* "bn_update_running", "profile", "conv_math" (0 fp32 FFMA, 1 tcgen05 3xTF32, 2 tcgen05 split-fp16 pairs), "use_graph" (CUDA-graph replay, default 1) */
+int nrgbd_kvnet_set_option(nrgbd_kvnet* e, const char* key, int value);   /* "bn_update_running", "profile", "conv_math" (0 fp32 FFMA, 1 wgmma 3xTF32, 2 wgmma split-fp16 pairs), "use_graph" (CUDA-graph replay, default 1) */
 /* with option "profile"=1 the engine brackets its conv (category 0, work = flops) and plane-sweep
  * (category 1, work = algorithmic bytes) launches with CUDA events; this returns and clears the sums. */
 int nrgbd_kvnet_profile_read(nrgbd_kvnet* e, int category, double* ms, double* work, long long* launches);

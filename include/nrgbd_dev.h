@@ -10,16 +10,10 @@
 #ifdef __cplusplus
 extern "C" {
 #endif
-void nrgbd_conv_tc_set_nacc(int n);                /* cap on the rotating main accumulators of conv_tc (0 = auto) */
-void nrgbd_conv_tc_set_dev(int stages, int flags); /* ring depth cap; A/B flags listed in csrc/conv_tc.cu */
-void nrgbd_conv_tc_set_debug_buffer(long long* device_buf); /* [grid][64] clock64 stamps (tools/tc_timeline.py) */
-int nrgbd_mma_probe(int BN, int n_mma, int pattern, int nd, int grp, int two_warps, int n_ctas, long long* out,
-                    nrgbd_stream_t stream);        /* raw tcgen05.mma issue / execution rate probe */
-void nrgbd_dev_set_bn_blocks_per_sm(int b);      /* BatchNorm pass: grid cap in blocks per SM (0 = chosen by tensor size: 8, or 32 from 128 MB) */
+void nrgbd_dev_set_bn_blocks_per_sm(int b);      /* BatchNorm pass: grid cap in blocks per SM (0 = chosen by tensor size: 8, or 32 from 64 MB) */
 void nrgbd_dev_set_bn_unroll(int u);               /* BatchNorm pass: 16-byte vectors in flight per thread (1, 2 or 4; 0 = chosen by tensor size) */
-void nrgbd_dev_conv_h2_set_flags(int flags);       /* conv_f16.cu variants: flags listed next to g_h2_flags */
-void nrgbd_dev_conv_h2_set_smem_cap_kb(int kb);    /* cap on conv_h2's dynamic shared memory (0 = maximum): co-residency experiments */
-void nrgbd_dev_conv_h2_set_debug_buffer(long long* device_buf); /* [grid.y][grid.x][16] clock64 stamps (tools/h2_timeline.py) */
+void nrgbd_dev_conv_h2_set_flags(int flags);       /* tensor-core conv variants: flags listed next to g_h2_flags (conv_f16.cu) */
+void nrgbd_dev_conv_h2_set_smem_cap_kb(int kb);    /* cap on the tensor-core conv's dynamic shared memory per CTA (0 = by plan) */
 #ifdef __cplusplus
 }
 #endif

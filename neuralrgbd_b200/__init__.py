@@ -1,4 +1,4 @@
-"""neuralrgbd_b200: B200-native plane-sweep depth-probability-volume engine behind the
+"""neuralrgbd_b200: H100-native plane-sweep depth-probability-volume engine behind the
 NVlabs/neuralrgbd call surface (`models.KVNET.KVNET`, `warping.homography.*`, `mutils.misc`).
 
 `install_as_reference_modules()` puts the engine behind the reference's own import names so that an
@@ -23,7 +23,7 @@ _PATCHES = (
 def install_as_reference_modules(reference_code_dir=None):
     """Route the reference's hot path through libnrgbd.
 
-    reference_code_dir: the `code/` directory of an NVlabs/neuralrgbd checkout (e.g. baseline/_ref/code). It is put on
+    reference_code_dir: the `code/` directory of an NVlabs/neuralrgbd checkout (e.g. $NRGBD_REFERENCE_CODE). It is put on
     sys.path and the reference's OWN modules are imported; then the mirrored functions / classes are set as
     attributes on them (`warping.homography.est_swp_volume_v4`, `warp_img_feats_v3`, `warp_img_feats_mgpu`,
     `resample_vol_cuda`, `mutils.misc.depth_val_regression`, `models.KVNET.KVNET`, ...). Everything else the reference

@@ -109,14 +109,9 @@ SIGNATURES = {
 # include/nrgbd_dev.h: development probes / A-B knobs. Bound only by dev_lib() (tools/, kernel-variant tests), never by the
 # product modules.
 DEV_SIGNATURES = {
-    'nrgbd_conv_tc_set_nacc': (None, [c_int]),
-    'nrgbd_conv_tc_set_dev': (None, [c_int, c_int]),
-    'nrgbd_conv_tc_set_debug_buffer': (None, [c_vp]),
-    'nrgbd_mma_probe': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     'nrgbd_dev_set_bn_unroll': (None, [c_int]),
     'nrgbd_dev_set_bn_blocks_per_sm': (None, [c_int]),
     'nrgbd_dev_conv_h2_set_flags': (None, [c_int]),
-    'nrgbd_dev_conv_h2_set_debug_buffer': (None, [c_vp]),
     'nrgbd_dev_conv_h2_set_smem_cap_kb': (None, [c_int]),
 }
 

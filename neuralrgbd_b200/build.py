@@ -1,9 +1,9 @@
-"""Build libnrgbd.so (in-tree) with nvcc for sm_100a.
+"""Build libnrgbd.so (in-tree) with nvcc for sm_90a.
 
     python -m neuralrgbd_b200.build [--force]
 
 Every csrc/*.cu / *.cpp is compiled with
-    nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3
+    nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3
 into neuralrgbd_b200/_build/*.o and linked into neuralrgbd_b200/libnrgbd.so. nvcc
 cross-compiles without a GPU; the .so is git-ignored but travels to the GPU box.
 """
@@ -18,7 +18,7 @@ CSRC = os.path.join(HERE, 'csrc')
 OBJ = os.path.join(HERE, '_build')
 LIB = os.path.join(HERE, 'libnrgbd.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
          '-Xcompiler', '-fPIC', '-I', os.path.join(os.path.dirname(HERE), 'include'), '-I', CSRC]
 
 
@@ -52,7 +52,7 @@ def build(force=False, verbose=False):
         with ThreadPoolExecutor(max_workers=min(8, len(jobs))) as ex:
             list(ex.map(run, jobs))
     if jobs or not os.path.exists(LIB) or force:
-        run([NVCC, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a', '-lcudart'])
+        run([NVCC, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a', '-lcudart'])
     return LIB
 
 

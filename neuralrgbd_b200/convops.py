@@ -130,7 +130,7 @@ def upsample_bilinear_ac(x, size):
 
 
 # ---------------------------------------------------------------------------------------------
-# tensor-core (tcgen05, 3xTF32) variants
+# tensor-core (wgmma, 3xTF32) variants
 # ---------------------------------------------------------------------------------------------
 def pad_to(c, m):
     return (c + m - 1) // m * m
@@ -173,7 +173,7 @@ def pack_weight_tc(w, transposed=False):
 
 def conv_tc(x, w, bias=None, stride=1, pad=0, dilation=1, leaky=False, want_stats=False, impl='v1'):
     """Tensor-core counterpart of conv() (same arguments / returns). impl: 'v1' (pre-split activations
-    from global memory) or 'v2' (raw activations, in-kernel split, A operand from TMEM)."""
+    from global memory) or 'v2' (raw activations, split into scratch right before the GEMM)."""
     L = _lib.lib()
     is3d = x.dim() == 5
     N = x.shape[0]
@@ -252,7 +252,7 @@ def conv_tc_bn_in(x_raw, in_stats, gamma, beta, w, bias=None, stride=1, pad=0, d
 
 
 # ---------------------------------------------------------------------------------------------
-# second-generation tensor-core path (csrc/conv_f16.cu): tcgen05 kind::f16 on split-fp16 operand pairs
+# second-generation tensor-core path (csrc/conv_f16.cu): wgmma on split-fp16 operand pairs
 # ---------------------------------------------------------------------------------------------
 def h2_plan(Cin, Cout):
     L = _lib.lib()

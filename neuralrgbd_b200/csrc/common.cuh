@@ -1,4 +1,4 @@
-// Shared helpers for the nrgbd sm_100a kernels.
+// Shared helpers for the nrgbd sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -34,6 +34,16 @@ void nrgbd_set_error(const char* fmt, ...);
 #define NRGBD_LAUNCH_CHECK() NRGBD_CUDA_CHECK(cudaGetLastError())
 
 static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
+
+// SMs of the current device (queried once per translation unit): grid caps of the grid-stride kernels
+static inline int nrgbd_sm_count() {
+  static int n = 0;
+  if (n < 1) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) n = 1;
+  }
+  return n;
+}
 
 // launch counter (bench.py reports it as gpu_launches)
 extern "C" void nrgbd_count_launch(int n);

@@ -13,7 +13,7 @@
 //
 // This is the exact-fp32 (CUDA-core FFMA) path: it is the parity anchor for the conv stacks.
 // DESIGN.md explains why single-pass TF32/BF16 tensor-core operands cannot meet the 1e-4 DPV
-// tolerance (SURVEY §7 'hard parts') and what the tcgen05 3xTF32 variant must do.
+// tolerance (SURVEY §7 'hard parts') and what the wgmma 3xTF32 variant must do.
 #include "common.cuh"
 
 namespace {
@@ -410,9 +410,12 @@ tap_gather_sum_kernel(const float* __restrict__ Q, int D, int H, int W, int Cs, 
   out[((size_t)nd * H + y) * W + x] = acc;
 }
 
-// BatchNorm pass shape, measured over a K-Net volume (1248x376 / 4, D = 128, 64 channels; tools/bench_kernels.py bnsweep): one vector
-// per thread and 8 blocks per SM 418 us (4.6 TB/s) / 680 us with a pair residual; TWO vectors in flight and 32 blocks per SM
-// 333 us (5.8 TB/s) / 471 us (6.1 TB/s = 93 % of the measured copy bandwidth); four vectors 343 / 535 us.
+// BatchNorm pass shape, measured over a K-Net volume (1248x376 / 4, D = 128, 64 channels; tools/bench_kernels.py bnsweep) on an H100
+// SXM (400 W power limit): TWO vectors in flight and 32 blocks per SM 700 us (2.75 TB/s of algorithmic traffic, 82 % of the 3.35 TB/s
+// data-sheet HBM bandwidth) / 1030 us with a pair residual; 1 or 4 vectors and 16 / 32 blocks per SM within 2 % of that; 8 blocks
+// per SM 13-15 % slower whatever the vector count. The same ordering holds at 120x160, D = 64 (245 MB) and at 5x240x320 (98 MB: 95 us
+// against 108 us for the light shape). At 5x120x160 (24.6 MB, mostly L2-resident on the H100's 50 MB) the light shape - one vector,
+// 8 blocks per SM, 41 us - is as fast as any, the streaming one 49 us: the switch sits at 64 MB.
 int g_bn_unroll = 0;           // development override of the vectors in flight per thread (0 = by size; nrgbd_dev_set_bn_unroll)
 int g_bn_blocks_per_sm = 0;    // development override of the grid cap in blocks per SM (0 = by size; nrgbd_dev_set_bn_blocks_per_sm)
 
@@ -543,7 +546,7 @@ int nrgbd_bn_apply_stats(const float* x, const double* stats, double count, cons
   NRGBD_REQUIRE(x && stats && gamma && beta && y && Cs % 4 == 0 && C <= Cs && C <= 512 && n_pos > 0 && count > 0, "bad arguments");
   long long n4 = n_pos * Cs / 4;
   long long blocks = (n4 + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > nrgbd_sm_count() * 8ll) blocks = nrgbd_sm_count() * 8ll;
   bn_apply_stats_kernel<1><<<(unsigned)blocks, 256, 0, st>>>(x, stats, count, gamma, beta, eps, run_mean, run_var, momentum, res, nullptr,
                                                             nullptr, relu, n4, Cs, C, y, nullptr, nullptr, nullptr, nullptr);
   NRGBD_COUNT(1);
@@ -566,11 +569,11 @@ int nrgbd_bn_apply_stats_pair(const float* x, double* stats, double count, const
   const uint2* rl = reinterpret_cast<const uint2*>(res_lo);
   long long n4 = n_pos * Cs / 4;
   long long blocks = (n4 + 255) / 256;
-  // streaming shape (two vectors in flight, 32 blocks per SM) for tensors that do not fit L2 anyway (>= 128 MB of fp32: K-Net volumes,
-  // the 1080p feature maps); the small 2-D passes of a 640x480 frame are launch / L2-latency bound and keep the light shape
-  const bool big = n4 >= (8ll << 20);
+  // streaming shape (two vectors in flight, 32 blocks per SM) for tensors that do not fit L2 anyway (>= 64 MB of fp32: K-Net volumes,
+  // the larger feature maps); the small 2-D passes of a 640x480 frame are launch / L2-latency bound and keep the light shape
+  const bool big = n4 >= (4ll << 20);
   const int unroll = g_bn_unroll > 0 ? g_bn_unroll : (big ? 2 : 1);
-  const long long cap = 148ll * (g_bn_blocks_per_sm > 0 ? g_bn_blocks_per_sm : (big ? 32 : 8));
+  const long long cap = (long long)nrgbd_sm_count() * (g_bn_blocks_per_sm > 0 ? g_bn_blocks_per_sm : (big ? 32 : 8));
   if (blocks > cap) blocks = cap;
   if (unroll == 4)
     bn_apply_stats_kernel<4><<<(unsigned)blocks, 256, 0, st>>>(x, stats, count, gamma, beta, eps, run_mean, run_var, momentum, res, rh, rl,

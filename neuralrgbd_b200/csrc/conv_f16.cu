@@ -1,90 +1,70 @@
-// Tensor-core convolution, second generation: tcgen05 kind::f16 implicit GEMM on SPLIT-FP16 operand pairs with a
-// shared-memory HALO tile (SURVEY §8 a5, a8, a10; DESIGN.md §4.4).
+// Tensor-core convolution: wgmma implicit GEMM on SPLIT operand pairs with a shared-memory HALO tile
+// (SURVEY §8 a5, a8, a10; DESIGN.md §4.4). Hopper (sm_90a): TMA + mbarrier pipeline, wgmma from shared memory,
+// fp32 accumulators in registers.
 //
-// Arithmetic. Every fp32 operand is carried as two halves: a = hi + lo * 2^-11 with hi = RN_f16(a) and
-// lo = RN_f16((a - hi) * 2^11) (a - hi is exact in fp32; the 2^11 scale keeps the residual out of the fp16 subnormal
-// range). A product is accumulated in fp32 TMEM as
-//     main  += a_hi * b_hi                       cross += a_hi * b_lo + a_lo * b_hi          out = main + 2^-11 * cross
-// - the same 22-bit significand product as the 3xTF32 kernel of conv_tc.cu (dropped term 2^-22 |a b|), but kind::f16
-// runs at twice the TF32 MMA rate with half the operand bytes, and needs no in-kernel operand converter: activations
-// are produced in pair form by the previous pass (nrgbd_split_f16_pair or the fused BatchNorm pass), so both operands
-// go TMA -> shared memory -> tensor core and the kernel has the canonical producer / issuer / epilogue structure.
+// Arithmetic. Every fp32 operand is carried as two parts. Split-fp16 pairs (the default path, this file's entry points):
+// a = hi + lo * 2^-11 with hi = RN_f16(a) and lo = RN_f16((a - hi) * 2^11) (a - hi is exact in fp32; the 2^11 scale keeps
+// the residual out of the fp16 subnormal range). 3xTF32 pairs (conv_tc.cu): a = hi + lo, both TF32. A product is
+// accumulated as
+//     main  += a_hi * b_hi                       cross += a_hi * b_lo + a_lo * b_hi          out = main + scale * cross
+// (dropped term ~2^-22 |a b|). Activations are produced in pair form by the previous pass (nrgbd_split_f16_pair or the
+// fused BatchNorm pass), so both operands go TMA -> shared memory -> tensor core.
 //
-// Halo tile. The round-1 kernel fetched one activation box per filter tap: a 3x3 convolution read its input tile
-// nine times from L2 and was L2-bandwidth bound on the 64-channel layers (DESIGN.md §6). Here one (TH + 2p) x (TW + 2p)
-// pixel halo box per (depth tap, 32-channel chunk) is staged once and all in-plane taps read it through shifted
-// UMMA descriptors: the output tile is 16 rows x 8 columns, so one 8-row UMMA core-matrix group is exactly one tile
-// row, a tap (dy, dx) is a start-address offset of (dy * pitch + dx) pixel rows and the stride-byte-offset between
-// groups is the halo pitch (pitch * row bytes, not a multiple of the swizzle atom: the hardware swizzle is a function
-// of the absolute shared-memory address, as is TMA's, so any 16-byte-aligned row offset stays consistent).
-// Strided convolutions fall back to one box per tap ("tap mode", same kernel).
+// Halo tile. One (TH + 2p) x (TW + 2p) pixel halo box per (depth tap, 32-channel chunk) is staged once and all in-plane
+// taps read it through shifted wgmma descriptors: the output tile is 16 rows x 8 columns, so one 8-row core-matrix group
+// is exactly one tile row, a tap (dy, dx) is a start-address offset of (dy * pitch + dx) pixel rows and the stride-byte-
+// offset between groups is the halo pitch (pitch * row bytes, not a multiple of the swizzle atom: the swizzle is a
+// function of the absolute shared-memory address, as is TMA's, so any 16-byte-aligned row offset stays consistent).
+// A 3x3 convolution reads its input tile 1.4x instead of 9x. Strided convolutions use one box per tap ("tap mode").
 //
-// Roles (one 128-pixel x BN-channel tile per CTA; grid.y splits Cout into chunks of BN <= 128):
-//   warp 0      TMA producer: halo / tap box of the hi and the lo activation planes into the A ring, one
-//               [hi rows | lo rows] K-major weight tile per (tap, chunk) into the B ring; expect-tx mbarriers.
-//   warp 1      MMA issuer: per tap and 16-channel slice a_hi x [b_hi | b_lo] as ONE MMA of width 2 BN (main and cross
-//               accumulators are adjacent TMEM columns), then a_lo x b_hi; tcgen05.commit frees the slots.
-//   warps 2-5   (+ 6-9 when the CTA owns the SM) epilogue: tcgen05.ld, main + 2^-11 cross, bias / LeakyReLU, swizzled
-//               staging tile, TMA tensor stores per 32-channel slab, BatchNorm column sums from the staged tile.
-#include <cstdlib>
+// Roles (one 128-pixel x BN-channel tile per CTA, grid.y = Cout chunks of BN <= 128 channels):
+//   warps 0-7   two consumer warpgroups, 64 pixels (8 tile rows) each: per K step and tap, wgmma a_hi x b_hi -> main,
+//               a_hi x b_lo and a_lo x b_hi -> cross; the ring slots of step s are released once step s + 1 is issued
+//               and step s has retired (wgmma.wait_group 1); then the epilogue straight from the registers: main +
+//               scale * cross, bias / LeakyReLU, fp32 or fp16-pair stores, BatchNorm column sums (one pair of fp64
+//               atomics per column and CTA).
+//   warp 8      TMA producer: halo / tap box of the hi and the lo activation planes into the A ring, G taps of the hi and
+//               lo K-major weight tiles into the B ring; expect-tx mbarriers.
 #include <cuda.h>
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "conv_wgmma.cuh"
+#include "wgmma.cuh"
 #include "../../include/nrgbd_dev.h"
 
 namespace {
 
 constexpr int TH = 16, TW = 8;         // output tile: 16 rows x 8 columns = 128 GEMM rows
-constexpr int MAX_TAP2D = 16;
-constexpr float LO_SCALE = 2048.f;     // 2^11
-constexpr float LO_INV = 1.f / 2048.f;
-constexpr float H_MAX = 65504.f;
+constexpr int WG_THREADS = 288;        // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr int BKC = 32;                // input channels per K chunk
 
-struct H2Params {
+struct WgParams {
   float* y; const float* bias; double* stats;
-  void *y_hi, *y_lo;                     // pair_out: the output is written as the split-fp16 operand pair of the next convolution
-  int pair_out;
+  __half *y_hi, *y_lo;
   int N, Dz, Hy, Wx, tiles_x, tiles_y;
-  int cin_chunks, bkc, row_bytes;        // channels per K chunk (32 | 64), bytes of one pixel row of a tile (64 | 128)
-  int n_kz, n_tap;                       // depth taps, in-plane taps
-  int halo;                              // 1: one halo tile per (kz, chunk) serves all in-plane taps; 0: one box per tap
-  int in_stride, org_y, org_x;           // halo mode: tile origin in the input = out * 1 + org
-  int Cout, BN, BN_last;                 // logical output channels; channels per CTA (blockIdx.y * BN = first one); width of the last chunk
-  int Dout, Hout, Wout, Cs_out, c_off, out_stride, out_off_y, out_off_x;
-  int leaky, stages_a, stages_b, tmem_cols, tma_store, dev_flags;
-  int n_chunks, acc_stride;              // Cout chunks; TMEM columns between the two accumulator sets
-  int msub;                              // 128-pixel sub-tiles stacked vertically in one work item (1, 2 or 4): they share every weight tile
-  uint32_t a_sub16;                      // distance between the sub-tiles' first rows inside the A (halo) tile, in 16-byte units
-  uint32_t staging_bytes;
-  uint32_t a_tile_bytes, a_stage_bytes, a_tx_bytes, b_tile_bytes;      // b_tile_bytes: one B ring slot = G taps x [hi | lo] tile
-  int gtaps;                             // in-plane taps per pipeline step (G)
-  uint32_t a_desc_hi, b_desc_hi;         // constant high words of the shared-memory descriptors (SBO, version, swizzle mode)
-  long long* dbg;
+  int cin_chunks, n_kz, n_tap, halo, in_stride, org_y, org_x;
+  int Cout, c_first;                     // logical output channels; first channel of this launch's chunk 0
+  int Dout, Hout, Wout, Cs_out, c_off, out_stride, out_off_y, out_off_x, leaky;
+  int stages_a, stages_b, box_w, box_h;  // ring depths; activation box in pixels (halo pitch x halo rows, or the tile)
+  uint32_t a_tile_bytes, a_stage_bytes, a_tx_bytes, b_stage_bytes, wg_row16;   // wg_row16: 8 tile rows down the A tile, 16-byte units
+  uint32_t a_desc_hi, b_desc_hi;         // high words of the shared-memory descriptors (SBO, swizzle mode)
   signed char dz[3];
-  signed char dy[MAX_TAP2D], dx[MAX_TAP2D];
-  unsigned short a_off16[MAX_TAP2D];     // halo mode: byte offset of the tap inside the halo tile, in 16-byte units
-  unsigned char wsel[3 * MAX_TAP2D];     // weight slice of (kz, tap)
+  signed char dy[WG_MAX_TAP2D], dx[WG_MAX_TAP2D];
+  unsigned short a_off16[WG_MAX_TAP2D];  // halo mode: offset of the tap inside the halo tile, 16-byte units
+  unsigned char wsel[3 * WG_MAX_TAP2D];
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .b32 %%rx;\n\t.reg .pred %%px;\n\t"
-      "elect.sync %%rx|%%px, %1;\n\t"
-      "@%%px mov.s32 %0, 1;\n\t}"
-      : "+r"(pred) : "r"(0xffffffffu));
-  return pred != 0;
-}
-__device__ __forceinline__ int uniform_warp_idx() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x / 32), 0); }
 
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
 }
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  if (elect_one()) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 // Bounded spin: a protocol bug becomes a trap (an error the caller sees) instead of a hung GPU.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
@@ -100,149 +80,69 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
   __trap();
 }
-// development: wait + accumulate the cycles spent waiting (only when a debug buffer is attached)
-__device__ __forceinline__ void mbar_wait_t(uint32_t bar, uint32_t parity, bool timed, long long& acc) {
-  if (!timed) { mbar_wait(bar, parity); return; }
-  const long long t0 = clock64();
-  mbar_wait(bar, parity);
-  acc += clock64() - t0;
-}
 __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2, int c3, int c4) {
-  if (elect_one()) asm volatile(
+  asm volatile(
       "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
       ::"r"(dst), "l"((uint64_t)tm), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
 }
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2, int c3) {
-  if (elect_one()) asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"((uint64_t)tm), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-// low word of a K-major shared-memory matrix descriptor: start address >> 4 [0,14), LBO (ignored when swizzled) = 1 [16,30)
-__device__ __forceinline__ uint32_t desc_lo(uint32_t saddr) { return ((saddr & 0x3FFFFu) >> 4) | (1u << 16); }
-__device__ __forceinline__ uint64_t desc_of(uint32_t hi, uint32_t lo) { return ((uint64_t)hi << 32) | (uint64_t)lo; }
-__device__ __forceinline__ void umma_f16_raw(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+      ::"r"(dst), "l"((uint64_t)tm), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-// Lean issue forms: the 64-bit shared-memory descriptors are packed from (low word, constant high word) inside the asm
-// block, the accumulate predicate is a constant. (Measured on the first version of this kernel: descriptor high words
-// re-loaded from the parameter bank + 64-bit adds + a branch per MMA = ~15 uniform-datapath instructions and ~150
-// cycles per tcgen05.mma, three times the tensor time of an N = 128 MMA.)
-__device__ __forceinline__ void umma_f16_acc(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t idesc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "setp.eq.u32 p, 0, 0;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-      ::"r"(tmem_d), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc) : "memory");
-}
-__device__ __forceinline__ void umma_f16_first(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                               uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-      ::"r"(tmem_d), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void umma_commit_raw(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  if (elect_one()) umma_commit_raw(bar);
+// K-major shared-memory matrix descriptor: start address >> 4 [0,14), LBO >> 4 [16,30) (unused when swizzled: 1),
+// SBO >> 4 [32,46), swizzle mode [62,64) (1: 128 B, 2: 64 B); the high word is precomputed on the host.
+__device__ __forceinline__ uint64_t wg_desc(uint32_t saddr, uint32_t hi) {
+  return ((uint64_t)hi << 32) | (uint64_t)(((saddr & 0x3FFFFu) >> 4) | (1u << 16));
 }
 
-constexpr int H2_THREADS = 320;        // warps: 0 TMA producer, 1 MMA issuer (+ TMEM alloc), 2-5 and 6-9 two epilogue groups
-constexpr int EP_GROUPS = 2;
+template <int BN, bool TF32>
+__device__ __forceinline__ void wg_mma(float* d, uint64_t a, uint64_t b) {
+  if constexpr (TF32) Wgmma<BN>::tf32(d, a, b); else Wgmma<BN>::f16(d, a, b);
+}
 
-// Persistent CTA (one per SM): loops over work items (output tile x Cout chunk) with the operand rings running
-// continuously across items and TWO accumulator sets in TMEM, so that the epilogue of item i (TMEM -> registers ->
-// staging -> TMA store, BatchNorm sums) overlaps the MMAs of item i+1, and barrier set-up / TMEM allocation / the first
-// TMA latency are paid once per SM instead of once per tile (measured on the one-tile-per-CTA form of this kernel:
-// set-up 1.2K + first operands 2-6K + epilogue 3.5K cycles per tile around a 4K-cycle MMA main loop).
-// NKS: 16-channel MMA slices per K chunk (2: 32-channel chunks, 64-byte rows). MSUB: 128-pixel sub-tiles per work item.
-// G: in-plane taps per pipeline step (one weight TMA, one barrier round trip and one commit per G taps: the issuing
-// thread's fixed cost per step - waits, fences, elect, ring arithmetic, ~380 cycles measured - is what bounded the
-// G = 1 form, not L2 traffic: switching all TMA traffic off changed nothing).
-template <int NKS, int MSUB, int G>
-__global__ void __launch_bounds__(H2_THREADS, 1)
-conv_h2_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
-               const __grid_constant__ CUtensorMap tm_b, const __grid_constant__ CUtensorMap tm_b_last,
-               const __grid_constant__ CUtensorMap tm_y, const __grid_constant__ CUtensorMap tm_yh,
-               const __grid_constant__ CUtensorMap tm_yl, const H2Params p) {
-  // shared memory: [A ring: stages_a x (hi tile | lo tile)][B ring: stages_b x ([b_hi rows | b_lo rows])][staging][barriers]
+// BN: output channels per CTA (16..128). TF32: operand kind. G: in-plane taps per pipeline step (one weight box and one
+// barrier round trip per G taps).
+template <int BN, bool TF32, int G>
+__global__ void __launch_bounds__(WG_THREADS, BN <= 64 ? 2 : 1)
+conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
+               const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo, const WgParams p) {
+  constexpr int RB = TF32 ? 128 : 64;                 // bytes of one 32-channel pixel row
+  constexpr int KS = TF32 ? 4 : 2;                    // MMA K slices per 32-channel chunk (32 bytes each)
+  constexpr float SCALE = TF32 ? 1.f : 1.f / 2048.f;
+  constexpr uint32_t B_HALF = (uint32_t)(G * BN * RB);
+  constexpr int NJ = BN / 8;                          // 8-column accumulator blocks
+  // shared memory: [A ring: stages_a x (hi | lo)][B ring: stages_b x (hi G taps | lo G taps)][column sums 8 x 2 x BN][barriers]
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t smem_base = smem_u32(smem_raw);
-  if (smem_base & 1023u) __trap();
-  uint8_t* smem_gen = smem_raw;
-  const uint32_t b_ring = smem_base + (uint32_t)p.stages_a * p.a_stage_bytes;
-  const uint32_t ring_bytes = (uint32_t)p.stages_a * p.a_stage_bytes + (uint32_t)p.stages_b * p.b_tile_bytes;
-  const uint32_t stage_off = ring_bytes;                       // output staging slabs (16 KB per 32 channels)
-  const uint32_t bars = smem_base + ring_bytes + p.staging_bytes;
-  // barriers: a_full[8] a_empty[8] b_full[16] b_empty[16] tmem_full[2] tmem_empty[2]
-  const uint32_t bar_afull = bars, bar_aempty = bars + 64, bar_bfull = bars + 128, bar_bempty = bars + 256, bar_tfull = bars + 384,
-                 bar_tempty = bars + 400;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem_gen + ring_bytes + p.staging_bytes + 416);
-
-  const long long t_start = clock64();
-  const int warp = uniform_warp_idx(), lane = threadIdx.x % 32;
-  long long* dbg = p.dbg ? p.dbg + (long long)blockIdx.x * 16 : nullptr;
-  const bool timed = dbg != nullptr;
+  const uint32_t base = smem_u32(smem_raw);
+  if (base & 1023u) __trap();
+  const uint32_t b_ring = base + (uint32_t)p.stages_a * p.a_stage_bytes;
+  const uint32_t sums_off = (uint32_t)p.stages_a * p.a_stage_bytes + (uint32_t)p.stages_b * p.b_stage_bytes;
+  float* part = reinterpret_cast<float*>(smem_raw + sums_off);
+  const uint32_t bars = base + sums_off + 8u * 2u * BN * 4u;
+  const uint32_t bar_afull = bars, bar_aempty = bars + 64, bar_bfull = bars + 128, bar_bempty = bars + 192;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < p.stages_a; ++s) { mbar_init(bar_afull + 8 * s, 1); mbar_init(bar_aempty + 8 * s, 1); }
-    for (int s = 0; s < p.stages_b; ++s) { mbar_init(bar_bfull + 8 * s, 1); mbar_init(bar_bempty + 8 * s, 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(bar_tfull + 8 * s, 1); mbar_init(bar_tempty + 8 * s, 4 * EP_GROUPS); }
+    for (int s = 0; s < p.stages_a; ++s) { mbar_init(bar_afull + 8 * s, 1); mbar_init(bar_aempty + 8 * s, 8); }
+    for (int s = 0; s < p.stages_b; ++s) { mbar_init(bar_bfull + 8 * s, 1); mbar_init(bar_bempty + 8 * s, 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tm_a_hi) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tm_a_lo) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tm_b) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tm_b_last) : "memory");
-    if (p.tma_store && !p.pair_out) asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tm_y) : "memory");
-    if (p.pair_out) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tm_yh) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tm_yl) : "memory");
-    }
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"((uint32_t)p.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  if (dbg && threadIdx.x == 0) { dbg[0] = t_start; dbg[1] = clock64(); }
-  const int tiles = p.tiles_x * p.tiles_y * p.Dz * p.N;
-  const int n_items = tiles * p.n_chunks;        // item = chunk * tiles + tile: consecutive CTAs work on neighbouring tiles
-  const int groups_per_chunk = p.n_tap / G;      // G divides n_tap (host)
-  const int steps_per_item = p.n_kz * p.cin_chunks * groups_per_chunk;
 
-  if (warp == 0) {
-    // ===== TMA producer: runs ahead of the issuer by the ring depths, across item boundaries =====
-    int sa = 0, sb = 0;
-    uint32_t pha = 0, phb = 0;
-    long long w_a = 0, w_b = 0;
-    int n_a = 0, n_b = 0;
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      const int chunk = item / tiles;
-      int t = item - chunk * tiles;
-      const int tx = t % p.tiles_x; t /= p.tiles_x;
-      const int ty = t % p.tiles_y; t /= p.tiles_y;
-      const int z0 = t % p.Dz, n0 = t / p.Dz;
-      const int ox0 = tx * TW, oy0 = ty * TH * p.msub;
-      const bool last_chunk = chunk == p.n_chunks - 1;
-      const CUtensorMap* tmb = last_chunk ? &tm_b_last : &tm_b;
-      const uint32_t b_tx_bytes = (uint32_t)(2 * (last_chunk ? p.BN_last : p.BN) * p.row_bytes);
-      const int cbase = chunk * p.BN;
+  int t = blockIdx.x;
+  const int tx = t % p.tiles_x; t /= p.tiles_x;
+  const int ty = t % p.tiles_y; t /= p.tiles_y;
+  const int z0 = t % p.Dz, n0 = t / p.Dz;
+  const int ox0 = tx * TW, oy0 = ty * TH;
+  const int cbase = p.c_first + (int)blockIdx.y * BN;
+  const int n_steps = p.n_kz * p.cin_chunks * (p.n_tap / G);
+
+  if (warp == 8) {
+    // ===== TMA producer =====
+    if (lane == 0) {
+      int sa = 0, sb = 0;
+      uint32_t pha = 0, phb = 0;
       for (int kz = 0; kz < p.n_kz; ++kz) {
         const int cz = z0 + p.dz[kz];
         for (int cc = 0; cc < p.cin_chunks; ++cc) {
@@ -250,328 +150,354 @@ conv_h2_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
             if (!p.halo || tap == 0) {
               const int cx = ox0 * p.in_stride + (p.halo ? p.org_x : (int)p.dx[tap]);
               const int cy = oy0 * p.in_stride + (p.halo ? p.org_y : (int)p.dy[tap]);
-              mbar_wait_t(bar_aempty + 8 * sa, pha ^ 1u, timed, w_a);
-              if ((p.dev_flags & 512) && n_a >= p.stages_a) {          // development: no activation traffic after the first ring fill
-                if (elect_one()) mbar_arrive(bar_afull + 8 * sa);
-              } else {
-                mbar_expect_tx(bar_afull + 8 * sa, p.a_tx_bytes);
-                const uint32_t dst = smem_base + (uint32_t)sa * p.a_stage_bytes;
-                tma_load_5d(dst, &tm_a_hi, bar_afull + 8 * sa, cc * p.bkc, cx, cy, cz, n0);
-                tma_load_5d(dst + p.a_tile_bytes, &tm_a_lo, bar_afull + 8 * sa, cc * p.bkc, cx, cy, cz, n0);
-              }
-              ++n_a;
+              mbar_wait(bar_aempty + 8 * sa, pha ^ 1u);
+              mbar_expect_tx(bar_afull + 8 * sa, p.a_tx_bytes);
+              const uint32_t dst = base + (uint32_t)sa * p.a_stage_bytes;
+              tma_load_5d(dst, &tm_a_hi, bar_afull + 8 * sa, cc * BKC, cx, cy, cz, n0);
+              tma_load_5d(dst + p.a_tile_bytes, &tm_a_lo, bar_afull + 8 * sa, cc * BKC, cx, cy, cz, n0);
               if (++sa == p.stages_a) { sa = 0; pha ^= 1u; }
             }
-            mbar_wait_t(bar_bempty + 8 * sb, phb ^ 1u, timed, w_b);
-            if ((p.dev_flags & 256) && n_b >= p.stages_b) {            // development: no weight traffic after the first ring fill
-              if (elect_one()) mbar_arrive(bar_bfull + 8 * sb);
-            } else {
-              // G consecutive weight slices (taps) in one box: [bkc][BN][hi | lo][G]
-              mbar_expect_tx(bar_bfull + 8 * sb, b_tx_bytes * G);
-              tma_load_4d(b_ring + (uint32_t)sb * p.b_tile_bytes, tmb, bar_bfull + 8 * sb, cc * p.bkc, cbase, 0, p.wsel[kz * p.n_tap + tap]);
-            }
-            ++n_b;
+            mbar_wait(bar_bempty + 8 * sb, phb ^ 1u);
+            mbar_expect_tx(bar_bfull + 8 * sb, 2 * B_HALF);
+            const uint32_t dst = b_ring + (uint32_t)sb * p.b_stage_bytes;
+            const int ws = p.wsel[kz * p.n_tap + tap];
+            tma_load_3d(dst, &tm_b_hi, bar_bfull + 8 * sb, cc * BKC, cbase, ws);
+            tma_load_3d(dst + B_HALF, &tm_b_lo, bar_bfull + 8 * sb, cc * BKC, cbase, ws);
             if (++sb == p.stages_b) { sb = 0; phb ^= 1u; }
           }
         }
       }
     }
-    if (dbg && lane == 0) { dbg[8] = clock64(); dbg[9] = w_a; dbg[10] = w_b; }
-  } else if (warp == 1) {
-    // ===== MMA issuer (software-pipelined: the barrier waits of step s+1 run before the last MMA of step s is issued,
-    // while the tensor pipe still holds queued work - tcgen05.mma issue blocks at the tensor rate, so whatever this
-    // thread does between two steps is otherwise tensor idle time) =====
-    int sa = 0, sb = 0, sa_cur = 0;
-    uint32_t pha = 0, phb = 0;
-    int acc = 0; uint32_t acc_ph = 0;
-    long long w_a = 0, w_b = 0, w_t = 0, t_loop = 0;
-    uint32_t a_hw, b_hw;                            // descriptor high words, pinned in registers
-    asm volatile("mov.b32 %0, %1;" : "=r"(a_hw) : "r"(p.a_desc_hi));
-    asm volatile("mov.b32 %0, %1;" : "=r"(b_hw) : "r"(p.b_desc_hi));
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      const int chunk = item / tiles;
-      const int BN = chunk == p.n_chunks - 1 ? p.BN_last : p.BN;
-      // instruction descriptor (kind::f16): D fp32 [4,6)=1, A / B fp16 = 0, both K-major, N>>3 [17,23), M>>4 [24,29)
-      const uint32_t idesc_w = (1u << 4) | ((uint32_t)((2 * BN) >> 3) << 17) | ((128u >> 4) << 24);
-      const uint32_t idesc_n = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((128u >> 4) << 24);
-      const uint32_t d_main = tmem_base + (uint32_t)(acc * p.acc_stride), d_cross = d_main + (uint32_t)BN;
-      // (every MSUB sub-tile is issued, also those of a bottom-edge item that hold no output row: TMA zero-filled their
-      // operands and the epilogue skips them - straight-line issue code matters more than those few MMAs)
-      mbar_wait_t(bar_tempty + 8 * acc, acc_ph ^ 1u, timed, w_t);       // the epilogue has drained this accumulator set
-      // barriers of the first step
-      mbar_wait_t(bar_afull + 8 * sa, pha, timed, w_a);
+    return;
+  }
+
+  // ===== consumers: warpgroup cw owns tile rows [8 cw, 8 cw + 8) =====
+  const int cw = warp >> 2;
+  float acc_m[BN / 2], acc_c[BN / 2];
+#pragma unroll
+  for (int k = 0; k < BN / 2; ++k) { acc_m[k] = 0.f; acc_c[k] = 0.f; }
+  const uint32_t wg_off = (uint32_t)cw * p.wg_row16 * 16u;
+  int sa = 0, sb = 0, sa_cur = 0, tap = 0;
+  uint32_t pha = 0, phb = 0;
+  int rel_a = -1, rel_b = -1;                         // slots of the previous step, released once it has retired
+  for (int step = 0; step < n_steps; ++step) {
+    const bool new_a = !p.halo || tap == 0;
+    if (new_a) {
+      mbar_wait(bar_afull + 8 * sa, pha);
       sa_cur = sa;
       if (++sa == p.stages_a) { sa = 0; pha ^= 1u; }
-      mbar_wait_t(bar_bfull + 8 * sb, phb, timed, w_b);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const long long tl0 = timed ? clock64() : 0;
-      int tap = 0;
-      const uint32_t bt16 = (uint32_t)(2 * BN * p.row_bytes) >> 4, sub16 = p.a_sub16, dsub = (uint32_t)(2 * BN);     // one tap's [hi | lo] weight tile
-      for (int step = 0; step < steps_per_item; ++step) {
-        const uint32_t a_addr = smem_base + (uint32_t)sa_cur * p.a_stage_bytes;
-        const uint32_t la_hi = desc_lo(a_addr), la_lo = desc_lo(a_addr + p.a_tile_bytes);
-        const uint32_t lb = desc_lo(b_ring + (uint32_t)sb * p.b_tile_bytes);
-        const uint32_t bar_be = bar_bempty + 8 * sb, bar_ae = bar_aempty + 8 * sa_cur;
-        const bool last_of_a = !p.halo || tap + G == p.n_tap;
-        const uint32_t acc0 = step > 0 ? 1u : 0u;
-        uint32_t off[G];
-#pragma unroll
-        for (int g = 0; g < G; ++g) off[g] = p.halo ? (uint32_t)p.a_off16[tap + g] : 0u;
-        if (elect_one()) {
-          // all wide MMAs (a_hi x [b_hi | b_lo] -> main | cross) of the step, then all narrow ones (a_lo x b_hi -> cross);
-          // the very last MMA is held back until the next step's operands have been waited for
-#pragma unroll
-          for (int g = 0; g < G; ++g) {
-#pragma unroll
-            for (int sub = 0; sub < MSUB; ++sub) {
-              const uint32_t ao = la_hi + off[g] + (uint32_t)sub * sub16, bo = lb + (uint32_t)g * bt16, dm = d_main + (uint32_t)sub * dsub;
-              if (g == 0) umma_f16_first(dm, ao, a_hw, bo, b_hw, idesc_w, acc0);
-              else umma_f16_acc(dm, ao, a_hw, bo, b_hw, idesc_w);
-#pragma unroll
-              for (int ks = 1; ks < NKS; ++ks) umma_f16_acc(dm, ao + 2 * ks, a_hw, bo + 2 * ks, b_hw, idesc_w);
-            }
-          }
-          if (!(p.dev_flags & 1024)) {
-#pragma unroll
-            for (int g = 0; g < G; ++g) {
-#pragma unroll
-              for (int sub = 0; sub < MSUB; ++sub) {
-                const uint32_t ao = la_lo + off[g] + (uint32_t)sub * sub16, bo = lb + (uint32_t)g * bt16, dc = d_cross + (uint32_t)sub * dsub;
-#pragma unroll
-                for (int ks = 0; ks < NKS; ++ks)
-                  if (!(g == G - 1 && sub == MSUB - 1 && ks == NKS - 1)) umma_f16_acc(dc, ao + 2 * ks, a_hw, bo + 2 * ks, b_hw, idesc_n);
-              }
-            }
-          }
-        }
-        __syncwarp();
-        // advance to the next step and wait for its operands while the MMAs above execute
-        if (++sb == p.stages_b) { sb = 0; phb ^= 1u; }
-        tap += G; if (tap == p.n_tap) tap = 0;
-        if (step + 1 < steps_per_item) {
-          if (!p.halo || tap == 0) {
-            mbar_wait_t(bar_afull + 8 * sa, pha, timed, w_a);
-            sa_cur = sa;
-            if (++sa == p.stages_a) { sa = 0; pha ^= 1u; }
-          }
-          mbar_wait_t(bar_bfull + 8 * sb, phb, timed, w_b);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        }
-        if (elect_one()) {
-          umma_f16_acc(d_cross + (uint32_t)(MSUB - 1) * dsub, la_lo + off[G - 1] + (uint32_t)(MSUB - 1) * sub16 + 2 * (NKS - 1), a_hw,
-                       lb + (uint32_t)(G - 1) * bt16 + 2 * (NKS - 1), b_hw, idesc_n);
-          umma_commit_raw(bar_be);                   // weight tiles of this step consumed
-          if (last_of_a) umma_commit_raw(bar_ae);    // activation (halo) tile consumed
-        }
-        __syncwarp();
-      }
-      umma_commit(bar_tfull + 8 * acc);              // accumulators of this item complete -> epilogue
-      if (timed) t_loop += clock64() - tl0;
-      if (++acc == 2) { acc = 0; acc_ph ^= 1u; }
     }
-    if (dbg && lane == 0) { dbg[3] = clock64(); dbg[11] = w_a; dbg[12] = w_b; dbg[13] = w_t; dbg[14] = t_loop; }
-  } else {
-    // ===== epilogue: two independent groups of four warps. The work of an item is cut into units = (sub-tile, 32-channel
-    // slab); group g takes units g, g + 2, ... through its OWN 16 KB staging slab (TMA store + BatchNorm column sums), so
-    // the groups never wait for each other and a 32-channel layer (one slab per sub-tile) still keeps both busy =====
-    const int cg = warp >= 6 ? 1 : 0;
-    const int q = warp & 3;                       // TMEM lane quarter this warp may access
-    const int r = q * 32 + lane;                  // GEMM row = TMEM lane = pixel within the tile
-    const int py0 = r / TW, px = r % TW;
-    uint8_t* ep = smem_gen + stage_off + cg * 16384;
-    const uint32_t ep_addr = smem_base + stage_off + (uint32_t)(cg * 16384);
-    const bool tma_out = p.tma_store != 0 && !(p.dev_flags & 32);
-    const bool want_stats = p.stats && !(p.dev_flags & 16);
-    const uint32_t lane_base = tmem_base + ((uint32_t)(q * 32) << 16);
-    const bool storer = tma_out && q == 0 && lane == 0;            // one thread per group
-    int acc = 0; uint32_t acc_ph = 0;
-    long long w_t = 0, t_ep = 0;
-    // BatchNorm sums: every thread owns one (column, 32-row segment) of its group's slab and accumulates it in registers over
-    // all the units it sees (two register sets: a group alternates between at most two slabs); global atomics only when the
-    // column changes and at the end - per-tile atomics had the 32-channel layers queueing on 64 hot L2 addresses
-    double sa1 = 0.0, sa2 = 0.0, sb1 = 0.0, sb2 = 0.0;
-    int sa_col = -1, sb_col = -1;
-    const int e_g = q * 32 + lane;
-    const int s_col = e_g & 31, s_seg = e_g >> 5;
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      const int chunk = item / tiles;
-      int t = item - chunk * tiles;
-      const int tx = t % p.tiles_x; t /= p.tiles_x;
-      const int ty = t % p.tiles_y; t /= p.tiles_y;
-      const int z0 = t % p.Dz, n0 = t / p.Dz;
-      const int ox0 = tx * TW, oy00 = ty * TH * p.msub;
-      const int BN = chunk == p.n_chunks - 1 ? p.BN_last : p.BN;
-      const int cbase = chunk * p.BN;
-      const int n_here = min(BN, p.Cout - cbase);   // logical channels of this item
-      const int rows_left = p.Hy - oy00;
-      const int nsub = rows_left >= TH * p.msub ? p.msub : (rows_left + TH - 1) / TH;
-      const int n_slabs = (BN + 31) >> 5;
-      const int n_units = nsub * n_slabs;
-      const bool vec_ok = ((p.Cs_out | (p.c_off + cbase)) & 3) == 0;
-      mbar_wait_t(bar_tfull + 8 * acc, acc_ph, timed && threadIdx.x == 64, w_t);
-      const long long te0 = (timed && threadIdx.x == 64) ? clock64() : 0;
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      int k = 0;
-      for (int u = cg; u < n_units; u += EP_GROUPS, ++k) {
-        const int sub = u / n_slabs, sl = u - sub * n_slabs;
-        const int oy0 = oy00 + sub * TH;
-        const int iy = oy0 + py0, ix = ox0 + px;
-        const bool valid = iy < p.Hy && ix < p.Wx;
-        const int oy = iy * p.out_stride + p.out_off_y, ox = ix * p.out_stride + p.out_off_x;
-        float* dst = p.y + ((((long long)n0 * p.Dout + z0) * p.Hout + oy) * p.Wout + ox) * (long long)p.Cs_out + p.c_off + cbase;
-        // the group's staging slab is free again once its previous TMA store has read it and its column sums are done
-        if (storer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-        if (cg == 0) asm volatile("bar.sync 1, 128;" ::: "memory"); else asm volatile("bar.sync 2, 128;" ::: "memory");
-        const uint32_t acc_base = lane_base + (uint32_t)(acc * p.acc_stride + sub * 2 * BN);
+    mbar_wait(bar_bfull + 8 * sb, phb);
+    const uint32_t a_hi = base + (uint32_t)sa_cur * p.a_stage_bytes + wg_off;
+    const uint32_t b_hi = b_ring + (uint32_t)sb * p.b_stage_bytes;
+    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          const int c0 = sl * 32 + half * 16;
-          if (c0 >= BN && p.pair_out) {
-            // pair output: the store covers the whole 32-channel slab (pad channels of the operand pair must be zero)
-            const uint4 z = make_uint4(0u, 0u, 0u, 0u);
-            uint8_t* rowh = ep + r * 64;
-            const int sw = (r >> 1) & 3;
-            *reinterpret_cast<uint4*>(rowh + (((half * 2) ^ sw) << 4)) = z;
-            *reinterpret_cast<uint4*>(rowh + (((half * 2 + 1) ^ sw) << 4)) = z;
-            *reinterpret_cast<uint4*>(rowh + 8192 + (((half * 2) ^ sw) << 4)) = z;
-            *reinterpret_cast<uint4*>(rowh + 8192 + (((half * 2 + 1) ^ sw) << 4)) = z;
-          }
-          if (c0 < BN) {
-            uint32_t vm[16], vc[16];
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                : "=r"(vm[0]), "=r"(vm[1]), "=r"(vm[2]), "=r"(vm[3]), "=r"(vm[4]), "=r"(vm[5]), "=r"(vm[6]), "=r"(vm[7]), "=r"(vm[8]),
-                  "=r"(vm[9]), "=r"(vm[10]), "=r"(vm[11]), "=r"(vm[12]), "=r"(vm[13]), "=r"(vm[14]), "=r"(vm[15])
-                : "r"(acc_base + (uint32_t)c0) : "memory");
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                : "=r"(vc[0]), "=r"(vc[1]), "=r"(vc[2]), "=r"(vc[3]), "=r"(vc[4]), "=r"(vc[5]), "=r"(vc[6]), "=r"(vc[7]), "=r"(vc[8]),
-                  "=r"(vc[9]), "=r"(vc[10]), "=r"(vc[11]), "=r"(vc[12]), "=r"(vc[13]), "=r"(vc[14]), "=r"(vc[15])
-                : "r"(acc_base + (uint32_t)(BN + c0)) : "memory");
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            float f[16];
+    for (int g = 0; g < G; ++g) {
+      const uint32_t ao = a_hi + (p.halo ? (uint32_t)p.a_off16[tap + g] * 16u : 0u);
 #pragma unroll
-            for (int j = 0; j < 16; ++j) f[j] = fmaf(__uint_as_float(vc[j]), LO_INV, __uint_as_float(vm[j]));
-            if (p.bias) {
+      for (int ks = 0; ks < KS; ++ks) {
+        const uint32_t ah = ao + 32u * ks, al = ah + p.a_tile_bytes;
+        const uint32_t bh = b_hi + (uint32_t)(g * BN * RB) + 32u * ks, bl = bh + B_HALF;
+        wg_mma<BN, TF32>(acc_m, wg_desc(ah, p.a_desc_hi), wg_desc(bh, p.b_desc_hi));
+        wg_mma<BN, TF32>(acc_c, wg_desc(ah, p.a_desc_hi), wg_desc(bl, p.b_desc_hi));
+        wg_mma<BN, TF32>(acc_c, wg_desc(al, p.a_desc_hi), wg_desc(bh, p.b_desc_hi));
+      }
+    }
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+    asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+    if (lane == 0) {
+      if (rel_b >= 0) mbar_arrive(bar_bempty + 8 * rel_b);
+      if (rel_a >= 0) mbar_arrive(bar_aempty + 8 * rel_a);
+    }
+    tap += G;
+    const bool last_of_a = !p.halo || tap == p.n_tap;
+    if (tap == p.n_tap) tap = 0;
+    rel_b = sb; rel_a = last_of_a ? sa_cur : -1;
+    if (++sb == p.stages_b) { sb = 0; phb ^= 1u; }
+  }
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+  // (the producer issues no further loads: the last slots need no release)
+
+  // ===== epilogue from the accumulator registers =====
+  const int w4 = warp & 3;
+  const int n_here = min(BN, p.Cout - cbase);
+  const bool pair = p.y_hi != nullptr;
+  const bool vec2 = ((p.Cs_out | (p.c_off + cbase)) & 1) == 0;
+  float* dst_row[2] = {nullptr, nullptr};
+  long long pix[2] = {0, 0};
+  bool valid[2];
 #pragma unroll
-              for (int j = 0; j < 16; ++j) if (c0 + j < n_here) f[j] += __ldg(p.bias + cbase + c0 + j);
-            }
-            if (p.leaky) {
+  for (int i = 0; i < 2; ++i) {
+    const int r = 16 * w4 + (lane >> 2) + 8 * i;      // GEMM row within the warpgroup
+    const int iy = oy0 + 8 * cw + (r >> 3), ix = ox0 + (r & 7);
+    valid[i] = iy < p.Hy && ix < p.Wx;
+    const int oy = iy * p.out_stride + p.out_off_y, ox = ix * p.out_stride + p.out_off_x;
+    pix[i] = (((long long)n0 * p.Dout + z0) * p.Hout + oy) * p.Wout + ox;
+    if (!pair) dst_row[i] = p.y + pix[i] * (long long)p.Cs_out + p.c_off + cbase;
+  }
+  constexpr int NJ_PAIR = ((BN + 31) / 32) * 4;       // pair output: pad channels up to the next 32 are stored as zeros
+  const int nj_store = pair ? NJ_PAIR : NJ;
 #pragma unroll
-              for (int j = 0; j < 16; ++j) f[j] = f[j] >= 0.f ? f[j] : f[j] * 0.01f;
-            }
-            if (!valid) {
+  for (int j = 0; j < NJ_PAIR; ++j) {
+    if (j >= nj_store) break;
+    const int c = 8 * j + 2 * (lane & 3);
+    float v[2][2];
 #pragma unroll
-              for (int j = 0; j < 16; ++j) f[j] = 0.f;
-            } else if (c0 + 16 > n_here) {
+    for (int i = 0; i < 2; ++i)
 #pragma unroll
-              for (int j = 0; j < 16; ++j) if (c0 + j >= n_here) f[j] = 0.f;
-            }
-            if (p.pair_out) {
-              // two 64-byte-row half tiles [hi 8 KB | lo 8 KB] in the group's slab, 64-byte swizzle (chunk ^= row / 2 mod 4)
-              uint32_t hw[8], lw[8];
-#pragma unroll
-              for (int j = 0; j < 16; j += 2) {
-                __half h0, l0, h1, l1;
-                nrgbd_split_pair(f[j], h0, l0); nrgbd_split_pair(f[j + 1], h1, l1);
-                hw[j >> 1] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
-                lw[j >> 1] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
-              }
-              uint8_t* rowh = ep + r * 64;
-              const int sw = (r >> 1) & 3;
-              *reinterpret_cast<uint4*>(rowh + (((half * 2) ^ sw) << 4)) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-              *reinterpret_cast<uint4*>(rowh + (((half * 2 + 1) ^ sw) << 4)) = make_uint4(hw[4], hw[5], hw[6], hw[7]);
-              *reinterpret_cast<uint4*>(rowh + 8192 + (((half * 2) ^ sw) << 4)) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-              *reinterpret_cast<uint4*>(rowh + 8192 + (((half * 2 + 1) ^ sw) << 4)) = make_uint4(lw[4], lw[5], lw[6], lw[7]);
-            } else if (tma_out || want_stats) {
-              uint8_t* rowp = ep + r * 128;
-              const int j0 = half * 4;
-#pragma unroll
-              for (int jj = 0; jj < 4; ++jj)
-                *reinterpret_cast<float4*>(rowp + (((j0 + jj) ^ (r & 7)) << 4)) = make_float4(f[4 * jj], f[4 * jj + 1], f[4 * jj + 2], f[4 * jj + 3]);
-            }
-            if (valid && !tma_out && !p.pair_out && !(p.dev_flags & 32)) {
-              if (vec_ok && c0 + 16 <= n_here) {
-#pragma unroll
-                for (int j = 0; j < 16; j += 4) *reinterpret_cast<float4*>(dst + c0 + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-              } else {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) if (c0 + j < n_here) dst[c0 + j] = f[j];
-              }
-            }
-          }
+      for (int e = 0; e < 2; ++e) {
+        float f = 0.f;
+        if (j < NJ && c + e < n_here && valid[i]) {
+          f = fmaf(acc_c[4 * j + 2 * i + e], SCALE, acc_m[4 * j + 2 * i + e]);
+          if (p.bias) f += __ldg(p.bias + cbase + c + e);
+          if (p.leaky) f = f >= 0.f ? f : f * 0.01f;
         }
-        if (tma_out || want_stats) {
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // staged slab -> visible to the TMA engine
-          if (cg == 0) asm volatile("bar.sync 1, 128;" ::: "memory"); else asm volatile("bar.sync 2, 128;" ::: "memory");
-        }
-        if (storer && p.pair_out) {
-          asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
-                       ::"l"((uint64_t)&tm_yh), "r"(ep_addr), "r"(p.c_off + cbase + sl * 32), "r"(ox0), "r"(oy0), "r"(z0), "r"(n0)
-                       : "memory");
-          asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
-                       ::"l"((uint64_t)&tm_yl), "r"(ep_addr + 8192u), "r"(p.c_off + cbase + sl * 32), "r"(ox0), "r"(oy0), "r"(z0), "r"(n0)
-                       : "memory");
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        } else if (storer && sl * 32 < n_here) {
-          asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
-                       ::"l"((uint64_t)&tm_y), "r"(ep_addr), "r"(p.c_off + cbase + sl * 32), "r"(ox0), "r"(oy0), "r"(z0), "r"(n0)
-                       : "memory");
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
-        if (want_stats) {
-          const int co = sl * 32 + s_col;              // this thread's column of the slab, rows [32 s_seg, +32)
-          if (co < n_here) {
-            const uint8_t* colp = ep + (s_col & 3) * 4;
-            const int jc = s_col >> 2;
-            float s1 = 0.f, s2 = 0.f, t1 = 0.f, t2 = 0.f;
-#pragma unroll 4
-            for (int rr = s_seg * 32; rr < s_seg * 32 + 32; rr += 2) {
-              const float x0 = *reinterpret_cast<const float*>(colp + rr * 128 + ((jc ^ (rr & 7)) << 4));
-              const float x1 = *reinterpret_cast<const float*>(colp + (rr + 1) * 128 + ((jc ^ ((rr + 1) & 7)) << 4));
-              s1 += x0; s2 = fmaf(x0, x0, s2);
-              t1 += x1; t2 = fmaf(x1, x1, t2);
-            }
-            const int col = cbase + co;
-            if ((k & 1) == 0) {
-              if (sa_col != col) {                       // another column: flush the previous one's sums
-                if (sa_col >= 0) { atomicAdd(p.stats + sa_col, sa1); atomicAdd(p.stats + p.Cout + sa_col, sa2); }
-                sa_col = col; sa1 = 0.0; sa2 = 0.0;
-              }
-              sa1 += (double)(s1 + t1); sa2 += (double)(s2 + t2);
-            } else {
-              if (sb_col != col) {
-                if (sb_col >= 0) { atomicAdd(p.stats + sb_col, sb1); atomicAdd(p.stats + p.Cout + sb_col, sb2); }
-                sb_col = col; sb1 = 0.0; sb2 = 0.0;
-              }
-              sb1 += (double)(s1 + t1); sb2 += (double)(s2 + t2);
-            }
-          }
+        v[i][e] = f;
+      }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      if (!valid[i]) continue;
+      if (pair) {
+        __half h0, l0, h1, l1;
+        nrgbd_split_pair(v[i][0], h0, l0); nrgbd_split_pair(v[i][1], h1, l1);
+        const long long o = pix[i] * (long long)p.Cs_out + cbase + c;
+        *reinterpret_cast<__half2*>(p.y_hi + o) = __halves2half2(h0, h1);
+        *reinterpret_cast<__half2*>(p.y_lo + o) = __halves2half2(l0, l1);
+      } else if (vec2 && c + 1 < n_here) {
+        *reinterpret_cast<float2*>(dst_row[i] + c) = make_float2(v[i][0], v[i][1]);
+      } else {
+        if (c < n_here) dst_row[i][c] = v[i][0];
+        if (c + 1 < n_here) dst_row[i][c + 1] = v[i][1];
+      }
+    }
+    if (p.stats && j < NJ) {
+      // column sums over this warp's 16 rows: the thread's two rows, then across the 8 lane quads
+      float s1[2], s2[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        s1[e] = v[0][e] + v[1][e];
+        s2[e] = fmaf(v[0][e], v[0][e], v[1][e] * v[1][e]);
+#pragma unroll
+        for (int m = 4; m < 32; m <<= 1) {
+          s1[e] += __shfl_xor_sync(0xffffffffu, s1[e], m);
+          s2[e] += __shfl_xor_sync(0xffffffffu, s2[e], m);
         }
       }
-      // every tcgen05.ld of this warp has completed (wait::ld above): hand the accumulator set back to the issuer
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_tempty + 8 * acc);
-      if (timed && threadIdx.x == 64) t_ep += clock64() - te0;
-      if (++acc == 2) { acc = 0; acc_ph ^= 1u; }
+      if (lane < 4) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) { part[(warp * 2) * BN + c + e] = s1[e]; part[(warp * 2 + 1) * BN + c + e] = s2[e]; }
+      }
     }
-    if (sa_col >= 0) { atomicAdd(p.stats + sa_col, sa1); atomicAdd(p.stats + p.Cout + sa_col, sa2); }
-    if (sb_col >= 0) { atomicAdd(p.stats + sb_col, sb1); atomicAdd(p.stats + p.Cout + sb_col, sb2); }
-    if (storer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // shared memory must outlive the stores' reads
-    if (dbg && threadIdx.x == 64) { dbg[5] = clock64(); dbg[4] = w_t; dbg[15] = t_ep; }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols) : "memory");
-  }
-  if (dbg && threadIdx.x == 32) {
-    unsigned smid; asm("mov.u32 %0, %%smid;" : "=r"(smid));
-    dbg[6] = clock64(); dbg[7] = smid;
+  if (p.stats) {
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    const int c = threadIdx.x;
+    if (c < n_here) {
+      double a1 = 0.0, a2 = 0.0;
+#pragma unroll
+      for (int w = 0; w < 8; ++w) { a1 += (double)part[(w * 2) * BN + c]; a2 += (double)part[(w * 2 + 1) * BN + c]; }
+      atomicAdd(p.stats + cbase + c, a1);
+      atomicAdd(p.stats + p.Cout + cbase + c, a2);
+    }
   }
 }
 
+int g_h2_smem_cap_kb = 0;   // development: cap on the dynamic shared memory per CTA (0 = chosen by the plan below)
+int g_h2_flags = 0;         // development knobs (nrgbd_dev_conv_h2_set_flags), all off in production:
+                            //   4 one box per tap (no halo tile)   128 one tap per pipeline step
+
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+EncodeTiledFn get_encode() {
+  static EncodeTiledFn fn = nullptr;
+  if (!fn) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
+      fn = (EncodeTiledFn)p;
+  }
+  return fn;
+}
+
+// Encoded maps are memoised per thread (the engine's pool hands out the same blocks every frame).
+struct MapKey { const void* p; long long a; int b, c, d, e, f, g, h, i; };
+struct MapEnt { MapKey k; CUtensorMap m; };
+inline bool same_key(const MapKey& x, const MapKey& y) {
+  return x.p == y.p && x.a == y.a && x.b == y.b && x.c == y.c && x.d == y.d && x.e == y.e && x.f == y.f && x.g == y.g && x.h == y.h && x.i == y.i;
+}
+thread_local MapEnt g_maps[1024];
+inline unsigned key_slot(const MapKey& k) {
+  unsigned long long h = (unsigned long long)k.p * 0x9E3779B97F4A7C15ull;
+  h ^= (unsigned long long)(k.a * 73856093ll) ^ (unsigned long long)(k.b * 19349663u) ^ (unsigned long long)(k.c * 83492791u) ^
+       (unsigned long long)(k.d * 2654435761u) ^ (unsigned long long)(k.e * 40503u) ^ (unsigned long long)(k.f * 2246822519u) ^
+       (unsigned long long)(k.g * 3266489917u) ^ (unsigned long long)(k.h * 668265263u) ^ (unsigned long long)(k.i * 374761393u);
+  return (unsigned)(h >> 40) & 1023u;
+}
+
+// 5-D map over a channels-last tensor [N][D][H][W][Cs] of `esize`-byte elements; box [32][box_w (after stride)][box_h]
+int encode_act_map(CUtensorMap* tm, const void* x, int esize, int N, int D, int H, int W, int C, int Cs, int box_w, int box_h, int stride) {
+  MapKey k{x, (long long)N * 8 + esize, D, H, W, C, Cs, box_w, box_h, stride};
+  MapEnt& e = g_maps[key_slot(k)];
+  if (same_key(e.k, k) && e.k.p) { *tm = e.m; return NRGBD_OK; }
+  EncodeTiledFn enc = get_encode();
+  if (!enc) { nrgbd_set_error("cuTensorMapEncodeTiled unavailable"); return NRGBD_ERR_CUDA; }
+  cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)D, (cuuint64_t)N};
+  cuuint64_t strides[4] = {(cuuint64_t)Cs * esize, (cuuint64_t)W * Cs * esize, (cuuint64_t)H * W * Cs * esize, (cuuint64_t)D * H * W * Cs * esize};
+  cuuint32_t box[5] = {(cuuint32_t)BKC, (cuuint32_t)(box_w * stride), (cuuint32_t)(box_h * stride), 1, 1};
+  cuuint32_t estr[5] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1, 1};
+  CUresult r = enc(tm, esize == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, const_cast<void*>(x), dims, strides, box,
+                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, esize == 2 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { nrgbd_set_error("cuTensorMapEncodeTiled(activation, esize %d) failed: %d", esize, (int)r); return NRGBD_ERR_CUDA; }
+  e.k = k; e.m = *tm;
+  return NRGBD_OK;
+}
+
+// 3-D map over one half of the packed weights: [taps (tap_stride elements apart)][Cout_pad][Cin_pad]; box [32][BN][G]
+int encode_w_map(CUtensorMap* tm, const void* w, int esize, long long tap_stride, int taps, int Cout_pad, int Cin_pad, int BN, int G) {
+  MapKey k{w, tap_stride * 8 + esize, taps, Cout_pad, Cin_pad, BN, G, -7, -7, -7};
+  MapEnt& e = g_maps[key_slot(k)];
+  if (same_key(e.k, k) && e.k.p) { *tm = e.m; return NRGBD_OK; }
+  EncodeTiledFn enc = get_encode();
+  if (!enc) { nrgbd_set_error("cuTensorMapEncodeTiled unavailable"); return NRGBD_ERR_CUDA; }
+  cuuint64_t dims[3] = {(cuuint64_t)Cin_pad, (cuuint64_t)Cout_pad, (cuuint64_t)taps};
+  cuuint64_t strides[2] = {(cuuint64_t)Cin_pad * esize, (cuuint64_t)tap_stride * esize};
+  cuuint32_t box[3] = {(cuuint32_t)BKC, (cuuint32_t)BN, (cuuint32_t)G};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = enc(tm, esize == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(w), dims, strides, box,
+                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, esize == 2 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { nrgbd_set_error("cuTensorMapEncodeTiled(weights, esize %d) failed: %d", esize, (int)r); return NRGBD_ERR_CUDA; }
+  e.k = k; e.m = *tm;
+  return NRGBD_OK;
+}
+
+inline uint32_t round_up(uint32_t v, uint32_t m) { return (v + m - 1) / m * m; }
+
+typedef void (*WgKernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const WgParams);
+
+template <bool TF32, int G>
+WgKernel pick_kernel(int BN) {
+  switch (BN) {
+    case 16: return conv_wg_kernel<16, TF32, G>;
+    case 32: return conv_wg_kernel<32, TF32, G>;
+    case 48: return conv_wg_kernel<48, TF32, G>;
+    case 64: return conv_wg_kernel<64, TF32, G>;
+    case 80: return conv_wg_kernel<80, TF32, G>;
+    case 96: return conv_wg_kernel<96, TF32, G>;
+    case 112: return conv_wg_kernel<112, TF32, G>;
+    case 128: return conv_wg_kernel<128, TF32, G>;
+  }
+  return nullptr;
+}
+
+// One launch: output channels [c_first, c_first + n_chunks * BN) in chunks of BN.
+int launch_chunks(const WgConv& c, WgParams p, int BN, int n_chunks, int c_first, cudaStream_t st) {
+  const bool tf32 = c.tf32 != 0;
+  const int esize = tf32 ? 4 : 2, RB = BKC * esize;
+  p.c_first = c_first;
+  // taps per pipeline step: a whole kernel row when the weight slices of the taps are consecutive (plain convolutions)
+  int G = 1;
+  if (p.halo && p.n_tap % 3 == 0 && !(g_h2_flags & 128)) {
+    bool consecutive = true;
+    for (int t = 1; t < p.n_kz * p.n_tap; ++t) consecutive = consecutive && c.wsel[t] == c.wsel[t - 1] + 1;
+    if (consecutive) G = 3;
+  }
+  // shared memory: two CTAs per SM when BN <= 64 and two A + two B stages fit half of the SM's 228 KB
+  const size_t extra = (size_t)8 * 2 * BN * 4 + 256;
+  auto plan = [&](size_t cap, int g, int& sa, int& sb) {
+    const size_t b_stage = (size_t)2 * g * BN * RB;
+    sa = 2;
+    if (cap < extra + 2 * (size_t)p.a_stage_bytes + 2 * b_stage) return false;
+    sb = (int)((cap - extra - 2 * (size_t)p.a_stage_bytes) / b_stage);
+    if (sb > 8) sb = 8;
+    if (sb >= 6 && cap >= extra + 3 * (size_t)p.a_stage_bytes + 4 * b_stage) { sa = 3; sb = (int)((cap - extra - 3 * (size_t)p.a_stage_bytes) / b_stage); if (sb > 8) sb = 8; }
+    return true;
+  };
+  size_t cap = g_h2_smem_cap_kb > 0 ? (size_t)g_h2_smem_cap_kb * 1024 : (BN <= 64 ? 115712 - 1024 : 232448);
+  int sa = 0, sb = 0;
+  bool ok = plan(cap, G, sa, sb);
+  if (!ok && G == 3) { G = 1; ok = plan(cap, G, sa, sb); }
+  if (!ok) { cap = 232448; ok = plan(cap, G, sa, sb); }
+  if (!ok) { nrgbd_set_error("conv_wgmma: tile does not fit the shared-memory pipeline"); return NRGBD_ERR_UNSUPPORTED; }
+  p.stages_a = sa; p.stages_b = sb;
+  p.b_stage_bytes = (uint32_t)(2 * G * BN * RB);
+  const size_t smem = (size_t)sa * p.a_stage_bytes + (size_t)sb * p.b_stage_bytes + extra;
+  CUtensorMap tb_hi, tb_lo;
+  int rc = encode_w_map(&tb_hi, c.w_hi, esize, c.w_tap_stride, c.n_wslices, c.Cout_pad, c.Cin_pad, BN, G);
+  if (rc == NRGBD_OK) rc = encode_w_map(&tb_lo, c.w_lo, esize, c.w_tap_stride, c.n_wslices, c.Cout_pad, c.Cin_pad, BN, G);
+  if (rc != NRGBD_OK) return rc;
+  CUtensorMap ta_hi, ta_lo;
+  rc = encode_act_map(&ta_hi, c.x_hi, esize, c.N, c.Din, c.Hin, c.Win, c.Cin_pad, c.Cs_in, p.box_w, p.box_h, p.in_stride);
+  if (rc == NRGBD_OK) rc = encode_act_map(&ta_lo, c.x_lo, esize, c.N, c.Din, c.Hin, c.Win, c.Cin_pad, c.Cs_in, p.box_w, p.box_h, p.in_stride);
+  if (rc != NRGBD_OK) return rc;
+  WgKernel fn = tf32 ? (G == 3 ? pick_kernel<true, 3>(BN) : pick_kernel<true, 1>(BN)) : (G == 3 ? pick_kernel<false, 3>(BN) : pick_kernel<false, 1>(BN));
+  if (!fn) { nrgbd_set_error("conv_wgmma: unsupported chunk width %d", BN); return NRGBD_ERR_UNSUPPORTED; }
+  static size_t configured[2][2][8] = {};
+  size_t& conf = configured[tf32][G == 3][BN / 16 - 1];
+  if (smem > conf) {
+    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) { nrgbd_set_error("conv_wgmma: cannot opt in to %zu bytes of shared memory: %s", smem, cudaGetErrorString(e)); return NRGBD_ERR_CUDA; }
+    conf = smem;
+  }
+  const long long tiles = (long long)p.N * p.Dz * p.tiles_x * p.tiles_y;
+  fn<<<dim3((unsigned)tiles, (unsigned)n_chunks), WG_THREADS, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, p);
+  return NRGBD_OK;
+}
+
+}  // namespace
+
+int conv_wgmma(const WgConv& c, cudaStream_t st) {
+  NRGBD_REQUIRE(c.n_tap >= 1 && c.n_tap <= WG_MAX_TAP2D && c.n_kz >= 1 && c.n_kz <= 3 && c.Cin_pad % BKC == 0 && c.Cout_pad % 16 == 0,
+                "unsupported convolution shape");
+  const int esize = c.tf32 ? 4 : 2, RB = BKC * esize;
+  WgParams p{};
+  p.y = c.y; p.bias = c.bias; p.stats = c.stats;
+  p.y_hi = reinterpret_cast<__half*>(c.y_hi); p.y_lo = reinterpret_cast<__half*>(c.y_lo);
+  p.N = c.N; p.Dz = c.Din; p.Hy = c.Hy; p.Wx = c.Wx;
+  p.tiles_x = ceil_div(c.Wx, TW); p.tiles_y = ceil_div(c.Hy, TH);
+  p.cin_chunks = c.Cin_pad / BKC; p.n_kz = c.n_kz; p.n_tap = c.n_tap; p.in_stride = c.in_stride;
+  p.Cout = c.Cout; p.Dout = c.Dout; p.Hout = c.Hout; p.Wout = c.Wout; p.Cs_out = c.Cs_out; p.c_off = c.c_off;
+  p.out_stride = c.out_stride; p.out_off_y = c.out_off_y; p.out_off_x = c.out_off_x; p.leaky = c.leaky;
+  for (int a = 0; a < 3; ++a) p.dz[a] = c.dz[a];
+  for (int t = 0; t < WG_MAX_TAP2D; ++t) { p.dy[t] = c.dy[t]; p.dx[t] = c.dx[t]; }
+  for (int t = 0; t < 3 * WG_MAX_TAP2D; ++t) p.wsel[t] = c.wsel[t];
+  // halo: stride-1 filters with more than one in-plane tap
+  p.halo = (c.in_stride == 1 && c.n_tap > 1 && !(g_h2_flags & 4)) ? 1 : 0;
+  int pitch = TW, halo_rows = TH;
+  if (p.halo) {
+    int min_dy = 127, max_dy = -127, min_dx = 127, max_dx = -127;
+    for (int t = 0; t < c.n_tap; ++t) {
+      min_dy = c.dy[t] < min_dy ? c.dy[t] : min_dy; max_dy = c.dy[t] > max_dy ? c.dy[t] : max_dy;
+      min_dx = c.dx[t] < min_dx ? c.dx[t] : min_dx; max_dx = c.dx[t] > max_dx ? c.dx[t] : max_dx;
+    }
+    pitch = TW + (max_dx - min_dx); halo_rows = TH + (max_dy - min_dy);
+    if (pitch > 16 || halo_rows > TH + 16) { p.halo = 0; pitch = TW; halo_rows = TH; }
+    else {
+      p.org_y = min_dy; p.org_x = min_dx;
+      for (int t = 0; t < c.n_tap; ++t) p.a_off16[t] = (unsigned short)((((c.dy[t] - min_dy) * pitch + (c.dx[t] - min_dx)) * RB) >> 4);
+    }
+  }
+  const uint32_t swz_mode = c.tf32 ? 1u : 2u;                    // 128-byte / 64-byte swizzle = one pixel row
+  p.a_desc_hi = (uint32_t)((pitch * RB) >> 4) | (swz_mode << 30);  // SBO = one row of the (halo) tile
+  p.b_desc_hi = (uint32_t)((8 * RB) >> 4) | (swz_mode << 30);
+  p.wg_row16 = (uint32_t)((8 * pitch * RB) >> 4);
+  p.box_w = pitch; p.box_h = halo_rows;
+  p.a_tx_bytes = 2u * (uint32_t)(halo_rows * pitch * RB);
+  p.a_tile_bytes = round_up((uint32_t)(halo_rows * pitch * RB), 1024);
+  p.a_stage_bytes = 2 * p.a_tile_bytes;
+  // Cout in chunks of 128 channels, the last one narrower (320 = 128 + 128 + 64): one launch per chunk width
+  const int n_chunks = (c.Cout_pad + 127) / 128;
+  const int BN = c.Cout_pad < 128 ? c.Cout_pad : 128;
+  const int BN_last = c.Cout_pad - (n_chunks - 1) * BN;
+  const int n_full = BN_last == BN ? n_chunks : n_chunks - 1;
+  int rc = launch_chunks(c, p, BN, n_full, 0, st);
+  if (rc == NRGBD_OK && n_full < n_chunks) rc = launch_chunks(c, p, BN_last, 1, n_full * BN, st);
+  return rc;
+}
+
+namespace {
 // ---- operand preparation -------------------------------------------------------------------------------------------
 __device__ __forceinline__ void split_pair(float a, __half& hi, __half& lo) { nrgbd_split_pair(a, hi, lo); }
 
@@ -609,211 +535,11 @@ __global__ void pack_weight_h2_kernel(const float* __restrict__ w, int kind, int
   out[(long long)t * 2 * tile + tile + (long long)co * Cin_pad + ci] = l;
 }
 
-long long* g_h2_dbg = nullptr;   // development: [grid.y][grid.x][16] clock64 stamps (tools/h2_timeline.py)
-int g_h2_smem_cap_kb = 0;          // development: cap on the dynamic shared memory of conv_h2 (0 = the 227 KB maximum)
-int g_h2_flags = 0;     // development / probe knobs (nrgbd_dev_conv_h2_set_flags), all off in production:
-                        //   1 base-offset field in the A descriptor   2 halo pitch 16   4 one box per tap (no halo)
-                        //   8 64-channel chunks (128-byte rows) when Cin allows   16 skip BN statistics   32 skip stores   64 one sub-tile per item   128 one tap per pipeline step
-                        //   256 / 512 no weight / activation TMA traffic after the first ring fill   1024 skip the narrow MMAs (timing probes: results are wrong)
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
-
-// Encoded maps are memoised per thread (the engine's pool hands out the same blocks every frame).
-struct MapKey { const void* p; int a, b, c, d, e, f, g, h, i; };
-struct MapEnt { MapKey k; CUtensorMap m; };
-inline bool same_key(const MapKey& x, const MapKey& y) {
-  return x.p == y.p && x.a == y.a && x.b == y.b && x.c == y.c && x.d == y.d && x.e == y.e && x.f == y.f && x.g == y.g && x.h == y.h && x.i == y.i;
-}
-thread_local MapEnt g_maps[1024];
-inline unsigned key_slot(const MapKey& k) {
-  unsigned long long h = (unsigned long long)k.p * 0x9E3779B97F4A7C15ull;
-  h ^= (unsigned long long)(k.a * 73856093u) ^ (unsigned long long)(k.b * 19349663u) ^ (unsigned long long)(k.c * 83492791u) ^
-       (unsigned long long)(k.d * 2654435761u) ^ (unsigned long long)(k.e * 40503u) ^ (unsigned long long)(k.f * 2246822519u) ^
-       (unsigned long long)(k.g * 3266489917u) ^ (unsigned long long)(k.h * 668265263u) ^ (unsigned long long)(k.i * 374761393u);
-  return (unsigned)(h >> 40) & 1023u;
-}
-
-// 5-D map over a channels-last tensor [N][D][H][W][Cs] of `esize`-byte elements; box [box_c][box_w (elements after stride)][box_h]
-int encode_cl_map(CUtensorMap* tm, const void* x, int esize, int N, int D, int H, int W, int C, int Cs, int box_c, int box_w, int box_h,
-                  int stride, int swizzle_bytes) {
-  MapKey k{x, N * 2 + (esize == 2), D, H, W, C, Cs, box_c * 1024 + stride, box_w, box_h * 256 + swizzle_bytes / 32};
-  MapEnt& e = g_maps[key_slot(k)];
-  if (same_key(e.k, k) && e.k.p) { *tm = e.m; return NRGBD_OK; }
-  EncodeTiledFn enc = get_encode();
-  if (!enc) { nrgbd_set_error("cuTensorMapEncodeTiled unavailable"); return NRGBD_ERR_CUDA; }
-  cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)D, (cuuint64_t)N};
-  cuuint64_t strides[4] = {(cuuint64_t)Cs * esize, (cuuint64_t)W * Cs * esize, (cuuint64_t)H * W * Cs * esize, (cuuint64_t)D * H * W * Cs * esize};
-  cuuint32_t box[5] = {(cuuint32_t)box_c, (cuuint32_t)(box_w * stride), (cuuint32_t)(box_h * stride), 1, 1};
-  cuuint32_t estr[5] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1, 1};
-  CUtensorMapSwizzle sw = swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_NONE;
-  CUresult r = enc(tm, esize == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, const_cast<void*>(x), dims, strides, box,
-                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { nrgbd_set_error("cuTensorMapEncodeTiled(activation, esize %d) failed: %d", esize, (int)r); return NRGBD_ERR_CUDA; }
-  e.k = k; e.m = *tm;
-  return NRGBD_OK;
-}
-
-// 4-D map over the packed weights [taps][2][Cout_pad][Cin_pad] halves; box [bkc][BN][2][1]
-int encode_w_map(CUtensorMap* tm, const __half* w, int taps, int Cout_pad, int Cin_pad, int bkc, int BN, int swizzle_bytes, int G) {
-  MapKey k{w, taps, Cout_pad, Cin_pad, bkc, BN, swizzle_bytes, G, -7, -7};
-  MapEnt& e = g_maps[key_slot(k)];
-  if (same_key(e.k, k) && e.k.p) { *tm = e.m; return NRGBD_OK; }
-  EncodeTiledFn enc = get_encode();
-  if (!enc) { nrgbd_set_error("cuTensorMapEncodeTiled unavailable"); return NRGBD_ERR_CUDA; }
-  cuuint64_t dims[4] = {(cuuint64_t)Cin_pad, (cuuint64_t)Cout_pad, 2, (cuuint64_t)taps};
-  cuuint64_t strides[3] = {(cuuint64_t)Cin_pad * 2, (cuuint64_t)Cout_pad * Cin_pad * 2, (cuuint64_t)2 * Cout_pad * Cin_pad * 2};
-  cuuint32_t box[4] = {(cuuint32_t)bkc, (cuuint32_t)BN, 2, (cuuint32_t)G};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUtensorMapSwizzle sw = swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(w), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { nrgbd_set_error("cuTensorMapEncodeTiled(weights, f16 pair) failed: %d", (int)r); return NRGBD_ERR_CUDA; }
-  e.k = k; e.m = *tm;
-  return NRGBD_OK;
-}
-
-inline uint32_t round_up(uint32_t v, uint32_t m) { return (v + m - 1) / m * m; }
-
-// kd x kh x kw taps given as tables; halo geometry derived here.
-int launch_h2(const __half* x_hi, const __half* x_lo, int N, int Din, int Hin, int Win, int Cin_pad, int Cs_in, const __half* w, int n_wslices,
-              int Cout_pad, int kh, int kw, int dil, H2Params& p, cudaStream_t st) {
-  p.dev_flags = g_h2_flags; p.dbg = g_h2_dbg;
-  p.bkc = 32;        // (64-channel chunks / 128-byte rows were measured: no gain, and the rings get too shallow)
-  p.row_bytes = 2 * p.bkc;
-  p.cin_chunks = Cin_pad / p.bkc;
-  // sub-tiles per work item: as many as the double-buffered accumulators allow (2 sets x msub x (main | cross) x BN <= 512
-  // TMEM columns); they share every weight tile, which halves / quarters both the weight traffic and the per-step issue overhead
-  p.msub = p.BN <= 32 ? 4 : p.BN <= 64 ? 2 : 1;
-  if (g_h2_flags & 64) p.msub = 1;
-  while (p.msub > 1 && TH * (p.msub / 2) >= p.Hy) p.msub /= 2;      // small maps
-  p.tiles_x = ceil_div(p.Wx, TW); p.tiles_y = ceil_div(p.Hy, TH * p.msub);
-  const int n_chunks = (Cout_pad + p.BN - 1) / p.BN;
-  p.BN_last = Cout_pad - (n_chunks - 1) * p.BN;
-  // halo: stride-1 filters with more than one in-plane tap
-  p.halo = (p.in_stride == 1 && p.n_tap > 1 && !(g_h2_flags & 4)) ? 1 : 0;
-  const int THM = TH * p.msub;
-  int pitch = TW, halo_rows = THM;
-  if (p.halo) {
-    int min_dy = 127, max_dy = -127, min_dx = 127, max_dx = -127;
-    for (int t = 0; t < p.n_tap; ++t) {
-      min_dy = p.dy[t] < min_dy ? p.dy[t] : min_dy; max_dy = p.dy[t] > max_dy ? p.dy[t] : max_dy;
-      min_dx = p.dx[t] < min_dx ? p.dx[t] : min_dx; max_dx = p.dx[t] > max_dx ? p.dx[t] : max_dx;
-    }
-    pitch = TW + (max_dx - min_dx); halo_rows = THM + (max_dy - min_dy);
-    if (g_h2_flags & 2) pitch = 16;
-    if (pitch > 16 || halo_rows > THM + 16) { p.halo = 0; pitch = TW; halo_rows = THM; }
-    else {
-      p.org_y = min_dy; p.org_x = min_dx;
-      for (int t = 0; t < p.n_tap; ++t)
-        p.a_off16[t] = (unsigned short)((((p.dy[t] - min_dy) * pitch + (p.dx[t] - min_dx)) * p.row_bytes) >> 4);
-    }
-  }
-  const int swz = p.row_bytes;                                  // 64-byte or 128-byte swizzle = one pixel row
-  const uint32_t layout = swz == 128 ? 2u : 4u;                 // UMMA LayoutType: SWIZZLE_128B = 2, SWIZZLE_64B = 4
-  p.a_desc_hi = (uint32_t)((pitch * p.row_bytes) >> 4) | (1u << 14) | (layout << 29);      // SBO = one tile row of the (halo) tile
-  p.b_desc_hi = (uint32_t)((8 * p.row_bytes) >> 4) | (1u << 14) | (layout << 29);
-  p.a_sub16 = (uint32_t)((TH * pitch * p.row_bytes) >> 4);          // 16 tile rows further down the (halo) tile
-  p.a_tx_bytes = 2u * (uint32_t)(halo_rows * pitch * p.row_bytes);
-  p.a_tile_bytes = round_up((uint32_t)(halo_rows * pitch * p.row_bytes), 1024);
-  p.a_stage_bytes = 2 * p.a_tile_bytes;
-  // taps per pipeline step: a whole kernel row when the weight slices of the taps are consecutive (plain convolutions)
-  p.gtaps = 1;
-  if (p.halo && p.n_tap % 3 == 0 && !(g_h2_flags & 128)) {
-    bool consecutive = true;
-    for (int t = 1; t < p.n_kz * p.n_tap; ++t) consecutive = consecutive && p.wsel[t] == p.wsel[t - 1] + 1;
-    if (consecutive) p.gtaps = 3;
-  }
-  p.b_tile_bytes = (uint32_t)(2 * p.BN * p.row_bytes * p.gtaps);
-  CUtensorMap ta_hi, ta_lo, tb, tb_last, ty;
-  int rc = encode_cl_map(&ta_hi, x_hi, 2, N, Din, Hin, Win, Cin_pad, Cs_in, p.bkc, pitch, halo_rows, p.in_stride, swz);
-  if (rc == NRGBD_OK) rc = encode_cl_map(&ta_lo, x_lo, 2, N, Din, Hin, Win, Cin_pad, Cs_in, p.bkc, pitch, halo_rows, p.in_stride, swz);
-  if (rc == NRGBD_OK) rc = encode_w_map(&tb, w, n_wslices, Cout_pad, Cin_pad, p.bkc, p.BN, swz, p.gtaps);
-  tb_last = tb;
-  if (rc == NRGBD_OK && p.BN_last != p.BN) rc = encode_w_map(&tb_last, w, n_wslices, Cout_pad, Cin_pad, p.bkc, p.BN_last, swz, p.gtaps);
-  if (rc != NRGBD_OK) return rc;
-  // resource plan: one persistent CTA per SM; two accumulator sets (main | cross each) in TMEM
-  p.n_chunks = n_chunks;
-  p.acc_stride = 2 * p.BN * p.msub;
-  int cols = 32; while (cols < 2 * p.acc_stride) cols <<= 1;
-  p.tmem_cols = cols;
-  p.staging_bytes = 2u * 16384u;            // one 32-channel output slab per epilogue group
-  // shared-memory budget of the CTA. Leaving part of the SM's 228 KB free lets blocks of OTHER kernels (BatchNorm / layout /
-  // sweep passes of another frame in flight) co-reside with the persistent conv CTA and use the issue slots it leaves idle.
-  size_t smem_cap = g_h2_smem_cap_kb > 0 ? (size_t)g_h2_smem_cap_kb * 1024 : 232448;
-  if (2 * (size_t)p.a_stage_bytes + 2 * (size_t)p.b_tile_bytes + 512 + p.staging_bytes > smem_cap) smem_cap = 232448;     // this shape needs the full SM
-  const size_t budget = smem_cap - 512 - p.staging_bytes;
-  int stages_a = p.msub > 1 ? 2 : 3;
-  if ((size_t)stages_a * p.a_stage_bytes + 3 * (size_t)p.b_tile_bytes > budget) stages_a = 2;
-  int stages_b = (int)((budget - (size_t)stages_a * p.a_stage_bytes) / p.b_tile_bytes);
-  if (stages_b > 16) stages_b = 16;
-  if (stages_b < 2) { nrgbd_set_error("conv_h2: tile does not fit the shared-memory pipeline"); return NRGBD_ERR_UNSUPPORTED; }
-  p.stages_a = stages_a; p.stages_b = stages_b;
-  const size_t ring = (size_t)stages_a * p.a_stage_bytes + (size_t)stages_b * p.b_tile_bytes;
-  const size_t smem = ring + p.staging_bytes + 512;
-  ty = ta_hi;
-  p.tma_store = 0;
-  if (!p.pair_out && p.out_stride == 1 && p.out_off_y == 0 && p.out_off_x == 0 && p.Cs_out % 4 == 0 && p.c_off % 4 == 0 &&
-      ((uintptr_t)p.y & 15) == 0 && !(g_h2_flags & 2048)) {
-    rc = encode_cl_map(&ty, p.y, 4, N, p.Dout, p.Hout, p.Wout, p.c_off + p.Cout, p.Cs_out, 32, TW, TH, 1, 128);
-    if (rc != NRGBD_OK) return rc;
-    p.tma_store = 1;
-  }
-  CUtensorMap tyh = ta_hi, tyl = ta_hi;
-  if (p.pair_out) {
-    // the output as the operand pair of the next convolution: two half tensors with the fp32 tensor's layout, all Cs_out
-    // channels stored (pad channels as zeros), 64-byte swizzled staging
-    if (!(p.out_stride == 1 && p.out_off_y == 0 && p.out_off_x == 0 && p.Cs_out % 32 == 0 && p.c_off == 0 && p.stats == nullptr &&
-          (((uintptr_t)p.y_hi | (uintptr_t)p.y_lo) & 15) == 0 && p.y_hi && p.y_lo)) {
-      nrgbd_set_error("conv_h2: pair output needs a dense stride-1 output with Cs_out % 32 == 0, c_off == 0 and no statistics");
-      return NRGBD_ERR_UNSUPPORTED;
-    }
-    rc = encode_cl_map(&tyh, p.y_hi, 2, N, p.Dout, p.Hout, p.Wout, p.Cs_out, p.Cs_out, 32, TW, TH, 1, 64);
-    if (rc == NRGBD_OK) rc = encode_cl_map(&tyl, p.y_lo, 2, N, p.Dout, p.Hout, p.Wout, p.Cs_out, p.Cs_out, 32, TW, TH, 1, 64);
-    if (rc != NRGBD_OK) return rc;
-    p.tma_store = 1;
-  }
-  typedef void (*KernelFn)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
-                           const CUtensorMap, const H2Params);
-  KernelFn fn = nullptr;
-  int slot = 0;
-  if (p.bkc != 32) { nrgbd_set_error("conv_h2: only 32-channel chunks are instantiated"); return NRGBD_ERR_UNSUPPORTED; }
-  if (p.gtaps == 3) {
-    if (p.msub == 4) { fn = conv_h2_kernel<2, 4, 3>; slot = 0; } else if (p.msub == 2) { fn = conv_h2_kernel<2, 2, 3>; slot = 1; } else { fn = conv_h2_kernel<2, 1, 3>; slot = 2; }
-  } else {
-    if (p.msub == 4) { fn = conv_h2_kernel<2, 4, 1>; slot = 3; } else if (p.msub == 2) { fn = conv_h2_kernel<2, 2, 1>; slot = 4; } else { fn = conv_h2_kernel<2, 1, 1>; slot = 5; }
-  }
-  static size_t configured[6] = {0, 0, 0, 0, 0, 0};
-  if (smem > configured[slot]) {
-    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) { nrgbd_set_error("conv_h2: cannot opt in to %zu bytes of shared memory: %s", smem, cudaGetErrorString(e)); return NRGBD_ERR_CUDA; }
-    configured[slot] = smem;
-  }
-  static int n_sm = 0;
-  if (!n_sm) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev); if (n_sm < 1) n_sm = 148; }
-  const long long items = (long long)N * p.Dz * p.tiles_x * p.tiles_y * n_chunks;      // tiles_y counts msub-high tiles
-  const unsigned grid = (unsigned)(items < n_sm ? items : n_sm);
-  fn<<<grid, H2_THREADS, smem, st>>>(ta_hi, ta_lo, tb, tb_last, ty, tyh, tyl, p);
-  return NRGBD_OK;
-}
-
 }  // namespace
 
 extern "C" {
 
 void nrgbd_dev_conv_h2_set_flags(int flags) { g_h2_flags = flags; }
-void nrgbd_dev_conv_h2_set_debug_buffer(long long* buf) { g_h2_dbg = buf; }
 void nrgbd_dev_conv_h2_set_smem_cap_kb(int kb) { g_h2_smem_cap_kb = kb; }
 
 // Channel plan of the f16-pair path: Cin padded to 32; Cout padded to 16 and cut into chunks of BN = min(128, Cout_pad)
@@ -830,7 +556,7 @@ int nrgbd_conv_h2_plan(int Cin, int Cout, int* Cin_pad, int* Cout_pad, int* BN) 
 int nrgbd_split_f16_pair(const float* x, long long n, void* hi, void* lo, cudaStream_t st) {
   NRGBD_REQUIRE(x && hi && lo && n > 0 && n % 4 == 0, "bad arguments");
   long long blocks = (n / 4 + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > nrgbd_sm_count() * 16ll) blocks = nrgbd_sm_count() * 16ll;
   split_f16_pair_kernel<<<(unsigned)blocks, 256, 0, st>>>(reinterpret_cast<const float4*>(x), n / 4, reinterpret_cast<uint2*>(hi),
                                                          reinterpret_cast<uint2*>(lo));
   NRGBD_COUNT(1);
@@ -878,25 +604,29 @@ static int conv_nhwc_h2_impl(const void* x_hi, const void* x_lo, int N, int Din,
   NRGBD_REQUIRE(x_hi && x_lo && w, "null pointer");
   NRGBD_REQUIRE(Cin_pad % 32 == 0 && Cin_pad >= 32 && Cin_pad <= Cs_in && Cs_in % 8 == 0 && Cout_pad % 16 == 0 && Cout <= Cout_pad && Cout > Cout_pad - 16 &&
                     BN == (Cout_pad < 128 ? Cout_pad : 128), "channel counts not supported by the f16-pair tensor-core path");
-  NRGBD_REQUIRE(kd >= 1 && kd <= 3 && kh * kw <= MAX_TAP2D && stride >= 1 && stride <= 8, "unsupported filter");
+  NRGBD_REQUIRE(kd >= 1 && kd <= 3 && kh * kw <= WG_MAX_TAP2D && stride >= 1 && stride <= 8, "unsupported filter");
   NRGBD_REQUIRE(Hout == (Hin + 2 * pad - dilation * (kh - 1) - 1) / stride + 1 &&
                     Wout == (Win + 2 * pad - dilation * (kw - 1) - 1) / stride + 1, "output extent mismatch");
-  H2Params p{};
-  p.y = y; p.bias = bias; p.stats = stats;
-  p.y_hi = y_hi; p.y_lo = y_lo; p.pair_out = y_hi ? 1 : 0;
-  p.N = N; p.Dz = Din; p.Hy = Hout; p.Wx = Wout;
-  p.in_stride = stride; p.Cout = Cout; p.BN = BN;
-  p.Dout = Din; p.Hout = Hout; p.Wout = Wout; p.Cs_out = Cs_out; p.c_off = c_off;
-  p.out_stride = 1; p.out_off_y = 0; p.out_off_x = 0; p.leaky = leaky;
-  p.n_kz = kd; p.n_tap = kh * kw;
-  for (int a = 0; a < kd; ++a) p.dz[a] = (signed char)(a - kd / 2);
+  if (y_hi) {
+    // the output as the operand pair of the next convolution: every Cs_out channel stored, pad channels as zeros
+    NRGBD_REQUIRE(Cs_out % 32 == 0 && Cs_out >= Cout_pad && c_off == 0 && stats == nullptr && (((uintptr_t)y_hi | (uintptr_t)y_lo) & 15) == 0 && y_lo,
+                  "pair output needs Cs_out % 32 == 0, c_off == 0 and no statistics");
+  }
+  WgConv c{};
+  c.tf32 = 0;
+  c.x_hi = x_hi; c.x_lo = x_lo; c.N = N; c.Din = Din; c.Hin = Hin; c.Win = Win; c.Cin_pad = Cin_pad; c.Cs_in = Cs_in;
+  c.w_hi = w; c.w_lo = reinterpret_cast<const __half*>(w) + (long long)Cout_pad * Cin_pad; c.w_tap_stride = 2ll * Cout_pad * Cin_pad;
+  c.n_wslices = kd * kh * kw; c.Cout_pad = Cout_pad;
+  c.bias = bias; c.stats = stats; c.y = y; c.y_hi = y_hi; c.y_lo = y_lo;
+  c.Cout = Cout; c.Dout = Din; c.Hout = Hout; c.Wout = Wout; c.Cs_out = Cs_out; c.c_off = c_off;
+  c.out_stride = 1; c.out_off_y = 0; c.out_off_x = 0; c.leaky = leaky;
+  c.Hy = Hout; c.Wx = Wout; c.in_stride = stride; c.n_kz = kd; c.n_tap = kh * kw;
+  for (int a = 0; a < kd; ++a) c.dz[a] = (signed char)(a - kd / 2);
   int t = 0;
   for (int b = 0; b < kh; ++b)
-    for (int c = 0; c < kw; ++c) { p.dy[t] = (signed char)(b * dilation - pad); p.dx[t] = (signed char)(c * dilation - pad); ++t; }
-  for (int a = 0; a < kd; ++a)
-    for (int u = 0; u < kh * kw; ++u) p.wsel[a * kh * kw + u] = (unsigned char)(a * kh * kw + u);
-  int rc = launch_h2(reinterpret_cast<const __half*>(x_hi), reinterpret_cast<const __half*>(x_lo), N, Din, Hin, Win, Cin_pad, Cs_in,
-                     reinterpret_cast<const __half*>(w), kd * kh * kw, Cout_pad, kh, kw, dilation, p, st);
+    for (int e = 0; e < kw; ++e) { c.dy[t] = (signed char)(b * dilation - pad); c.dx[t] = (signed char)(e * dilation - pad); ++t; }
+  for (int a = 0; a < kd * kh * kw; ++a) c.wsel[a] = (unsigned char)a;
+  int rc = conv_wgmma(c, st);
   if (rc != NRGBD_OK) return rc;
   NRGBD_COUNT(1);
   NRGBD_LAUNCH_CHECK();
@@ -914,21 +644,22 @@ int nrgbd_conv_transpose2d_k4s2_nhwc_h2(const void* x_hi, const void* x_lo, int 
   const int dys[2][2] = {{0, -1}, {1, 0}};
   for (int py = 0; py < 2; ++py)
     for (int px = 0; px < 2; ++px) {
-      H2Params p{};
-      p.y = y; p.bias = bias; p.stats = nullptr;
-      p.N = N; p.Dz = 1; p.Hy = Hin; p.Wx = Win;
-      p.in_stride = 1; p.Cout = Cout; p.BN = BN;
-      p.Dout = 1; p.Hout = 2 * Hin; p.Wout = 2 * Win; p.Cs_out = Cs_out; p.c_off = c_off;
-      p.out_stride = 2; p.out_off_y = py; p.out_off_x = px; p.leaky = leaky;
-      p.n_kz = 1; p.n_tap = 4; p.dz[0] = 0;
+      WgConv c{};
+      c.tf32 = 0;
+      c.x_hi = x_hi; c.x_lo = x_lo; c.N = N; c.Din = 1; c.Hin = Hin; c.Win = Win; c.Cin_pad = Cin_pad; c.Cs_in = Cs_in;
+      c.w_hi = w; c.w_lo = reinterpret_cast<const __half*>(w) + (long long)Cout_pad * Cin_pad; c.w_tap_stride = 2ll * Cout_pad * Cin_pad;
+      c.n_wslices = 16; c.Cout_pad = Cout_pad;
+      c.bias = bias; c.stats = nullptr; c.y = y;
+      c.Cout = Cout; c.Dout = 1; c.Hout = 2 * Hin; c.Wout = 2 * Win; c.Cs_out = Cs_out; c.c_off = c_off;
+      c.out_stride = 2; c.out_off_y = py; c.out_off_x = px; c.leaky = leaky;
+      c.Hy = Hin; c.Wx = Win; c.in_stride = 1; c.n_kz = 1; c.n_tap = 4;
       int t = 0;
       for (int a = 0; a < 2; ++a)
         for (int b = 0; b < 2; ++b) {
-          p.dy[t] = (signed char)dys[py][a]; p.dx[t] = (signed char)dys[px][b];
-          p.wsel[t] = (unsigned char)(kys[py][a] * 4 + kys[px][b]); ++t;
+          c.dy[t] = (signed char)dys[py][a]; c.dx[t] = (signed char)dys[px][b];
+          c.wsel[t] = (unsigned char)(kys[py][a] * 4 + kys[px][b]); ++t;
         }
-      int rc = launch_h2(reinterpret_cast<const __half*>(x_hi), reinterpret_cast<const __half*>(x_lo), N, 1, Hin, Win, Cin_pad, Cs_in,
-                         reinterpret_cast<const __half*>(w), 16, Cout_pad, 2, 2, 1, p, st);
+      int rc = conv_wgmma(c, st);
       if (rc != NRGBD_OK) return rc;
     }
   NRGBD_COUNT(4);

@@ -1,949 +1,31 @@
-// Tensor-core convolution for the KVNET conv stacks: tcgen05 / TMEM / TMA implicit GEMM with
-// error-compensated 3xTF32 products (SURVEY §8 a5, a8, a10; DESIGN.md §4, §7).
+// Tensor-core convolution with error-compensated 3xTF32 products (SURVEY §8 a5, a8, a10; DESIGN.md §4.2):
+// the `conv_math = 'tf32x3'` path. The GEMM is the wgmma kernel of conv_f16.cu (conv_wgmma) on TF32 operand pairs.
 //
 // Why 3xTF32: the reference's results must be matched to 1e-4 on the DPV through 61 (2-D) / 12 (3-D)
 // convolutions separated by batch-statistics BatchNorm; single-pass TF32 operands give 1e-2-level
 // DPV errors (SURVEY §7). Each fp32 operand is split a = a_hi + a_lo with a_hi = RN_tf32(a),
 // a_lo = RN_tf32(a - a_hi) and the product is accumulated as a_hi*b_hi + a_lo*b_hi + a_hi*b_lo in
-// the fp32 TMEM accumulator (dropped term <= 2^-22 |a b|).
+// fp32 (dropped term <= 2^-22 |a b|).
 //
-// Two kernels share the helpers below (one 128-pixel x Cout output tile per CTA in both):
-//
-// conv_tc2_kernel<GROUPS>  - the production kernel (DESIGN.md 4.2 has the measurements behind every choice)
-//   warp 0      TMA producer: per K-step (one filter tap x 32 input channels) an 8x16-pixel x 32-channel box of the RAW
-//               activation (5-D tensor map over [N][D][H][W][C]; padding = TMA out-of-bounds zero fill, conv stride =
-//               element stride, dilation / transposed-conv parity = box origin) into the activation ring, and the
-//               hi / lo weight slices into the weight ring; 128-byte-swizzled K-major tiles, mbarrier expect-tx.
-//   warps 2-5   (+ 7-10 when the CTA owns the SM) operand converters: one pixel row per thread, optional BatchNorm+ReLU
-//               of the input, hi / lo split in registers, tcgen05.st into a TMEM operand buffer; then the epilogue:
-//               tcgen05.ld, fp32 sum of the accumulators, bias / LeakyReLU, swizzled staging tile in shared memory,
-//               cp.async.bulk.tensor stores per 32-channel slab, BatchNorm column sums from the same tile.
-//   warp 1      MMA issuer (software-pipelined): a_hi x [b_hi | b_lo] as one MMA of width 2 Cout, a_lo x b_hi as a
-//               second, A from TMEM, B from shared memory; tcgen05.commit frees the weight slot / operand buffer.
-// conv_tc_kernel  - v1, kept as the fallback for Cout_pad > 128 and as a measured reference point: operands pre-split
-//   in global memory (nrgbd_split_tf32), four TMA loads per K-step, both operands from shared memory, two issue
-//   streams, direct vector stores.
-#include <cstdlib>
+// Two forms of the entry points:
+//   nrgbd_conv_nhwc_tc*   the activations arrive pre-split (nrgbd_split_tf32);
+//   nrgbd_conv_nhwc_tc2*  raw fp32 activations (optionally the RAW output of the producing convolution, normalised here
+//                         with its batch statistics: *_bn_in); the split (and the BatchNorm + ReLU) runs as one pass into
+//                         stream-ordered scratch memory right before the GEMM: 4 B read + 8 B written per element, the
+//                         same traffic as nrgbd_split_tf32. The *_bn_in form is what saves a pass: it replaces the separate
+//                         BatchNorm pass (4 B read + 4 B written) in front of that split.
 #include <cuda.h>
 
 #include "common.cuh"
-#include "../../include/nrgbd_dev.h"
+#include "conv_wgmma.cuh"
+#include "../../include/nrgbd.h"
 
 namespace {
 
-constexpr int TH = 8, TW = 16;       // spatial tile: 8 rows x 16 columns = 128 GEMM rows
-constexpr int BK = 32;               // input channels per K-step (128 bytes = one swizzle row)
-constexpr int A_TILE_BYTES = 128 * BK * 4;
-constexpr int MAX_TAPS_TC = 27;
-constexpr int NUM_THREADS = 224;      // warps: 0 TMA, 1 MMA stream 0 (+TMEM alloc), 2-5 epilogue, 6 MMA stream 1
-
-struct TcParams {
-  float* y; const float* bias; double* stats;
-  int N, Dz, Hy, Wx;                 // iteration space (output positions before out_stride/off)
-  int tiles_x, tiles_y;
-  int cin_chunks, n_taps, in_stride;
-  int Cout, Cout_pad;
-  int Dout, Hout, Wout, Cs_out, c_off, out_stride, out_off_y, out_off_x;
-  int leaky, stages, tmem_cols, nacc, dev_flags;   // nacc: rotating main accumulators (nm)
-  int nl;                            // v2: number of TMEM operand buffers (2 or 4)
-  int n_issue;                       // MMA issue streams (warps): 1 or 2
-  int tma_store;                     // v2: output tile leaves through a TMA tensor store (stride-1 outputs)
-  int stages_a;                      // v2: activation-ring depth (stages = weight-ring depth)
-  // v2, optional: training-mode BatchNorm (+ReLU) of the INPUT tensor applied in the converter (the producing conv
-  // left raw outputs + per-channel sums): x' = [relu](x * scale[c] + shift[c]), zero outside the image
-  const double* in_stats; double in_count;
-  const float* in_gamma; const float* in_beta; float* in_run_mean; float* in_run_var;
-  float in_eps, in_momentum;
-  int in_relu, in_C, in_H, in_W, in_D;
-  long long* dbg;                    // optional [grid][64] clock64 timestamps (development)
-  signed char dz[MAX_TAPS_TC], dy[MAX_TAPS_TC], dx[MAX_TAPS_TC];
-  unsigned char wsel[MAX_TAPS_TC];
-};
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-// One elected lane of a converged warp (cute::elect_one_sync): keeps tcgen05 / TMA issue on the
-// uniform datapath instead of a per-instruction divergence loop.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .b32 %%rx;\n\t.reg .pred %%px;\n\t"
-      "elect.sync %%rx|%%px, %1;\n\t"
-      "@%%px mov.s32 %0, 1;\n\t}"
-      : "+r"(pred) : "r"(0xffffffffu));
-  return pred != 0;
-}
-__device__ __forceinline__ int uniform_warp_idx() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x / 32), 0); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  if (elect_one()) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-// Bounded spin: a protocol bug becomes a trap (error) instead of a hung GPU.
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0;
-#pragma unroll 1
-  for (uint32_t it = 0; it < (1u << 28); ++it) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.b32 %0, 1, 0, p;\n\t}"
-        : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    if (done) return;
-  }
-  __trap();
-}
-
-__device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2,
-                                            int c3, int c4) {
-  if (elect_one()) asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-      ::"r"(dst), "l"((uint64_t)tm), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2) {
-  if (elect_one()) asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(dst), "l"((uint64_t)tm), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, sm_100):
-// start address >> 4 [0,14), LBO >> 4 [16,30) (ignored for swizzled K-major, set to 1),
-// SBO >> 4 [32,46) = 1024 B between 8-row groups, version 1 [46,48), layout SWIZZLE_128B (2) [61,64).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) |
-         ((uint64_t)2 << 61);
-}
-
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if (elect_one()) asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// Raw (un-elected) forms for use inside ONE `if (elect_one())` block per K-step: measured with
-// tools/mma_probe.py, a per-MMA elect + 64-bit descriptor construction costs ~75 issue cycles per MMA,
-// more than the tensor work of an N <= 128 MMA (16-64 cycles), so the issue stream must be lean:
-// descriptors are (constant high word, low word = stage base + immediate).
-constexpr uint32_t DESC_HI = (uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29);     // SBO, version 1, SWIZZLE_128B
-__device__ __forceinline__ uint32_t desc_lo(uint32_t saddr) { return ((saddr & 0x3FFFFu) >> 4) | (1u << 16); }
-__device__ __forceinline__ uint64_t desc_of(uint32_t lo) { return ((uint64_t)DESC_HI << 32) | (uint64_t)lo; }
-__device__ __forceinline__ void umma_tf32_raw(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_tf32_ts_raw(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit_raw(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  if (elect_one()) asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-__global__ void __launch_bounds__(NUM_THREADS, 2)
-conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
-               const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
-               const TcParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  const long long t_start = clock64();
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
-  const int BN = p.Cout_pad;
-  const uint32_t b_tile_bytes = (uint32_t)BN * BK * 4;
-  const uint32_t stage_bytes = 2 * A_TILE_BYTES + 2 * b_tile_bytes;
-  const uint32_t bars = smem_base + p.stages * stage_bytes;       // full[stages], empty[stages], tmem_full, tmem_ptr
-  const uint32_t bar_full = bars, bar_empty = bars + 8 * p.stages, bar_tmem = bars + 16 * p.stages;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem_gen + p.stages * stage_bytes + 16 * p.stages + 8);
-
-  const int warp = uniform_warp_idx(), lane = threadIdx.x % 32;
-
-  // tile coordinates
-  int t = blockIdx.x;
-  const int tx = t % p.tiles_x; t /= p.tiles_x;
-  const int ty = t % p.tiles_y; t /= p.tiles_y;
-  const int z0 = t % p.Dz;
-  const int n0 = t / p.Dz;
-  const int ox0 = tx * TW, oy0 = ty * TH;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < p.stages; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, p.n_issue); }
-    mbar_init(bar_tmem, p.n_issue);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tm_a_hi) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tm_a_lo) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tm_b_hi) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tm_b_lo) : "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"((uint32_t)p.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  if (p.dbg && threadIdx.x == 0) { p.dbg[blockIdx.x * 64 + 0] = t_start; p.dbg[blockIdx.x * 64 + 1] = clock64(); }
-
-  const int nk = p.n_taps * p.cin_chunks;
-
-  if (warp == 0) {
-    {
-      // ===== TMA producer (whole warp converged; one elected lane issues) =====
-      for (int ks = 0; ks < nk; ++ks) {
-        const int s = ks % p.stages;
-        const uint32_t ph = (uint32_t)(ks / p.stages) & 1u;
-        mbar_wait(bar_empty + 8 * s, ph ^ 1u);
-        const bool one = (p.dev_flags & 1) != 0;
-        mbar_expect_tx(bar_full + 8 * s, one ? stage_bytes / 2 : stage_bytes);
-        const int tap = ks / p.cin_chunks, cc = ks - tap * p.cin_chunks;
-        const uint32_t sa = smem_base + s * stage_bytes;
-        const int cx = ox0 * p.in_stride + p.dx[tap], cy = oy0 * p.in_stride + p.dy[tap], cz = z0 + p.dz[tap];
-        tma_load_5d(sa, &tm_a_hi, bar_full + 8 * s, cc * BK, cx, cy, cz, n0);
-        if (!one) tma_load_5d(sa + A_TILE_BYTES, &tm_a_lo, bar_full + 8 * s, cc * BK, cx, cy, cz, n0);
-        tma_load_3d(sa + 2 * A_TILE_BYTES, &tm_b_hi, bar_full + 8 * s, cc * BK, 0, p.wsel[tap]);
-        if (!one) tma_load_3d(sa + 2 * A_TILE_BYTES + b_tile_bytes, &tm_b_lo, bar_full + 8 * s, cc * BK, 0, p.wsel[tap]);
-      }
-    }
-  } else if (warp == 1 || warp == 6) {
-    const int w = warp == 1 ? 0 : 1;
-    if (w < p.n_issue) {
-      // ===== MMA issue stream w (whole warp converged; one elected lane issues) =====
-      // One issuing warp sustains about one tcgen05.mma per ~100 cycles whatever N, the pipeline depth
-      // or the operand bytes (measured: 1320 cycles per 12-MMA K-step for N = 64 and N = 128 alike;
-      // rotating or grouping destinations does not help), while independent streams scale. So the
-      // K-slices of every K-step are divided between n_issue warps, each with its own accumulator
-      // pair so that no ordering between the streams is needed:
-      //   columns [(2w)*BN, +BN)   stream w: a_hi*b_hi        (fp32 accumulation truncates: two half-
-      //   columns [(2w+1)*BN, +BN) stream w: cross terms        length chains + RN sum in the epilogue)
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((128u >> 4) << 24);
-      const int k_lo = w * (BK / 8) / p.n_issue, k_hi = (w + 1) * (BK / 8) / p.n_issue;
-      const uint32_t d_base = tmem_base + (uint32_t)(w * (p.nacc + 1) * BN);   // stream w: nacc rotating mains, then cross terms
-      const uint32_t d_lo = d_base + (uint32_t)(p.nacc * BN);
-      const bool one = (p.dev_flags & 1) != 0;
-      for (int ks = 0; ks < nk; ++ks) {
-        const int s = ks % p.stages;
-        const uint32_t ph = (uint32_t)(ks / p.stages) & 1u;
-        mbar_wait(bar_full + 8 * s, ph);
-        if (p.dbg && ks == 0 && lane == 0 && w == 0) p.dbg[blockIdx.x * 64 + 2] = clock64();      // first operands landed
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t sa = smem_base + s * stage_bytes;
-        const uint32_t d_main = d_base + (uint32_t)((ks % p.nacc) * BN);        // rotates per K-step (RZ drift)
-        const uint32_t la_hi = desc_lo(sa), la_lo = desc_lo(sa + A_TILE_BYTES);
-        const uint32_t lb_hi = desc_lo(sa + 2 * A_TILE_BYTES), lb_lo = desc_lo(sa + 2 * A_TILE_BYTES + b_tile_bytes);
-        if (elect_one()) {
-#pragma unroll
-          for (int k4 = 0; k4 < BK / 8; ++k4) {
-            if (k4 >= k_lo && k4 < k_hi) {
-              const uint32_t acc = (ks > 0 || k4 > k_lo) ? 1u : 0u;
-              const uint32_t acc_m = (ks >= p.nacc || k4 > k_lo) ? 1u : 0u;
-              if (!one) {
-                umma_tf32_raw(d_lo, desc_of(la_lo + 2 * k4), desc_of(lb_hi + 2 * k4), idesc, acc);
-                umma_tf32_raw(d_lo, desc_of(la_hi + 2 * k4), desc_of(lb_lo + 2 * k4), idesc, 1u);
-              } else if (ks == 0 && k4 == k_lo) {
-                umma_tf32_raw(d_lo, desc_of(la_hi + 2 * k4), desc_of(lb_hi + 2 * k4), idesc, 0u);   // 1xTF32 experiment
-              }
-              umma_tf32_raw(d_main, desc_of(la_hi + 2 * k4), desc_of(lb_hi + 2 * k4), idesc, acc_m);
-            }
-          }
-          umma_commit_raw(bar_empty + 8 * s);       // this stream is done with the smem stage
-        }
-        __syncwarp();
-      }
-      umma_commit(bar_tmem);                      // this stream's accumulators are complete
-      if (p.dbg && lane == 0 && w == 0) p.dbg[blockIdx.x * 64 + 3] = clock64();      // all MMAs issued
-    }
-  } else if (warp >= 2 && warp <= 5) {
-    // ===== epilogue (warps 2..5): TMEM lanes [32*(warp%4), +32) =====
-    const int q = warp & 3;
-    const int r = q * 32 + lane;                  // GEMM row = TMEM lane = pixel within the tile
-    const int py = r / TW, px = r % TW;
-    const int iy = oy0 + py, ix = ox0 + px;
-    const bool valid = iy < p.Hy && ix < p.Wx;
-    const int oy = iy * p.out_stride + p.out_off_y, ox = ix * p.out_stride + p.out_off_x;
-    float* dst = p.y + ((((long long)n0 * p.Dout + z0) * p.Hout + oy) * p.Wout + ox) * (long long)p.Cs_out + p.c_off;
-    float* ep = reinterpret_cast<float*>(smem_gen);          // [128][BN+1] staging, reuses the pipeline stages
-    const int EPS = BN + 1;
-    mbar_wait(bar_tmem, 0);
-    if (p.dbg && threadIdx.x == 64) p.dbg[blockIdx.x * 64 + 4] = clock64();   // accumulator complete
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const bool vec_ok = ((p.Cs_out | p.c_off) & 3) == 0;
-    for (int c0 = 0; c0 < BN; c0 += 16) {
-      float accv[16];
-      {
-        // accumulator order: cross-term accumulators first (small), then the main chains; fetched
-        // four at a time back to back with one wait
-        const int per = p.nacc + 1;                         // accumulators per issue stream: nacc mains + cross terms
-        const int used_m = nk < p.nacc ? nk : p.nacc;       // mains actually written (rotation per K-step)
-        const int n_acc = p.n_issue * (used_m + 1);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) accv[j] = 0.f;
-#pragma unroll 1
-        for (int a0 = 0; a0 < n_acc; a0 += 4) {
-          uint32_t v[4][16];
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            if (a0 + u < n_acc) {
-              const int idx = a0 + u;
-              // cross-term accumulators first (small), then the mains of every stream
-              const int slot = (idx < p.n_issue) ? idx * per + p.nacc : ((idx - p.n_issue) / used_m) * per + (idx - p.n_issue) % used_m;
-              const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(slot * BN + c0);
-              asm volatile(
-                  "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                  : "=r"(v[u][0]), "=r"(v[u][1]), "=r"(v[u][2]), "=r"(v[u][3]), "=r"(v[u][4]), "=r"(v[u][5]), "=r"(v[u][6]),
-                    "=r"(v[u][7]), "=r"(v[u][8]), "=r"(v[u][9]), "=r"(v[u][10]), "=r"(v[u][11]), "=r"(v[u][12]),
-                    "=r"(v[u][13]), "=r"(v[u][14]), "=r"(v[u][15])
-                  : "r"(taddr) : "memory");
-            }
-          }
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            if (a0 + u < n_acc) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) accv[j] += __uint_as_float(v[u][j]);
-            }
-        }
-      }
-      float f[16];
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        float x = accv[j];
-        const int co = c0 + j;
-        if (p.bias && co < p.Cout) x += __ldg(p.bias + co);
-        if (p.leaky) x = x >= 0.f ? x : x * 0.01f;
-        f[j] = (valid && co < p.Cout) ? x : 0.f;
-      }
-      if (valid && !(p.dev_flags & 32)) {
-        if (vec_ok && c0 + 16 <= p.Cout) {
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) *reinterpret_cast<float4*>(dst + c0 + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) if (c0 + j < p.Cout) dst[c0 + j] = f[j];
-        }
-      }
-      if (p.stats && !(p.dev_flags & 16)) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) ep[r * EPS + c0 + j] = f[j];
-      }
-    }
-    if (p.dbg && threadIdx.x == 64) p.dbg[blockIdx.x * 64 + 5] = clock64();   // outputs stored
-    if (p.stats && !(p.dev_flags & 16)) {
-      asm volatile("bar.sync 1, 128;" ::: "memory");         // the four epilogue warps only
-      const int e = threadIdx.x - 64;                        // 0..127
-      for (int co = e; co < p.Cout; co += 128) {
-        float s1 = 0.f, s2 = 0.f;
-        for (int rr = 0; rr < 128; ++rr) { float x = ep[rr * EPS + co]; s1 += x; s2 = fmaf(x, x, s2); }
-        atomicAdd(p.stats + co, (double)s1);
-        atomicAdd(p.stats + p.Cout + co, (double)s2);
-      }
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols) : "memory");
-  }
-  if (p.dbg && threadIdx.x == 32) {
-    unsigned smid; asm("mov.u32 %0, %%smid;" : "=r"(smid));
-    p.dbg[blockIdx.x * 64 + 6] = clock64(); p.dbg[blockIdx.x * 64 + 7] = smid;
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// v2: in-kernel operand split, A operand from TMEM.
-// TMA brings the RAW fp32 activation box (16 KB per K-step instead of 32 KB of pre-split hi/lo:
-// the kernel is L2->SM bandwidth bound, DESIGN.md §4). Warps 2-5 read their pixel's 128-byte row
-// from the swizzled tile, split it in registers (cvt.rna.tf32) and tcgen05.st hi and lo into a
-// double-buffered TMEM operand region; warp 1 issues the three MMAs per K-slice with A from TMEM
-// and the pre-split K-major weights from smem. The separate split kernel and its HBM round trip
-// disappear.
-//   barriers: full[s]  TMA -> converter (A) and MMA (B)           (expect-tx)
-//             empty[s] 4 converter-warp arrivals + 1 tcgen05.commit -> TMA
-//             afull[b] 4 converter-warp arrivals -> MMA            (TMEM operand buffer b written)
-//             aempty[b] tcgen05.commit -> converter                (MMAs reading buffer b retired)
-//             tmem_full tcgen05.commit -> epilogue
-// ---------------------------------------------------------------------------------------------
-constexpr int NUM_THREADS2 = 224;       // one converter/epilogue group (two CTAs per SM)
-constexpr int NUM_THREADS2_G2 = 352;    // + warps 7-10: second converter/epilogue group (one CTA per SM)
-constexpr int A_BUF_COLS = 64;                 // 32 hi + 32 lo columns per TMEM operand buffer
-
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if (elect_one()) asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-        "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]),
-        "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]),
-        "r"(v[30]), "r"(v[31]) : "memory");
-}
-
-// GROUPS = number of 4-warp converter/epilogue groups. One warp per SM sub-partition issues an
-// instruction every ~4.7 cycles (measured: 174 SASS instructions of epilogue arithmetic = 818 cycles), so
-// with a single group both the operand conversion (~1000 cycles per K-step against a 768-cycle tensor
-// floor at N = 128) and the epilogue (~2400 cycles per 16-column chunk) are bound by one warp's issue
-// rate. With one CTA per SM a second group (warps 7-10) takes the odd K-steps / odd column chunks.
-template <int GROUPS>
-__global__ void __launch_bounds__(GROUPS == 2 ? NUM_THREADS2_G2 : NUM_THREADS2, GROUPS == 2 ? 1 : 2)
-conv_tc2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b_hi,
-                const __grid_constant__ CUtensorMap tm_b_lo, const __grid_constant__ CUtensorMap tm_y, const TcParams p) {
-  // Shared memory: [activation ring: stages_a x 16 KB][weight ring: stages x (hi | lo) tile][barriers].
-  // Two rings because the two operands live very differently long: a raw activation tile is free as soon as
-  // the converter warps have read it (TMA latency + ~700 cycles), a weight tile only when the MMAs that read
-  // it have retired (another ~2000 cycles) - and the K-step rate is ring depth / slot lifetime (measured:
-  // 2 -> 3 -> 4 joint stages = 62K -> 36K -> 31K cycles for the 128-channel layer). The 1024-byte alignment
-  // the swizzled tiles need is requested from the compiler instead of padded for: two CTAs per SM use every byte.
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t smem_base = smem_u32(smem_raw);
-  if (smem_base & 1023u) __trap();
-  uint8_t* smem_gen = smem_raw;
-  const int BN = p.Cout_pad;
-  const uint32_t b_tile_bytes = (uint32_t)BN * BK * 4;
-  const uint32_t b_slot_bytes = 2 * b_tile_bytes;
-  const uint32_t b_ring = smem_base + (uint32_t)p.stages_a * A_TILE_BYTES;
-  const uint32_t ring_bytes = (uint32_t)p.stages_a * A_TILE_BYTES + (uint32_t)p.stages * b_slot_bytes;
-  const uint32_t bars = smem_base + ring_bytes;
-  // barriers: a_full[8] a_empty[8] b_full[8] b_empty[8] afull[4] aempty[4] tmem
-  const uint32_t bar_full = bars, bar_empty = bars + 64, bar_bfull = bars + 128, bar_bempty = bars + 192,
-                 bar_afull = bars + 256, bar_aempty = bars + 288, bar_tmem = bars + 320;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem_gen + ring_bytes + 328);
-  float* in_sc = reinterpret_cast<float*>(smem_gen + ring_bytes + 512);        // [Cin_pad] scale, then [Cin_pad] shift
-  const int cin_pad = p.cin_chunks * BK;
-  float* in_sh = in_sc + cin_pad;
-
-  const long long t_start = clock64();
-  const int warp = uniform_warp_idx(), lane = threadIdx.x % 32;
-  int t = blockIdx.x;
-  const int tx = t % p.tiles_x; t /= p.tiles_x;
-  const int ty = t % p.tiles_y; t /= p.tiles_y;
-  const int z0 = t % p.Dz;
-  const int n0 = t / p.Dz;
-  const int ox0 = tx * TW, oy0 = ty * TH;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < p.stages_a; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 4); }
-    for (int s = 0; s < p.stages; ++s) { mbar_init(bar_bfull + 8 * s, 1); mbar_init(bar_bempty + 8 * s, p.n_issue); }
-    for (int b = 0; b < p.nl; ++b) { mbar_init(bar_afull + 8 * b, 4); mbar_init(bar_aempty + 8 * b, p.n_issue); }
-    mbar_init(bar_tmem, p.n_issue);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tm_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tm_b_hi) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tm_b_lo) : "memory");
-    if (p.tma_store) asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tm_y) : "memory");
-  }
-  if (p.in_stats) {
-    // the BatchNorm of the producing layer, finalised per CTA exactly as nrgbd_bn_apply_stats does (conv.cu)
-    for (int c = threadIdx.x; c < cin_pad; c += blockDim.x) {
-      float sc = 0.f, sh = 0.f;
-      if (c < p.in_C) {
-        const double mean = p.in_stats[c] / p.in_count;
-        double var = p.in_stats[p.in_C + c] / p.in_count - mean * mean;
-        if (var < 0) var = 0;
-        const float invstd = (float)(1.0 / sqrt(var + (double)p.in_eps));
-        sc = p.in_gamma[c] * invstd;
-        sh = p.in_beta[c] - (float)mean * sc;
-        if (p.in_run_mean && blockIdx.x == 0) {
-          const double unb = p.in_count > 1 ? var * p.in_count / (p.in_count - 1) : var;
-          p.in_run_mean[c] = (1.f - p.in_momentum) * p.in_run_mean[c] + p.in_momentum * (float)mean;
-          p.in_run_var[c] = (1.f - p.in_momentum) * p.in_run_var[c] + p.in_momentum * (float)unb;
-        }
-      }
-      in_sc[c] = sc; in_sh[c] = sh;
-    }
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"((uint32_t)p.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  if (p.dbg && threadIdx.x == 0) { p.dbg[blockIdx.x * 64 + 0] = t_start; p.dbg[blockIdx.x * 64 + 1] = clock64(); }
-  const uint32_t acc_cols = (uint32_t)(p.n_issue * (p.nacc + 1) * BN);   // operand buffers live after the accumulators
-  const int nk = p.n_taps * p.cin_chunks;
-
-  if (warp == 0) {
-    {
-      // Running counters, no division: each role is a single warp, and a lone warp issues one dependent
-      // instruction every ~4-5 cycles - a runtime % or / costs ~150 cycles of its K-step budget.
-      int sa = 0, sb = 0, tap = 0, cc = 0;
-      uint32_t pha = 0, phb = 0;
-      for (int ks = 0; ks < nk; ++ks) {
-        const int cx = ox0 * p.in_stride + p.dx[tap], cy = oy0 * p.in_stride + p.dy[tap], cz = z0 + p.dz[tap];
-        mbar_wait(bar_empty + 8 * sa, pha ^ 1u);
-        const bool tr = p.dbg && lane == 0 && ks >= 8 && ks < 14;
-        if (tr) p.dbg[blockIdx.x * 64 + 16 + (ks - 8) * 8 + 6] = clock64();
-        mbar_expect_tx(bar_full + 8 * sa, A_TILE_BYTES);
-        tma_load_5d(smem_base + sa * A_TILE_BYTES, &tm_a, bar_full + 8 * sa, cc * BK, cx, cy, cz, n0);
-        mbar_wait(bar_bempty + 8 * sb, phb ^ 1u);
-        if (tr) p.dbg[blockIdx.x * 64 + 16 + (ks - 8) * 8 + 7] = clock64();
-        mbar_expect_tx(bar_bfull + 8 * sb, b_slot_bytes);
-        const uint32_t sbm = b_ring + sb * b_slot_bytes;
-        tma_load_3d(sbm, &tm_b_hi, bar_bfull + 8 * sb, cc * BK, 0, p.wsel[tap]);
-        tma_load_3d(sbm + b_tile_bytes, &tm_b_lo, bar_bfull + 8 * sb, cc * BK, 0, p.wsel[tap]);
-        if (++cc == p.cin_chunks) { cc = 0; ++tap; }
-        if (++sa == p.stages_a) { sa = 0; pha ^= 1u; }
-        if (++sb == p.stages) { sb = 0; phb ^= 1u; }
-      }
-    }
-  } else if (warp == 1 || warp == 6) {
-    const int w = warp == 1 ? 0 : 1;
-    if (w < p.n_issue) {
-      // ===== MMA issue stream w (see conv_tc_kernel) =====
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((128u >> 4) << 24);
-      const int k_lo = w * (BK / 8) / p.n_issue, k_hi = (w + 1) * (BK / 8) / p.n_issue;
-      const uint32_t d_base = tmem_base + (uint32_t)(w * (p.nacc + 1) * BN);
-      const uint32_t d_lo = d_base + (uint32_t)(p.nacc * BN);
-      int s = 0, b = 0, m = 0;
-      uint32_t sph = 0, bph = 0;
-      if (p.n_issue == 1) {
-        // Single stream, software-pipelined: tcgen05.mma issue blocks at the tensor rate (the queue is short:
-        // 12 N=128 MMAs take ~770 cycles to issue), so anything this thread does between the last MMA of a
-        // K-step and the first of the next is tensor idle time (measured ~390 cycles per K-step). The waits
-        // and address arithmetic for K-step ks+1 therefore run before the last k-slice of K-step ks is issued,
-        // while the queue still holds work.
-        const bool concat = p.nacc == 1 && 2 * BN <= 256 && !(p.dev_flags & 4096);
-        const uint32_t idesc2 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)((2 * BN) >> 3) << 17) | ((128u >> 4) << 24);
-        mbar_wait(bar_bfull, 0);
-        mbar_wait(bar_afull, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        for (int ks = 0; ks < nk; ++ks) {
-          const uint32_t d_main = d_base + (uint32_t)(m * BN);
-          const uint32_t sbm = b_ring + s * b_slot_bytes;
-          const uint32_t a_hi0 = tmem_base + acc_cols + (uint32_t)(b * A_BUF_COLS);
-          const uint32_t lb_hi = desc_lo(sbm), lb_lo = desc_lo(sbm + b_tile_bytes);
-          const uint32_t acc0 = ks > 0 ? 1u : 0u, accm0 = ks >= p.nacc ? 1u : 0u;
-          const uint32_t bar_e = bar_bempty + 8 * s, bar_ae = bar_aempty + 8 * b;
-          const bool tr = p.dbg && lane == 0 && ks >= 8 && ks < 14;
-          if (tr) p.dbg[blockIdx.x * 64 + 16 + (ks - 8) * 8 + 4] = clock64();
-          if (concat) {
-            // one main accumulator: main | cross columns are adjacent and so are the hi | lo weight tiles, so
-            // a_hi x [b_hi | b_lo] is ONE MMA of width 2 BN (main and the a_hi*b_lo cross term), a_lo x b_hi a
-            // second one: 8 issue slots per K-step instead of 12 (a lone issuing thread tops out at ~48 cycles
-            // per MMA, above the 32-cycle tensor time of an N = 64 MMA)
-            // (the four wide MMAs first, then the narrow ones: alternating instruction shapes issue slower)
-            if (elect_one()) {
-#pragma unroll
-              for (int k4 = 0; k4 < BK / 8; ++k4)
-                umma_tf32_ts_raw(d_base, a_hi0 + k4 * 8, desc_of(lb_hi + 2 * k4), idesc2, k4 == 0 ? acc0 : 1u);
-#pragma unroll
-              for (int k4 = 0; k4 < BK / 16; ++k4)
-                umma_tf32_ts_raw(d_lo, a_hi0 + 32 + k4 * 8, desc_of(lb_hi + 2 * k4), idesc, 1u);
-            }
-          } else
-          if (elect_one()) {
-            umma_tf32_ts_raw(d_lo, a_hi0 + 32, desc_of(lb_hi), idesc, acc0);
-            umma_tf32_ts_raw(d_lo, a_hi0, desc_of(lb_lo), idesc, 1u);
-            umma_tf32_ts_raw(d_main, a_hi0, desc_of(lb_hi), idesc, accm0);
-#pragma unroll
-            for (int k4 = 1; k4 < BK / 8 - 1; ++k4) {
-              umma_tf32_ts_raw(d_lo, a_hi0 + 32 + k4 * 8, desc_of(lb_hi + 2 * k4), idesc, 1u);
-              umma_tf32_ts_raw(d_lo, a_hi0 + k4 * 8, desc_of(lb_lo + 2 * k4), idesc, 1u);
-              umma_tf32_ts_raw(d_main, a_hi0 + k4 * 8, desc_of(lb_hi + 2 * k4), idesc, 1u);
-            }
-          }
-          __syncwarp();
-          if (++s == p.stages) { s = 0; sph ^= 1u; }
-          if (++b == p.nl) { b = 0; bph ^= 1u; }
-          if (++m == p.nacc) m = 0;
-          if (ks + 1 < nk) {
-            mbar_wait(bar_bfull + 8 * s, sph);          // weights of the next K-step landed
-            mbar_wait(bar_afull + 8 * b, bph);          // its operand buffer is written
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          }
-          if (elect_one()) {
-            constexpr int k4 = BK / 8 - 1;
-            if (concat) {
-#pragma unroll
-              for (int kk = BK / 16; kk < BK / 8; ++kk)
-                umma_tf32_ts_raw(d_lo, a_hi0 + 32 + kk * 8, desc_of(lb_hi + 2 * kk), idesc, 1u);
-            } else {
-              umma_tf32_ts_raw(d_lo, a_hi0 + 32 + k4 * 8, desc_of(lb_hi + 2 * k4), idesc, 1u);
-              umma_tf32_ts_raw(d_lo, a_hi0 + k4 * 8, desc_of(lb_lo + 2 * k4), idesc, 1u);
-              umma_tf32_ts_raw(d_main, a_hi0 + k4 * 8, desc_of(lb_hi + 2 * k4), idesc, 1u);
-            }
-            umma_commit_raw(bar_e);        // weights of this stage consumed
-            umma_commit_raw(bar_ae);       // operand buffer consumed
-          }
-          if (tr) p.dbg[blockIdx.x * 64 + 16 + (ks - 8) * 8 + 5] = clock64();
-          __syncwarp();
-        }
-      } else
-      for (int ks = 0; ks < nk; ++ks) {
-        const uint32_t d_main = d_base + (uint32_t)(m * BN);
-        const bool fresh_main = ks < p.nacc;           // first use of this main accumulator: overwrite
-        mbar_wait(bar_bfull + 8 * s, sph);            // weights landed
-        mbar_wait(bar_afull + 8 * b, bph);            // operand buffer b written
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t sbm = b_ring + s * b_slot_bytes;
-        const uint32_t a_hi0 = tmem_base + acc_cols + (uint32_t)(b * A_BUF_COLS);
-        const uint32_t lb_hi = desc_lo(sbm), lb_lo = desc_lo(sbm + b_tile_bytes);
-        if (elect_one()) {
-#pragma unroll
-          for (int k4 = 0; k4 < BK / 8; ++k4) {
-            if (k4 >= k_lo && k4 < k_hi) {
-              const uint32_t a_hi = a_hi0 + k4 * 8, a_lo = a_hi0 + 32 + k4 * 8;
-              const uint32_t acc = (ks > 0 || k4 > k_lo) ? 1u : 0u;
-              const uint32_t acc_m = (!fresh_main || k4 > k_lo) ? 1u : 0u;
-              umma_tf32_ts_raw(d_lo, a_lo, desc_of(lb_hi + 2 * k4), idesc, acc);
-              umma_tf32_ts_raw(d_lo, a_hi, desc_of(lb_lo + 2 * k4), idesc, 1u);
-              umma_tf32_ts_raw(d_main, a_hi, desc_of(lb_hi + 2 * k4), idesc, acc_m);
-            }
-          }
-          umma_commit_raw(bar_bempty + 8 * s);     // weights of slot s consumed by this stream
-          umma_commit_raw(bar_aempty + 8 * b);     // operand buffer b consumed by this stream
-        }
-        __syncwarp();
-        if (++s == p.stages) { s = 0; sph ^= 1u; }
-        if (++b == p.nl) { b = 0; bph ^= 1u; }
-        if (++m == p.nacc) m = 0;
-      }
-      umma_commit(bar_tmem);
-    }
-  } else if ((warp >= 2 && warp <= 5) || warp >= 7) {
-    const int cg = warp >= 7 ? 1 : 0;             // converter / epilogue group
-    const int q = warp & 3;                       // TMEM lane quarter this warp may access
-    const int r = q * 32 + lane;                  // GEMM row = TMEM lane = pixel within the tile
-    // ===== operand converter: group cg owns K-steps cg, cg + GROUPS, ... (= operand buffer cg when GROUPS == 2) =====
-    int s = cg, b = cg;                           // stages_a >= 2 and nl >= 2 >= GROUPS
-    uint32_t sph = 0, bph = 0;
-    const bool fuse_in = p.in_stats != nullptr;
-    int f_cc = cg, f_tap = 0;                     // channel chunk / tap of this group's K-step (fused input BN only)
-    while (f_cc >= p.cin_chunks) { f_cc -= p.cin_chunks; ++f_tap; }
-    const int in_py = (oy0 + r / TW) * p.in_stride, in_px = (ox0 + r % TW) * p.in_stride;
-    for (int ks = cg; ks < nk; ks += GROUPS) {
-      mbar_wait(bar_full + 8 * s, sph);
-      const bool tr = p.dbg && threadIdx.x == 64 && ks >= 8 && ks < 14;
-      if (tr) p.dbg[blockIdx.x * 64 + 16 + (ks - 8) * 8 + 0] = clock64();
-      const uint8_t* row = smem_gen + (size_t)s * A_TILE_BYTES + (size_t)r * 128;
-      uint32_t hi[32], lo[32];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {               // 16-byte chunk j of this row sits at chunk (j ^ (r & 7))
-        const float4 v = *reinterpret_cast<const float4*>(row + ((j ^ (r & 7)) << 4));
-        float a[4] = {v.x, v.y, v.z, v.w};
-        if (fuse_in) {
-          // y = [relu](x * scale + shift) of the producing layer's BatchNorm, same fmaf as the stand-alone pass;
-          // TMA zero-filled the padding with RAW zeros, which must stay zeros of the normalised tensor
-          const int iy = in_py + p.dy[f_tap], ix = in_px + p.dx[f_tap], iz = z0 + p.dz[f_tap];
-          const bool inb = iy >= 0 && iy < p.in_H && ix >= 0 && ix < p.in_W && iz >= 0 && iz < p.in_D;
-          const float4 sc = *reinterpret_cast<const float4*>(in_sc + f_cc * BK + 4 * j);
-          const float4 sh = *reinterpret_cast<const float4*>(in_sh + f_cc * BK + 4 * j);
-          a[0] = fmaf(a[0], sc.x, sh.x); a[1] = fmaf(a[1], sc.y, sh.y); a[2] = fmaf(a[2], sc.z, sh.z); a[3] = fmaf(a[3], sc.w, sh.w);
-          if (p.in_relu) { a[0] = fmaxf(a[0], 0.f); a[1] = fmaxf(a[1], 0.f); a[2] = fmaxf(a[2], 0.f); a[3] = fmaxf(a[3], 0.f); }
-          if (!inb) { a[0] = 0.f; a[1] = 0.f; a[2] = 0.f; a[3] = 0.f; }
-        }
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          // hi = RN_tf32(a); lo = a - hi is exact in fp32 and |lo| <= 2^-12 |a|, so the tensor core's own
-          // truncation of lo to TF32 loses < 2^-23 |a|: no second rounding needed
-          uint32_t hb;
-          asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(a[k]));
-          hi[j * 4 + k] = hb; lo[j * 4 + k] = __float_as_uint(a[k] - __uint_as_float(hb));
-        }
-      }
-      if (tr) p.dbg[blockIdx.x * 64 + 16 + (ks - 8) * 8 + 1] = clock64();
-      mbar_wait(bar_aempty + 8 * b, bph ^ 1u);      // MMAs that read buffer b have retired
-      if (tr) p.dbg[blockIdx.x * 64 + 16 + (ks - 8) * 8 + 2] = clock64();
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t ta = tmem_base + ((uint32_t)(q * 32) << 16) + acc_cols + (uint32_t)(b * A_BUF_COLS);
-      tmem_st32(ta, hi);
-      tmem_st32(ta + 32, lo);
-      asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      // The raw tile is released only here, after the tcgen05.st that consumed hi / lo: the conversions are
-      // register-only work the compiler is free to sink below an earlier arrive, which would leave the
-      // shared-memory loads outstanding while TMA already refills the slot (seen as rare corrupt rows on
-      // large images once the activation ring had its own, early, release).
-      if (lane == 0) { mbar_arrive(bar_empty + 8 * s); mbar_arrive(bar_afull + 8 * b); }
-      if (tr) p.dbg[blockIdx.x * 64 + 16 + (ks - 8) * 8 + 3] = clock64();
-      f_cc += GROUPS;
-      while (f_cc >= p.cin_chunks) { f_cc -= p.cin_chunks; ++f_tap; }
-      s += GROUPS; if (s >= p.stages_a) { s -= p.stages_a; sph ^= 1u; }
-      b += GROUPS; if (b >= p.nl) { b -= p.nl; bph ^= 1u; }
-    }
-    // ===== epilogue =====
-    const int py = r / TW, px = r % TW;
-    const int iy = oy0 + py, ix = ox0 + px;
-    const bool valid = iy < p.Hy && ix < p.Wx;
-    const int oy = iy * p.out_stride + p.out_off_y, ox = ix * p.out_stride + p.out_off_x;
-    float* dst = p.y + ((((long long)n0 * p.Dout + z0) * p.Hout + oy) * p.Wout + ox) * (long long)p.Cs_out + p.c_off;
-    // Output staging: the finished tile is written to shared memory as BN/32 slabs of [128 pixels][32 channels]
-    // in the 128-byte-swizzled layout of a TMA box (the mirror image of the operand tile), from where (a) one
-    // thread sends it to global memory with cp.async.bulk.tensor stores - coalesced, clipped at the image and
-    // channel bounds by the tensor map, instead of 16-byte stores scattered over 32 lines per instruction
-    // (measured ~1000 cycles per 16-column chunk with eight warps storing) - and (b) the BatchNorm column
-    // sums are read conflict-free.
-    uint8_t* ep = smem_gen;
-    const bool tma_out = p.tma_store != 0 && !(p.dev_flags & 32);
-    const bool want_stats = p.stats && !(p.dev_flags & 16);
-    if (p.dbg && threadIdx.x == 64) p.dbg[blockIdx.x * 64 + 3] = clock64();   // converter done
-    mbar_wait(bar_tmem, 0);
-    if (p.dbg && threadIdx.x == 64) p.dbg[blockIdx.x * 64 + 4] = clock64();   // accumulators complete
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const bool vec_ok = ((p.Cs_out | p.c_off) & 3) == 0;
-    // accumulator slots that were written: per issue stream nacc rotating mains (only min(nk, nacc) of them
-    // used) + one cross-term accumulator
-    const int per = p.nacc + 1;
-    const int n_slots = p.n_issue * per;
-    uint32_t slot_mask = 0;
-    {
-      const int used_m = nk < p.nacc ? nk : p.nacc;
-      for (int a = 0; a < n_slots; ++a) if (a % per < used_m || a % per == p.nacc) slot_mask |= 1u << a;
-    }
-    const uint32_t lane_base = tmem_base + ((uint32_t)(q * 32) << 16);
-    // group cg owns the 32-channel slabs cg, cg + GROUPS, ...: as soon as a slab is staged its TMA store is issued,
-    // so the stores overlap the TMEM read-back of the following slabs
-    const bool storer = tma_out && q == 0 && lane == 0;            // one thread per group
-    for (int c0 = cg * 32; c0 < BN; c0 += ((c0 & 16) ? 32 * GROUPS - 16 : 16)) {
-      float accv[16];
-      const bool stamp = p.dbg && threadIdx.x == 64 && c0 == 16;
-      if (stamp) p.dbg[blockIdx.x * 64 + 8] = clock64();
-      {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) accv[j] = 0.f;
-#pragma unroll 1
-        for (int a0 = 0; a0 < n_slots; a0 += 4) {
-          uint32_t v[4][16];
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            if ((slot_mask >> (a0 + u)) & 1u) {
-              const uint32_t taddr = lane_base + (uint32_t)((a0 + u) * BN + c0);
-              asm volatile(
-                  "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                  : "=r"(v[u][0]), "=r"(v[u][1]), "=r"(v[u][2]), "=r"(v[u][3]), "=r"(v[u][4]), "=r"(v[u][5]), "=r"(v[u][6]),
-                    "=r"(v[u][7]), "=r"(v[u][8]), "=r"(v[u][9]), "=r"(v[u][10]), "=r"(v[u][11]), "=r"(v[u][12]),
-                    "=r"(v[u][13]), "=r"(v[u][14]), "=r"(v[u][15])
-                  : "r"(taddr) : "memory");
-            }
-          }
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            if ((slot_mask >> (a0 + u)) & 1u) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) accv[j] += __uint_as_float(v[u][j]);
-            }
-        }
-      }
-      if (stamp) p.dbg[blockIdx.x * 64 + 9] = clock64();
-      // branches, not selects: the common case (no bias, full chunk, pixel inside the image) executes nothing
-      float* f = accv;
-      if (p.bias) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) if (c0 + j < p.Cout) f[j] += __ldg(p.bias + c0 + j);
-      }
-      if (p.leaky) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) f[j] = f[j] >= 0.f ? f[j] : f[j] * 0.01f;
-      }
-      if (!valid) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) f[j] = 0.f;
-      } else if (c0 + 16 > p.Cout) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) if (c0 + j >= p.Cout) f[j] = 0.f;
-      }
-      if (stamp) p.dbg[blockIdx.x * 64 + 10] = clock64();
-      if (tma_out || want_stats) {
-        uint8_t* rowp = ep + (c0 >> 5) * 16384 + r * 128;
-        const int j0 = (c0 & 31) >> 2;
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj)
-          *reinterpret_cast<float4*>(rowp + (((j0 + jj) ^ (r & 7)) << 4)) = make_float4(f[4 * jj], f[4 * jj + 1], f[4 * jj + 2], f[4 * jj + 3]);
-      }
-      if (stamp) p.dbg[blockIdx.x * 64 + 11] = clock64();
-      if (valid && !tma_out && !(p.dev_flags & 32)) {
-        if (vec_ok && c0 + 16 <= p.Cout) {
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) *reinterpret_cast<float4*>(dst + c0 + j) = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) if (c0 + j < p.Cout) dst[c0 + j] = f[j];
-        }
-      }
-      if (stamp) p.dbg[blockIdx.x * 64 + 12] = clock64();
-      if (tma_out && ((c0 & 16) || c0 + 16 >= BN)) {       // last chunk of this slab
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // staged slab -> visible to the TMA engine
-        if (cg == 0) asm volatile("bar.sync 1, 128;" ::: "memory"); else asm volatile("bar.sync 2, 128;" ::: "memory");
-        const int sl = c0 >> 5;
-        if (storer && sl * 32 < p.Cout) {
-          asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
-                       ::"l"((uint64_t)&tm_y), "r"(smem_base + (uint32_t)(sl * 16384)), "r"(p.c_off + sl * 32), "r"(ox0), "r"(oy0), "r"(z0), "r"(n0)
-                       : "memory");
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
-      }
-    }
-    if (p.dbg && threadIdx.x == 64) p.dbg[blockIdx.x * 64 + 5] = clock64();   // outputs staged / stored
-    if (tma_out || want_stats) {
-      if (want_stats) {
-        asm volatile("bar.sync 3, %0;" ::"n"(128 * GROUPS) : "memory");            // every slab staged (epilogue warps only)
-        // column sums: the 128 * GROUPS epilogue threads split every column into row segments so that all of
-        // them work whatever Cout is (e.g. 64 channels, 128 threads: two 64-row segments per column)
-        const int e = cg * 128 + q * 32 + lane;
-        const int cw = (p.Cout + 31) & ~31;                       // columns rounded up to whole warps
-        const int nseg = cw <= 32 ? (128 * GROUPS) / 32 : cw <= 64 ? (128 * GROUPS) / 64 : cw <= 128 ? GROUPS : 1;
-        const int seg_rows = 128 / nseg;
-        const int co = e % cw, seg = e / cw;
-        if (cw <= 128 ? (seg < nseg && co < p.Cout) : false) {
-          const uint8_t* colp = ep + (co >> 5) * 16384 + (co & 3) * 4;
-          const int jc = (co & 31) >> 2;
-          float s1 = 0.f, s2 = 0.f, t1 = 0.f, t2 = 0.f;
-#pragma unroll 4
-          for (int rr = seg * seg_rows; rr < (seg + 1) * seg_rows; rr += 2) {
-            const float x0 = *reinterpret_cast<const float*>(colp + rr * 128 + ((jc ^ (rr & 7)) << 4));
-            const float x1 = *reinterpret_cast<const float*>(colp + (rr + 1) * 128 + ((jc ^ ((rr + 1) & 7)) << 4));
-            s1 += x0; s2 = fmaf(x0, x0, s2);
-            t1 += x1; t2 = fmaf(x1, x1, t2);
-          }
-          atomicAdd(p.stats + co, (double)(s1 + t1));
-          atomicAdd(p.stats + p.Cout + co, (double)(s2 + t2));
-        }
-      }
-      if (storer) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // shared memory must outlive the store's reads
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols) : "memory");
-  }
-  if (p.dbg && threadIdx.x == 32) {
-    unsigned smid; asm("mov.u32 %0, %%smid;" : "=r"(smid));
-    p.dbg[blockIdx.x * 64 + 6] = clock64(); p.dbg[blockIdx.x * 64 + 7] = smid;
-  }
-}
-
-
-// ---------------------------------------------------------------------------------------------
-// Development probe: raw tcgen05.mma issue / execution rate from resident shared-memory operands.
-// pattern 0: every MMA accumulates into the same columns; 1: destinations alternate over `nd`
-// accumulators per MMA; 2: groups of `grp` consecutive MMAs per destination. K slices cycle over the
-// four 32-byte slices of one 128-byte-swizzled tile. out[0] = cycles from first issue to completion.
-// ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 1)
-mma_probe_kernel(int BN, int n_mma, int pattern, int nd, int grp, int two_warps, long long* out) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
-  const uint32_t a_addr = smem_base, b_addr = smem_base + A_TILE_BYTES;
-  const uint32_t bar = smem_base + A_TILE_BYTES + 256 * 128;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem_gen + A_TILE_BYTES + 256 * 128 + 64);
-  const int warp = uniform_warp_idx(), lane = threadIdx.x % 32;
-  for (int i = threadIdx.x; i < (A_TILE_BYTES + 256 * 128) / 4; i += blockDim.x) reinterpret_cast<float*>(smem_gen)[i] = 1.0f;
-  if (threadIdx.x == 0) { mbar_init(bar, two_warps ? 2 : 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((128u >> 4) << 24);
-  long long t0 = 0;
-  if (pattern < 10 && (warp == 1 || (two_warps && warp == 2))) {
-    const int w = warp == 1 ? 0 : 1;
-    t0 = clock64();
-    if (pattern == 3) {          // lean issue stream: one elect per 12 MMAs, immediate descriptor advance
-      const uint32_t la = desc_lo(a_addr), lb = desc_lo(b_addr);
-      const uint32_t d0 = tmem_base + (uint32_t)(w * nd * BN);
-      for (int i = 0; i < n_mma; i += 12) {
-        if (elect_one()) {
-#pragma unroll
-          for (int j = 0; j < 12; ++j)
-            umma_tf32_raw(d0 + (uint32_t)((nd > 1 && (j % 3) != 2) ? BN : 0), desc_of(la + 2 * (j & 3)), desc_of(lb + 2 * (j & 3)), idesc, (i + j) >= 3 ? 1u : 0u);
-        }
-        __syncwarp();
-      }
-    } else if (pattern == 4) {   // lean TS stream: A operand from TMEM columns 384.. (contents irrelevant for timing)
-      const uint32_t lb = desc_lo(b_addr);
-      const uint32_t d0 = tmem_base + (uint32_t)(w * nd * BN), ta = tmem_base + 384u;
-      for (int i = 0; i < n_mma; i += 12) {
-        if (elect_one()) {
-#pragma unroll
-          for (int j = 0; j < 12; ++j)
-            umma_tf32_ts_raw(d0 + (uint32_t)((nd > 1 && (j % 3) != 2) ? BN : 0), ta + 8 * (j & 3) + 32 * ((j % 3) == 0), desc_of(lb + 2 * (j & 3)), idesc,
-                             (i + j) >= 3 ? 1u : 0u);
-        }
-        __syncwarp();
-      }
-    } else
-    for (int i = 0; i < n_mma; ++i) {
-      int d;
-      if (pattern == 0) d = 0; else if (pattern == 1) d = i % nd; else d = (i / grp) % nd;
-      d += w * nd;
-      const uint64_t ad = umma_desc_sw128(a_addr + (i & 3) * 32);
-      const uint64_t bd = umma_desc_sw128(b_addr + (i & 3) * 32);
-      umma_tf32(tmem_base + (uint32_t)(d * BN), ad, bd, idesc, i >= nd ? 1u : 0u);
-    }
-    umma_commit(bar);
-    const long long t1 = clock64();
-    mbar_wait(bar, 0);
-    const long long t2 = clock64();
-    if (lane == 0 && w == 0) { out[0] = t2 - t0; out[1] = t1 - t0; }
-  }
-  if (pattern >= 10) {
-    // TMEM read-back probe: every warp reads its 32 lanes, n_mma loads of 16 / 32 / 64 columns, one wait each
-    // (pattern 10/11/12) or one wait at the end (pattern 13: x16, 14: x32)
-    __syncthreads();
-    const uint32_t lane_base = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-    float acc = 0.f;
-    const long long a0 = clock64();
-    for (int i = 0; i < n_mma; ++i) {
-      const uint32_t col = (uint32_t)((i * 64) & 255);
-      if (pattern == 10 || pattern == 13) {
-        uint32_t v[16];
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                     : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-                       "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]) : "r"(lane_base + col) : "memory");
-        if (pattern == 10) asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int j = 0; j < 16; ++j) acc += __uint_as_float(v[j]);
-      } else {
-        uint32_t v[32];
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                     : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-                       "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-                       "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-                       "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31]) : "r"(lane_base + col) : "memory");
-        if (pattern == 11) asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc += __uint_as_float(v[j]);
-      }
-    }
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-    const long long a1 = clock64();
-    if (threadIdx.x == 0) { out[0] = a1 - a0; out[1] = (long long)acc; }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
+__device__ __forceinline__ float rn_tf32(float a) {
+  uint32_t b;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(b) : "f"(a));
+  return __uint_as_float(b);
 }
 
 // x -> hi = RN_tf32(x), lo = RN_tf32(x - hi)
@@ -955,15 +37,34 @@ split_tf32_kernel(const float4* __restrict__ x, long long n4, float4* __restrict
   float a[4] = {v.x, v.y, v.z, v.w}, h[4], l[4];
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
-    uint32_t hb, lb;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(a[k]));
-    h[k] = __uint_as_float(hb);
-    float d = a[k] - h[k];
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lb) : "f"(d));
-    l[k] = __uint_as_float(lb);
+    h[k] = rn_tf32(a[k]);
+    l[k] = rn_tf32(a[k] - h[k]);
   }
   hi[i] = make_float4(h[0], h[1], h[2], h[3]);
   lo[i] = make_float4(l[0], l[1], l[2], l[3]);
+}
+
+// channels-last x [pos][Cs] -> TF32 pair [pos][Cin_pad] of [relu](x * scale + shift) (scale == null: x itself); channels
+// >= C are zero
+__global__ void __launch_bounds__(256)
+split_tf32_bn_kernel(const float* __restrict__ x, long long n_pos, int Cs, int Cin_pad, int C, const float* __restrict__ scale,
+                     const float* __restrict__ shift, int relu, float* __restrict__ hi, float* __restrict__ lo) {
+  const long long n = n_pos * Cin_pad;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long pos = i / Cin_pad;
+    const int c = (int)(i - pos * Cin_pad);
+    float v = 0.f;
+    if (c < C) {
+      v = x[pos * Cs + c];
+      if (scale) {
+        v = fmaf(v, scale[c], shift[c]);
+        if (relu) v = fmaxf(v, 0.f);
+      }
+    }
+    const float h = rn_tf32(v);
+    hi[i] = h;
+    lo[i] = rn_tf32(v - h);
+  }
 }
 
 // PyTorch weight -> K-major packed hi / lo [tap][Cout_pad][Cin_pad]
@@ -977,231 +78,91 @@ __global__ void pack_weight_tc_kernel(const float* __restrict__ w, int kind, int
   int t = (int)(i / ((long long)Cout_pad * Cin_pad));
   float v = 0.f;
   if (co < Cout && ci < Cin) v = kind == 0 ? w[((long long)co * Cin + ci) * taps + t] : w[((long long)ci * Cout + co) * taps + t];
-  uint32_t hb, lb;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(v));
-  float h = __uint_as_float(hb);
-  float d = v - h;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lb) : "f"(d));
-  hi[i] = h; lo[i] = __uint_as_float(lb);
+  const float h = rn_tf32(v);
+  hi[i] = h; lo[i] = rn_tf32(v - h);
 }
 
-int g_force_nacc = 0;
-int g_force_stages = 0;     // development knobs (nrgbd_conv_tc_set_dev)
-long long* g_dbg = nullptr;
-// Development knobs (nrgbd_conv_tc_set_dev, include/nrgbd_dev.h), all off unless a tool sets them:
-//   1    v1: plain 1xTF32 (hi*hi only)            2    never two CTAs per SM        4    v1: single issue stream
-//   8    v2: two issue streams                    16   skip the BN statistics       32   skip the output stores
-//   64   v2: one converter / epilogue group       128  v2: two TMEM operand buffers 2048 v2: direct stores instead of TMA stores
-//   4096 v2: three-MMA K-slices with rotating main accumulators instead of the concatenated two-MMA form
-int g_dev_flags = 0;
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-  }
-  return fn;
+WgConv tf32_conv(const float* x_hi, const float* x_lo, int N, int Din, int Hin, int Win, int Cin_pad, int Cs_in, const float* w_hi,
+                 const float* w_lo, int n_wslices, const float* bias, int Cout, int Cout_pad, float* y, int Cs_out, int c_off, int leaky,
+                 double* stats) {
+  WgConv c{};
+  c.tf32 = 1;
+  c.x_hi = x_hi; c.x_lo = x_lo; c.N = N; c.Din = Din; c.Hin = Hin; c.Win = Win; c.Cin_pad = Cin_pad; c.Cs_in = Cs_in;
+  c.w_hi = w_hi; c.w_lo = w_lo; c.w_tap_stride = (long long)Cout_pad * Cin_pad; c.n_wslices = n_wslices; c.Cout_pad = Cout_pad;
+  c.bias = bias; c.stats = stats; c.y = y;
+  c.Cout = Cout; c.Cs_out = Cs_out; c.c_off = c_off; c.leaky = leaky;
+  return c;
 }
 
-// cuTensorMapEncodeTiled costs a few microseconds; a frame issues ~200 of them with a small set of
-// recurring (pointer, shape) combinations (the engine's buffer pool hands out the same blocks every
-// frame), so encoded maps are memoised per thread.
-struct MapKey { const void* p; int a, b, c, d, e, f, g; };
-struct MapEnt { MapKey k; CUtensorMap m; };
-inline bool same_key(const MapKey& x, const MapKey& y) {
-  return x.p == y.p && x.a == y.a && x.b == y.b && x.c == y.c && x.d == y.d && x.e == y.e && x.f == y.f && x.g == y.g;
-}
-thread_local MapEnt g_map_cache[512];
-thread_local int g_map_cache_n = 0;
-inline unsigned key_slot(const MapKey& k) {
-  unsigned long long h = (unsigned long long)k.p * 0x9E3779B97F4A7C15ull;
-  h ^= (unsigned long long)(k.a * 73856093u) ^ (unsigned long long)(k.b * 19349663u) ^ (unsigned long long)(k.c * 83492791u) ^
-       (unsigned long long)(k.d * 2654435761u) ^ (unsigned long long)(k.e * 40503u) ^ (unsigned long long)(k.f * 2246822519u) ^ (unsigned long long)(k.g * 3266489917u);
-  return (unsigned)(h >> 40) & 511u;
+int conv_tc_impl(const float* x_hi, const float* x_lo, int N, int Din, int Hin, int Win, int Cin_pad, int Cs_in, const float* w_hi,
+                 const float* w_lo, const float* bias, int Cout, int Cout_pad, int kd, int kh, int kw, int stride, int pad, int dilation,
+                 float* y, int Hout, int Wout, int Cs_out, int c_off, int leaky, double* stats, cudaStream_t st) {
+  WgConv c = tf32_conv(x_hi, x_lo, N, Din, Hin, Win, Cin_pad, Cs_in, w_hi, w_lo, kd * kh * kw, bias, Cout, Cout_pad, y, Cs_out, c_off, leaky, stats);
+  c.Dout = Din; c.Hout = Hout; c.Wout = Wout; c.out_stride = 1;
+  c.Hy = Hout; c.Wx = Wout; c.in_stride = stride; c.n_kz = kd; c.n_tap = kh * kw;
+  for (int a = 0; a < kd; ++a) c.dz[a] = (signed char)(a - kd / 2);
+  int t = 0;
+  for (int b = 0; b < kh; ++b)
+    for (int e = 0; e < kw; ++e) { c.dy[t] = (signed char)(b * dilation - pad); c.dx[t] = (signed char)(e * dilation - pad); ++t; }
+  for (int a = 0; a < kd * kh * kw; ++a) c.wsel[a] = (unsigned char)a;
+  return conv_wgmma(c, st);
 }
 
-int encode_act_map_uncached(CUtensorMap* tm, const float* x, int N, int D, int H, int W, int Cin_pad, int Cs, int stride);
-int encode_act_map(CUtensorMap* tm, const float* x, int N, int D, int H, int W, int Cin_pad, int Cs, int stride) {
-  MapKey k{x, N, D, H, W, Cin_pad, Cs, stride};
-  MapEnt& e = g_map_cache[key_slot(k)];
-  if (same_key(e.k, k) && e.k.p) { *tm = e.m; return NRGBD_OK; }
-  int rc = encode_act_map_uncached(tm, x, N, D, H, W, Cin_pad, Cs, stride);
-  if (rc == NRGBD_OK) { e.k = k; e.m = *tm; }
-  return rc;
-}
-
-int encode_act_map_uncached(CUtensorMap* tm, const float* x, int N, int D, int H, int W, int Cin_pad, int Cs, int stride) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) { nrgbd_set_error("cuTensorMapEncodeTiled unavailable"); return NRGBD_ERR_CUDA; }
-  cuuint64_t dims[5] = {(cuuint64_t)Cin_pad, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)D, (cuuint64_t)N};
-  cuuint64_t strides[4] = {(cuuint64_t)Cs * 4, (cuuint64_t)W * Cs * 4, (cuuint64_t)H * W * Cs * 4, (cuuint64_t)D * H * W * Cs * 4};
-  cuuint32_t box[5] = {(cuuint32_t)BK, (cuuint32_t)(TW * stride), (cuuint32_t)(TH * stride), 1, 1};
-  cuuint32_t estr[5] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, const_cast<float*>(x), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { nrgbd_set_error("cuTensorMapEncodeTiled(activation) failed: %d", (int)r); return NRGBD_ERR_CUDA; }
+// nn.ConvTranspose2d(kernel 4, stride 2, padding 1) as four output-parity classes of 2x2-tap convolutions
+int conv_transpose_tc_impl(const float* x_hi, const float* x_lo, int N, int Hin, int Win, int Cin_pad, int Cs_in, const float* w_hi,
+                           const float* w_lo, const float* bias, int Cout, int Cout_pad, float* y, int Cs_out, int c_off, int leaky,
+                           cudaStream_t st) {
+  const int kys[2][2] = {{1, 3}, {0, 2}};
+  const int dys[2][2] = {{0, -1}, {1, 0}};
+  for (int py = 0; py < 2; ++py)
+    for (int px = 0; px < 2; ++px) {
+      WgConv c = tf32_conv(x_hi, x_lo, N, 1, Hin, Win, Cin_pad, Cs_in, w_hi, w_lo, 16, bias, Cout, Cout_pad, y, Cs_out, c_off, leaky, nullptr);
+      c.Dout = 1; c.Hout = 2 * Hin; c.Wout = 2 * Win; c.out_stride = 2; c.out_off_y = py; c.out_off_x = px;
+      c.Hy = Hin; c.Wx = Win; c.in_stride = 1; c.n_kz = 1; c.n_tap = 4;
+      int t = 0;
+      for (int a = 0; a < 2; ++a)
+        for (int b = 0; b < 2; ++b) {
+          c.dy[t] = (signed char)dys[py][a]; c.dx[t] = (signed char)dys[px][b];
+          c.wsel[t] = (unsigned char)(kys[py][a] * 4 + kys[px][b]); ++t;
+        }
+      int rc = conv_wgmma(c, st);
+      if (rc != NRGBD_OK) return rc;
+    }
   return NRGBD_OK;
 }
 
-int encode_w_map_uncached(CUtensorMap* tm, const float* w, int taps, int Cout_pad, int Cin_pad);
-int encode_w_map(CUtensorMap* tm, const float* w, int taps, int Cout_pad, int Cin_pad) {
-  MapKey k{w, taps, Cout_pad, Cin_pad, -1, -1, -1, -1};
-  MapEnt& e = g_map_cache[key_slot(k)];
-  if (same_key(e.k, k) && e.k.p) { *tm = e.m; return NRGBD_OK; }
-  int rc = encode_w_map_uncached(tm, w, taps, Cout_pad, Cin_pad);
-  if (rc == NRGBD_OK) { e.k = k; e.m = *tm; }
-  return rc;
-}
+// Stream-ordered scratch for the split of raw activations: TF32 pair [n_pos][Cin_pad] (+ scale / shift of a fused input
+// BatchNorm), freed on the same stream after the GEMM.
+struct SplitScratch {
+  float *hi = nullptr, *lo = nullptr, *scale = nullptr, *shift = nullptr;
+  void* mem = nullptr;
+};
 
-int encode_w_map_uncached(CUtensorMap* tm, const float* w, int taps, int Cout_pad, int Cin_pad) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) { nrgbd_set_error("cuTensorMapEncodeTiled unavailable"); return NRGBD_ERR_CUDA; }
-  cuuint64_t dims[3] = {(cuuint64_t)Cin_pad, (cuuint64_t)Cout_pad, (cuuint64_t)taps};
-  cuuint64_t strides[2] = {(cuuint64_t)Cin_pad * 4, (cuuint64_t)Cout_pad * Cin_pad * 4};
-  cuuint32_t box[3] = {(cuuint32_t)BK, (cuuint32_t)Cout_pad, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(w), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { nrgbd_set_error("cuTensorMapEncodeTiled(weights) failed: %d", (int)r); return NRGBD_ERR_CUDA; }
-  return NRGBD_OK;
-}
-
-int launch_tc(const float* x_hi, const float* x_lo, int N, int Din, int Hin, int Win, int Cin_pad, int Cs_in, const float* w_hi,
-              const float* w_lo, int n_wslices, TcParams& p, cudaStream_t st) {
-  CUtensorMap ta_hi, ta_lo, tb_hi, tb_lo;
-  int rc = encode_act_map(&ta_hi, x_hi, N, Din, Hin, Win, Cin_pad, Cs_in, p.in_stride);
-  if (rc == NRGBD_OK) rc = encode_act_map(&ta_lo, x_lo, N, Din, Hin, Win, Cin_pad, Cs_in, p.in_stride);
-  if (rc == NRGBD_OK) rc = encode_w_map(&tb_hi, w_hi, n_wslices, p.Cout_pad, Cin_pad);
-  if (rc == NRGBD_OK) rc = encode_w_map(&tb_lo, w_lo, n_wslices, p.Cout_pad, Cin_pad);
-  if (rc != NRGBD_OK) return rc;
-  p.cin_chunks = Cin_pad / BK;
-  p.tiles_x = ceil_div(p.Wx, TW); p.tiles_y = ceil_div(p.Hy, TH);
-  // Resource plan. The per-K-step time does not depend on the pipeline depth (measured), but a tile's
-  // prologue + epilogue are ~35 % of its lifetime: when Cout_pad <= 64 use 2 stages and 256 TMEM
-  // columns so that two CTAs share an SM and one's epilogue overlaps the other's main loop.
-  const bool two_per_sm = p.Cout_pad <= 64 && !(g_dev_flags & 2);
-  const int tmem_budget = two_per_sm ? 256 : 512;
-  int n_issue = (!(g_dev_flags & 4) && 4 * p.Cout_pad <= tmem_budget) ? 2 : 1;   // v1: two streams measured 35 % faster
-  int nm = tmem_budget / (n_issue * p.Cout_pad) - 1;
-  if (nm > 4) nm = 4;
-  if (nm < 1) { nrgbd_set_error("conv_tc: accumulators do not fit TMEM"); return NRGBD_ERR_UNSUPPORTED; }
-  if (g_force_nacc > 0 && g_force_nacc < nm) nm = g_force_nacc;
-  p.n_issue = n_issue; p.nacc = nm; p.nl = 1;
-  int cols = 32; while (cols < n_issue * (nm + 1) * p.Cout_pad) cols <<= 1;
-  p.tmem_cols = cols;
-  const size_t stage = 2 * (size_t)A_TILE_BYTES + 2 * (size_t)p.Cout_pad * BK * 4;
-  int stages = two_per_sm ? 2 : (int)((220 * 1024 - 2048) / stage);
-  if (stages > 3) stages = 3;
-  if (g_force_stages > 0 && g_force_stages < stages) stages = g_force_stages;
-  p.dev_flags = g_dev_flags; p.dbg = g_dbg;
-  if (stages < 2) { nrgbd_set_error("conv_tc: Cout too large for the shared-memory pipeline"); return NRGBD_ERR_UNSUPPORTED; }
-  size_t ep_bytes = (size_t)128 * (p.Cout_pad + 1) * 4;
-  p.stages = stages;
-  size_t smem = (size_t)stages * stage + 1024 /*align*/ + 256 /*barriers*/;
-  if (stages * stage < ep_bytes) smem = ep_bytes + 1024 + 256;
-  static size_t configured = 0;
-  if (smem > configured) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) { nrgbd_set_error("conv_tc: cannot opt in to %zu bytes of shared memory: %s", smem, cudaGetErrorString(e)); return NRGBD_ERR_CUDA; }
-    configured = smem;
-  }
-  const long long tiles = (long long)N * p.Dz * p.tiles_x * p.tiles_y;
-  conv_tc_kernel<<<(unsigned)tiles, NUM_THREADS, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, p);
-  return NRGBD_OK;
-}
-
-// v2 launcher: raw activations, in-kernel split. Requires (nacc+1)*Cout_pad + 128 TMEM columns <= 512.
-int launch_tc2(const float* x, int N, int Din, int Hin, int Win, int Cin_pad, int Cs_in, const float* w_hi, const float* w_lo,
-               int n_wslices, TcParams& p, cudaStream_t st) {
-  CUtensorMap ta, tb_hi, tb_lo;
-  int rc = encode_act_map(&ta, x, N, Din, Hin, Win, Cin_pad, Cs_in, p.in_stride);
-  if (rc == NRGBD_OK) rc = encode_w_map(&tb_hi, w_hi, n_wslices, p.Cout_pad, Cin_pad);
-  if (rc == NRGBD_OK) rc = encode_w_map(&tb_lo, w_lo, n_wslices, p.Cout_pad, Cin_pad);
-  if (rc != NRGBD_OK) return rc;
-  p.cin_chunks = Cin_pad / BK;
-  p.tiles_x = ceil_div(p.Wx, TW); p.tiles_y = ceil_div(p.Hy, TH);
-  // Resource plan: Cout_pad <= 64 -> two CTAs per SM (one issue stream, 2 accumulators + 2 operand
-  // buffers = 256 TMEM columns, 3 x 32 KB stages); otherwise one CTA per SM.
-  const bool two_per_sm = p.Cout_pad <= 64 && !(g_dev_flags & 2);
-  // Operand buffers: the chain "buffer freed -> tcgen05.st of the next operands -> MMAs issued -> MMAs retired"
-  // is ~1100 cycles per K-step, longer than the 768-cycle tensor time of a K-step at N = 128, so with two
-  // buffers the tensor pipe idles a third of the time. One CTA per SM: four buffers when two accumulators
-  // (one main + the cross terms) still fit beside them.
-  int nbuf = (!two_per_sm && !(g_dev_flags & 128) && 2 * p.Cout_pad + 4 * A_BUF_COLS <= 512) ? 4 : 2;
-  const int tmem_budget = (two_per_sm ? 256 : 512) - nbuf * A_BUF_COLS;
-  int n_issue = ((g_dev_flags & 8) && 4 * p.Cout_pad <= tmem_budget) ? 2 : 1;
-  int nm = tmem_budget / (n_issue * p.Cout_pad) - 1;
-  if (nm > 4) nm = 4;
-  if (nm > 1 && n_issue == 1 && !(g_dev_flags & 4096)) nm = 1;     // one main accumulator: the two-MMA (concatenated) K-slice form
-  if (nm < 1) { nrgbd_set_error("conv_tc2: Cout too large for the TMEM operand buffers"); return NRGBD_ERR_UNSUPPORTED; }
-  if (g_force_nacc > 0 && g_force_nacc < nm) nm = g_force_nacc;
-  p.n_issue = n_issue; p.nacc = nm; p.nl = nbuf;
-  int cols = 32; while (cols < n_issue * (nm + 1) * p.Cout_pad + nbuf * A_BUF_COLS) cols <<= 1;
-  p.tmem_cols = cols;
-  // Ring depths (see the kernel): the weight ring gets everything the activation ring leaves. Budget per CTA:
-  // the 227 KB opt-in maximum, or half of the SM's 228 KB minus the 1 KB per-CTA reservation for two CTAs.
-  const size_t b_slot = 2 * (size_t)p.Cout_pad * BK * 4;
-  const size_t tbl = p.in_stats ? (size_t)2 * Cin_pad * 4 : 0;         // fused input BatchNorm: scale / shift tables
-  const size_t budget = (two_per_sm ? 115712 : 232448) - 512 - tbl;    // 512 bytes of barriers
-  int stages_a = 4, stages = (int)((budget - 4 * (size_t)A_TILE_BYTES) / b_slot);
-  if (stages < 5) { stages_a = 3; stages = (int)((budget - 3 * (size_t)A_TILE_BYTES) / b_slot); }
-  if (stages > 8) stages = 8;
-  if (g_force_stages > 0 && g_force_stages < stages) { stages = g_force_stages; if (stages_a > stages) stages_a = stages; }
-  p.dev_flags = g_dev_flags; p.dbg = g_dbg;
-  if (stages < 2) { nrgbd_set_error("conv_tc2: Cout too large for the shared-memory pipeline"); return NRGBD_ERR_UNSUPPORTED; }
-  p.stages = stages; p.stages_a = stages_a;
-  size_t ring = (size_t)stages_a * A_TILE_BYTES + (size_t)stages * b_slot;
-  const size_t ep_bytes = (size_t)((p.Cout_pad + 31) / 32) * 16384;    // output staging slabs alias the rings
-  if (ring < ep_bytes) ring = ep_bytes;
-  const size_t smem = ring + 512 + tbl;
-  p.in_H = Hin; p.in_W = Win; p.in_D = Din;
-  // TMA tensor store of the output tile: stride-1 outputs whose channel window starts on a 16-byte boundary
-  CUtensorMap ty = ta;
-  p.tma_store = 0;
-  if (p.out_stride == 1 && p.out_off_y == 0 && p.out_off_x == 0 && p.Cs_out % 4 == 0 && p.c_off % 4 == 0 &&
-      ((uintptr_t)p.y & 15) == 0 && !(g_dev_flags & 2048)) {
-    rc = encode_act_map(&ty, p.y, N, p.Dout, p.Hout, p.Wout, p.c_off + p.Cout, p.Cs_out, 1);
+int split_raw(const float* x, long long n_pos, int Cs_in, int Cin_pad, const nrgbd_bn_input* in_bn, SplitScratch& s, cudaStream_t st) {
+  const long long n = n_pos * Cin_pad;
+  const size_t bytes = (size_t)n * 8 + (in_bn ? (size_t)Cin_pad * 8 : 0);
+  NRGBD_CUDA_CHECK(cudaMallocAsync(&s.mem, bytes, st));
+  s.hi = reinterpret_cast<float*>(s.mem); s.lo = s.hi + n;
+  int C = Cin_pad, relu = 0;
+  if (in_bn) {
+    s.scale = s.lo + n; s.shift = s.scale + Cin_pad;
+    C = in_bn->C; relu = in_bn->relu;
+    const bool run = in_bn->running_mean && in_bn->running_var;
+    int rc = nrgbd_bn_finalize(in_bn->stats, C, in_bn->count, in_bn->gamma, in_bn->beta, in_bn->eps, s.scale, s.shift,
+                               run ? in_bn->running_mean : nullptr, run ? in_bn->running_var : nullptr, in_bn->momentum, st);
     if (rc != NRGBD_OK) return rc;
-    p.tma_store = 1;
   }
-  const bool two_groups = !two_per_sm && !(g_dev_flags & 64);
-  static size_t configured[2] = {0, 0};
-  if (smem > configured[two_groups]) {
-    cudaError_t e = two_groups ? cudaFuncSetAttribute(conv_tc2_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                               : cudaFuncSetAttribute(conv_tc2_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) { nrgbd_set_error("conv_tc2: cannot opt in to %zu bytes of shared memory: %s", smem, cudaGetErrorString(e)); return NRGBD_ERR_CUDA; }
-    configured[two_groups] = smem;
-  }
-  const long long tiles = (long long)N * p.Dz * p.tiles_x * p.tiles_y;
-  if (two_groups) conv_tc2_kernel<2><<<(unsigned)tiles, NUM_THREADS2_G2, smem, st>>>(ta, tb_hi, tb_lo, ty, p);
-  else conv_tc2_kernel<1><<<(unsigned)tiles, NUM_THREADS2, smem, st>>>(ta, tb_hi, tb_lo, ty, p);
+  long long blocks = (n + 255) / 256;
+  if (blocks > nrgbd_sm_count() * 16ll) blocks = nrgbd_sm_count() * 16ll;
+  split_tf32_bn_kernel<<<(unsigned)blocks, 256, 0, st>>>(x, n_pos, Cs_in, Cin_pad, C, s.scale, s.shift, relu, s.hi, s.lo);
+  NRGBD_COUNT(1);
+  NRGBD_LAUNCH_CHECK();
   return NRGBD_OK;
 }
 
 }  // namespace
 
 extern "C" {
-
-void nrgbd_conv_tc_set_nacc(int n) { g_force_nacc = n; }
-void nrgbd_conv_tc_set_dev(int stages, int flags) { g_force_stages = stages; g_dev_flags = flags; }
-void nrgbd_conv_tc_set_debug_buffer(long long* buf) { g_dbg = buf; }
-
-// Development probe (see mma_probe_kernel). out: 2 int64 on the device (total cycles, issue cycles).
-int nrgbd_mma_probe(int BN, int n_mma, int pattern, int nd, int grp, int two_warps, int n_ctas, long long* out, cudaStream_t st) {
-  NRGBD_REQUIRE(out && BN >= 16 && BN <= 256 && BN % 16 == 0 && nd >= 1 && (two_warps ? 2 : 1) * nd * BN <= 512 && grp >= 1, "bad arguments");
-  size_t smem = A_TILE_BYTES + 256 * 128 + 1024 + 256;
-  cudaFuncSetAttribute(mma_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  mma_probe_kernel<<<n_ctas, 128, smem, st>>>(BN, n_mma, pattern, nd, grp, two_warps, out);
-  NRGBD_LAUNCH_CHECK();
-  return NRGBD_OK;
-}
 
 // Whether the tensor-core path can run a convolution with these channel counts.
 int nrgbd_conv_tc_supported(int Cin_pad, int Cout_pad) {
@@ -1238,24 +199,11 @@ int nrgbd_conv_nhwc_tc(const float* x_hi, const float* x_lo, int N, int Din, int
   NRGBD_REQUIRE(x_hi && x_lo && w_hi && w_lo && y, "null pointer");
   NRGBD_REQUIRE(nrgbd_conv_tc_supported(Cin_pad, Cout_pad) && Cin_pad <= Cs_in && Cs_in % 4 == 0 && Cout <= Cout_pad,
                 "channel counts not supported by the tensor-core path");
-  NRGBD_REQUIRE(kd * kh * kw <= MAX_TAPS_TC && stride >= 1 && stride <= 8, "unsupported filter");
+  NRGBD_REQUIRE(kd >= 1 && kd <= 3 && kh * kw <= WG_MAX_TAP2D && stride >= 1 && stride <= 8, "unsupported filter");
   NRGBD_REQUIRE(Hout == (Hin + 2 * pad - dilation * (kh - 1) - 1) / stride + 1 &&
                     Wout == (Win + 2 * pad - dilation * (kw - 1) - 1) / stride + 1, "output extent mismatch");
-  TcParams p{};
-  p.y = y; p.bias = bias; p.stats = stats;
-  p.N = N; p.Dz = Din; p.Hy = Hout; p.Wx = Wout;
-  p.in_stride = stride; p.Cout = Cout; p.Cout_pad = Cout_pad;
-  p.Dout = Din; p.Hout = Hout; p.Wout = Wout; p.Cs_out = Cs_out; p.c_off = c_off;
-  p.out_stride = 1; p.out_off_y = 0; p.out_off_x = 0; p.leaky = leaky;
-  int t = 0;
-  for (int a = 0; a < kd; ++a)
-    for (int b = 0; b < kh; ++b)
-      for (int c = 0; c < kw; ++c) {
-        p.dz[t] = (signed char)(a - kd / 2); p.dy[t] = (signed char)(b * dilation - pad); p.dx[t] = (signed char)(c * dilation - pad);
-        p.wsel[t] = (unsigned char)t; ++t;
-      }
-  p.n_taps = t;
-  int rc = launch_tc(x_hi, x_lo, N, Din, Hin, Win, Cin_pad, Cs_in, w_hi, w_lo, t, p, st);
+  int rc = conv_tc_impl(x_hi, x_lo, N, Din, Hin, Win, Cin_pad, Cs_in, w_hi, w_lo, bias, Cout, Cout_pad, kd, kh, kw, stride, pad, dilation, y,
+                        Hout, Wout, Cs_out, c_off, leaky, stats, st);
   if (rc != NRGBD_OK) return rc;
   NRGBD_COUNT(1);
   NRGBD_LAUNCH_CHECK();
@@ -1269,32 +217,14 @@ int nrgbd_conv_transpose2d_k4s2_nhwc_tc(const float* x_hi, const float* x_lo, in
   NRGBD_REQUIRE(x_hi && x_lo && w_hi && w_lo && y, "null pointer");
   NRGBD_REQUIRE(nrgbd_conv_tc_supported(Cin_pad, Cout_pad) && Cin_pad <= Cs_in && Cs_in % 4 == 0 && Cout <= Cout_pad,
                 "channel counts not supported by the tensor-core path");
-  const int kys[2][2] = {{1, 3}, {0, 2}};
-  const int dys[2][2] = {{0, -1}, {1, 0}};
-  for (int py = 0; py < 2; ++py)
-    for (int px = 0; px < 2; ++px) {
-      TcParams p{};
-      p.y = y; p.bias = bias; p.stats = nullptr;
-      p.N = N; p.Dz = 1; p.Hy = Hin; p.Wx = Win;
-      p.in_stride = 1; p.Cout = Cout; p.Cout_pad = Cout_pad;
-      p.Dout = 1; p.Hout = 2 * Hin; p.Wout = 2 * Win; p.Cs_out = Cs_out; p.c_off = c_off;
-      p.out_stride = 2; p.out_off_y = py; p.out_off_x = px; p.leaky = leaky;
-      int t = 0;
-      for (int a = 0; a < 2; ++a)
-        for (int b = 0; b < 2; ++b) {
-          p.dz[t] = 0; p.dy[t] = (signed char)dys[py][a]; p.dx[t] = (signed char)dys[px][b];
-          p.wsel[t] = (unsigned char)(kys[py][a] * 4 + kys[px][b]); ++t;
-        }
-      p.n_taps = 4;
-      int rc = launch_tc(x_hi, x_lo, N, 1, Hin, Win, Cin_pad, Cs_in, w_hi, w_lo, 16, p, st);
-      if (rc != NRGBD_OK) return rc;
-    }
+  int rc = conv_transpose_tc_impl(x_hi, x_lo, N, Hin, Win, Cin_pad, Cs_in, w_hi, w_lo, bias, Cout, Cout_pad, y, Cs_out, c_off, leaky, st);
+  if (rc != NRGBD_OK) return rc;
   NRGBD_COUNT(4);
   NRGBD_LAUNCH_CHECK();
   return NRGBD_OK;
 }
 
-// v2 (in-kernel split): raw fp32 activations, TF32-split K-major weights. Cout_pad <= 128.
+// Raw fp32 activations, TF32-split K-major weights. Cout_pad <= 128.
 int nrgbd_conv_tc2_supported(int Cin_pad, int Cout_pad) {
   return (Cin_pad % 32 == 0 && Cin_pad >= 32 && Cout_pad % 16 == 0 && Cout_pad >= 16 && Cout_pad <= 128) ? 1 : 0;
 }
@@ -1306,32 +236,19 @@ static int conv_nhwc_tc2_impl(const float* x, int N, int Din, int Hin, int Win, 
   NRGBD_REQUIRE(x && w_hi && w_lo && y, "null pointer");
   NRGBD_REQUIRE(nrgbd_conv_tc2_supported(Cin_pad, Cout_pad) && Cin_pad <= Cs_in && Cs_in % 4 == 0 && Cout <= Cout_pad,
                 "channel counts not supported by the tensor-core path");
-  NRGBD_REQUIRE(kd * kh * kw <= MAX_TAPS_TC && stride >= 1 && stride <= 8, "unsupported filter");
+  NRGBD_REQUIRE(kd >= 1 && kd <= 3 && kh * kw <= WG_MAX_TAP2D && stride >= 1 && stride <= 8, "unsupported filter");
   NRGBD_REQUIRE(Hout == (Hin + 2 * pad - dilation * (kh - 1) - 1) / stride + 1 &&
                     Wout == (Win + 2 * pad - dilation * (kw - 1) - 1) / stride + 1, "output extent mismatch");
-  TcParams p{};
-  p.y = y; p.bias = bias; p.stats = stats;
-  p.N = N; p.Dz = Din; p.Hy = Hout; p.Wx = Wout;
-  p.in_stride = stride; p.Cout = Cout; p.Cout_pad = Cout_pad;
-  p.Dout = Din; p.Hout = Hout; p.Wout = Wout; p.Cs_out = Cs_out; p.c_off = c_off;
-  p.out_stride = 1; p.out_off_y = 0; p.out_off_x = 0; p.leaky = leaky;
-  p.in_stats = nullptr;
   if (in_bn) {
     NRGBD_REQUIRE(in_bn->stats && in_bn->gamma && in_bn->beta && in_bn->C >= 1 && in_bn->C <= Cin_pad && in_bn->count >= 1 &&
                       in_bn->stats != stats, "bad input BatchNorm descriptor");
-    p.in_stats = in_bn->stats; p.in_count = in_bn->count; p.in_gamma = in_bn->gamma; p.in_beta = in_bn->beta;
-    p.in_run_mean = in_bn->running_mean && in_bn->running_var ? in_bn->running_mean : nullptr; p.in_run_var = in_bn->running_var;
-    p.in_eps = in_bn->eps; p.in_momentum = in_bn->momentum; p.in_relu = in_bn->relu; p.in_C = in_bn->C;
   }
-  int t = 0;
-  for (int a = 0; a < kd; ++a)
-    for (int b = 0; b < kh; ++b)
-      for (int c = 0; c < kw; ++c) {
-        p.dz[t] = (signed char)(a - kd / 2); p.dy[t] = (signed char)(b * dilation - pad); p.dx[t] = (signed char)(c * dilation - pad);
-        p.wsel[t] = (unsigned char)t; ++t;
-      }
-  p.n_taps = t;
-  int rc = launch_tc2(x, N, Din, Hin, Win, Cin_pad, Cs_in, w_hi, w_lo, t, p, st);
+  SplitScratch s;
+  int rc = split_raw(x, (long long)N * Din * Hin * Win, Cs_in, Cin_pad, in_bn, s, st);
+  if (rc == NRGBD_OK)
+    rc = conv_tc_impl(s.hi, s.lo, N, Din, Hin, Win, Cin_pad, Cin_pad, w_hi, w_lo, bias, Cout, Cout_pad, kd, kh, kw, stride, pad, dilation, y, Hout,
+                      Wout, Cs_out, c_off, leaky, stats, st);
+  if (s.mem) NRGBD_CUDA_CHECK(cudaFreeAsync(s.mem, st));
   if (rc != NRGBD_OK) return rc;
   NRGBD_COUNT(1);
   NRGBD_LAUNCH_CHECK();
@@ -1346,7 +263,7 @@ int nrgbd_conv_nhwc_tc2(const float* x, int N, int Din, int Hin, int Win, int Ci
 }
 
 // Same convolution of [relu](BatchNorm_train(x)) where x is the RAW output of the producing conv and in_bn carries its
-// per-channel sums: the normalisation is applied while the operands are converted (no separate pass over x).
+// per-channel sums: the normalisation is applied in the operand split (no separate pass over x).
 int nrgbd_conv_nhwc_tc2_bn_in(const float* x, int N, int Din, int Hin, int Win, int Cin_pad, int Cs_in, const float* w_hi,
                               const float* w_lo, const float* bias, int Cout, int Cout_pad, int kd, int kh, int kw, int stride, int pad,
                               int dilation, float* y, int Hout, int Wout, int Cs_out, int c_off, int leaky, double* stats,
@@ -1362,26 +279,12 @@ int nrgbd_conv_transpose2d_k4s2_nhwc_tc2(const float* x, int N, int Hin, int Win
   NRGBD_REQUIRE(x && w_hi && w_lo && y, "null pointer");
   NRGBD_REQUIRE(nrgbd_conv_tc2_supported(Cin_pad, Cout_pad) && Cin_pad <= Cs_in && Cs_in % 4 == 0 && Cout <= Cout_pad,
                 "channel counts not supported by the tensor-core path");
-  const int kys[2][2] = {{1, 3}, {0, 2}};
-  const int dys[2][2] = {{0, -1}, {1, 0}};
-  for (int py = 0; py < 2; ++py)
-    for (int px = 0; px < 2; ++px) {
-      TcParams p{};
-      p.y = y; p.bias = bias; p.stats = nullptr;
-      p.N = N; p.Dz = 1; p.Hy = Hin; p.Wx = Win;
-      p.in_stride = 1; p.Cout = Cout; p.Cout_pad = Cout_pad;
-      p.Dout = 1; p.Hout = 2 * Hin; p.Wout = 2 * Win; p.Cs_out = Cs_out; p.c_off = c_off;
-      p.out_stride = 2; p.out_off_y = py; p.out_off_x = px; p.leaky = leaky;
-      int t = 0;
-      for (int a = 0; a < 2; ++a)
-        for (int b = 0; b < 2; ++b) {
-          p.dz[t] = 0; p.dy[t] = (signed char)dys[py][a]; p.dx[t] = (signed char)dys[px][b];
-          p.wsel[t] = (unsigned char)(kys[py][a] * 4 + kys[px][b]); ++t;
-        }
-      p.n_taps = 4;
-      int rc = launch_tc2(x, N, 1, Hin, Win, Cin_pad, Cs_in, w_hi, w_lo, 16, p, st);
-      if (rc != NRGBD_OK) return rc;
-    }
+  SplitScratch s;
+  int rc = split_raw(x, (long long)N * Hin * Win, Cs_in, Cin_pad, nullptr, s, st);
+  if (rc == NRGBD_OK)
+    rc = conv_transpose_tc_impl(s.hi, s.lo, N, Hin, Win, Cin_pad, Cin_pad, w_hi, w_lo, bias, Cout, Cout_pad, y, Cs_out, c_off, leaky, st);
+  if (s.mem) NRGBD_CUDA_CHECK(cudaFreeAsync(s.mem, st));
+  if (rc != NRGBD_OK) return rc;
   NRGBD_COUNT(4);
   NRGBD_LAUNCH_CHECK();
   return NRGBD_OK;

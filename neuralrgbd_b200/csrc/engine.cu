@@ -81,7 +81,7 @@ struct nrgbd_kvnet {
   std::unordered_map<std::string, PackedTc> packed_tc;
   std::unordered_map<std::string, PackedH2> packed_h2;
   std::unordered_map<const float*, PairBuf> pairs;   // activations that currently have a split-fp16 copy (conv_math 2)
-  int conv_math = 0;                // 0: exact fp32 FFMA implicit GEMM; 1: tcgen05 3xTF32; 2: tcgen05 split-fp16 pairs (conv_f16.cu)
+  int conv_math = 0;                // 0: exact fp32 FFMA implicit GEMM; 1: wgmma 3xTF32; 2: wgmma split-fp16 pairs (conv_f16.cu)
   bool packed_dirty = true;
   Camera cam[2];
   float* d_planes = nullptr;
@@ -90,7 +90,7 @@ struct nrgbd_kvnet {
   double* stats = nullptr;          // [2][512] per-channel sums of the conv in flight
   double* stats_b = nullptr;        // second set: a conv that consumes one BatchNorm (fused) while producing the next
   unsigned int* bn_counter = nullptr;   // f16-pair mode: the BatchNorm pass re-zeroes the statistics it consumed (no memset nodes)
-  int fuse_bn = 1;                  // 1: fold BasicBlock's first BN+ReLU into the second conv where planes >= 64 (tensor path); 2: everywhere
+  int fuse_bn = 1;                  // tf32x3: 1 folds a BN+ReLU whose only reader is a convolution into that convolution's operand split
   float* scale = nullptr;           // [512]
   float* shift = nullptr;           // [512]
   float* ws_sweep = nullptr;        // V*12
@@ -349,17 +349,13 @@ Act conv(Eng* e, const Act& x, const std::string& wname, int Cout, int kd, int k
   }
   if (use_tc(e, x, Cout)) {
     const PackedTc* pt = packw_tc(e, wname, Cout, x.C, kd * k * k, false);
-    if (!e->rc && nrgbd_conv_tc2_supported(pt->Cin_pad, pt->Cout_pad)) {       // in-kernel split, no extra pass
+    if (!e->rc && in_bn) {
+      // x is the RAW output of the producing conv: BatchNorm + ReLU are applied in the pass that splits the operands
+      // (4 B read + 8 B written per element, against 4 + 4 for a separate BatchNorm pass and 4 + 8 for the split after it)
       ProfScope ps(e, 0, flops, tag);
-      if (in_bn) {
-        ENG_CALL(e, nrgbd_conv_nhwc_tc2_bn_in(x.p, x.N, x.D, x.H, x.W, pt->Cin_pad, x.Cs, pt->hi, pt->lo, b, Cout, pt->Cout_pad, kd, k, k,
-                                              stride, pad, dil, y.p, Ho, Wo, y.Cs, c_off, leaky ? 1 : 0, want_stats ? stats_buf : nullptr,
-                                              in_bn, (nrgbd_stream_t)e->st));
-      } else {
-        ENG_CALL(e, nrgbd_conv_nhwc_tc2(x.p, x.N, x.D, x.H, x.W, pt->Cin_pad, x.Cs, pt->hi, pt->lo, b, Cout, pt->Cout_pad, kd, k, k,
-                                        stride, pad, dil, y.p, Ho, Wo, y.Cs, c_off, leaky ? 1 : 0, want_stats ? stats_buf : nullptr,
-                                        (nrgbd_stream_t)e->st));
-      }
+      ENG_CALL(e, nrgbd_conv_nhwc_tc2_bn_in(x.p, x.N, x.D, x.H, x.W, pt->Cin_pad, x.Cs, pt->hi, pt->lo, b, Cout, pt->Cout_pad, kd, k, k,
+                                            stride, pad, dil, y.p, Ho, Wo, y.Cs, c_off, leaky ? 1 : 0, want_stats ? stats_buf : nullptr,
+                                            in_bn, (nrgbd_stream_t)e->st));
       return y;
     }
     Act xh, xl;
@@ -424,7 +420,7 @@ Act convbn(Eng* e, const Act& x, const std::string& pre, int Cout, int kd, int k
   return y;
 }
 
-// Whether conv `Cin -> Cout` at this activation takes the in-kernel-split tensor path (the one that can fold an input BN)
+// Whether conv `Cin -> Cout` at this activation takes the 3xTF32 path that can fold an input BN into its operand split
 bool takes_tc2(Eng* e, const Act& x, int Cout) {
   return use_tc(e, x, Cout) && nrgbd_conv_tc2_supported(pad32(x.C), pad16(Cout));
 }
@@ -434,12 +430,10 @@ bool takes_tc2(Eng* e, const Act& x, int Cout) {
 // otherwise only its operand pair is written)
 Act basic_block(Eng* e, Act& x, const std::string& pre, int planes, int stride, int dil, bool down, bool fp32_out = true) {
   const int p1 = dil > 1 ? dil : 1;                  // psm_submodule.convbn :13
-  // Fused form (tensor path): conv1 leaves its RAW output and per-channel sums; BN1 + ReLU are applied by conv2 while it
-  // converts its operands (nrgbd_conv_nhwc_tc2_bn_in) - one read + one write of the 64/128-channel tensor less per block.
+  // Fused form (3xTF32 path): conv1 leaves its RAW output and per-channel sums; BN1 + ReLU are applied by conv2 while it
+  // splits its operands (nrgbd_conv_nhwc_tc2_bn_in) - one read + one write of the activation less per block.
   Act probe = x; probe.C = planes; probe.Cs = pad32(planes);
-  // Only where the consumer is not converter-bound: at 32 channels (N = 32 MMAs, two CTAs per SM) the operand converter is
-  // the critical warp and the extra fmaf/max per element costs more than the saved pass (measured: no net gain).
-  const bool fused = e->fuse_bn && (planes >= 64 || e->fuse_bn >= 2) && takes_tc2(e, x, planes) && takes_tc2(e, probe, planes);
+  const bool fused = e->fuse_bn && takes_tc2(e, x, planes) && takes_tc2(e, probe, planes);
   Act t;
   if (fused) t = conv(e, x, pre + ".conv1.0.0.weight", planes, 1, 3, stride, p1, dil, nullptr, false, true, nullptr, 0, -1, e->stats_b);
   else t = convbn(e, x, pre + ".conv1.0", planes, 1, 3, stride, 1, dil, true, nullptr, 2);
@@ -500,11 +494,11 @@ Act make_layer(Eng* e, Act x, bool own_x, const std::string& pre, int planes, in
 // psm_submodule.feature_extraction.forward :141-167 -> (layer1 output @1/2, features @1/4)
 void feature_cnn(Eng* e, const Act& x0, Act& l1_out, Act& feat_out) {
   const std::string P = "feature_extractor.feature_extraction";
-  // firstconv = convbn+ReLU x3 (psm_submodule.py:90-92). Tensor path: the first two BatchNorm+ReLU are folded into the
-  // conv that consumes them (the raw 5x240x320x32 tensors are read once by the next conv instead of read+written+read).
+  // firstconv = convbn+ReLU x3 (psm_submodule.py:90-92). 3xTF32 path: the first two BatchNorm+ReLU are folded into the
+  // operand split of the conv that consumes them (the raw 5x240x320x32 tensors are read once instead of read+written+read).
   Act c;
   Act probe32 = x0; probe32.C = 32; probe32.Cs = pad32(32); probe32.H = (x0.H + 2 - 3) / 2 + 1; probe32.W = (x0.W + 2 - 3) / 2 + 1;
-  if (e->fuse_bn >= 2 && takes_tc2(e, probe32, 32)) {            // development setting only: slower than the separate pass (see basic_block)
+  if (e->fuse_bn && takes_tc2(e, probe32, 32)) {
     auto bn_of = [&](const std::string& pre, double* stats, const Act& t) {
       nrgbd_bn_input bn;
       bn.stats = stats; bn.count = (double)t.pos();
@@ -836,7 +830,7 @@ int nrgbd_kvnet_set_option(nrgbd_kvnet* e, const char* key, int value) {
   if (k == "profile") { e->profile = value; return NRGBD_OK; }
   if (k == "fuse_bn") { if (e->fuse_bn != value) drop_graphs(e); e->fuse_bn = value; return NRGBD_OK; }
   if (k == "use_graph") { drop_graphs(e); e->use_graph = value; return NRGBD_OK; }
-  if (k == "conv_math") {            // 0: exact fp32 (CUDA cores); 1: tcgen05 3xTF32; 2: tcgen05 split-fp16 pairs
+  if (k == "conv_math") {            // 0: exact fp32 (CUDA cores); 1: wgmma 3xTF32; 2: wgmma split-fp16 pairs
     if (value < 0 || value > 2) { nrgbd_set_error("conv_math must be 0 (fp32), 1 (tf32x3) or 2 (f16x3)"); return NRGBD_ERR_BAD_ARG; }
     drop_graphs(e); e->conv_math = value;
     // f16-pair mode keeps the statistics buffers zero between uses (the BatchNorm pass re-zeroes what it consumed)

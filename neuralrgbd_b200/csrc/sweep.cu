@@ -173,8 +173,8 @@ plane_sweep_kernel(const float4* __restrict__ ref_w, const float4* __restrict__ 
 // ---------------------------------------------------------------------------------------------------------------
 // Second-generation kernel (C >= 64 wide channels, D <= 256): corner vectors are kept in REGISTERS across planes.
 //
-// Measured on the kernel above (profiles/r1_sweep_kernel_ncu_full.json): 158 M L1 sectors = 5.05 GB of L1 traffic for
-// 30.9 MB of algorithmic bytes - every (pixel, plane, view) re-fetched its four 268-byte corner vectors although, along
+// The kernel above re-fetches, for every (pixel, plane, view), its four 268-byte corner vectors - an L1 traffic of many GB
+// for 30.9 MB of algorithmic bytes at 640x480x64x4 - although, along
 // the epipolar line of one pixel, consecutive planes mostly hit the SAME corners (uniform depth planes: beyond the first
 // ~20 of 64 planes the total disparity change is about one texel) or the neighbouring column. Here the view loop is the
 // outer one and each lane keeps the four corner float4s of its channel slice from plane to plane: a plane whose (clamped)
@@ -344,11 +344,11 @@ int launch_sweep2(int G, int D, int hw, cudaStream_t st, const float4* ref_w, co
 #define NRGBD_SWEEP2_V(LN, P, NBV, BTV, MB)                                                                                          \
   plane_sweep2_kernel<LN, P, L1, NBV, BTV, MB><<<ceil_div((long long)hw * LN, BTV), BTV, 0, st>>>(ref_w, src_w, G, ref_n, src_n, t1, KR, \
                                                                                         rays, dpl, V, D, w, h, cx, cy, sigma, cost, bv, depth, conf)
-// 128-thread blocks with a 6-resident-block register target (80 registers, no spills): measured 232 us vs 241 us (256, 3)
-// and 277 us (256, 2) at 120x160x64x4x67; without the target ptxas takes 144 registers and the kernel runs at 419 us
+// 128-thread blocks with a 6-resident-block register target (80 registers, no spills); without the target ptxas takes 144
+// registers for this kernel and a block of it fills an SM on its own
 #define NRGBD_SWEEP2(LN, P, NBV) NRGBD_SWEEP2_V(LN, P, NBV, 128, 6)
-  if (G == 16 && (long long)hw * D >= (8ll << 20)) {      // 64 wide channels, large volumes: 8 lanes x 2 slices (measured: -12 % at 270x480x256x8,
-                                                           // +15 % at 120x160x64x4 where the lower occupancy costs more than the overhead saves)
+  if (G == 16 && (long long)hw * D >= (8ll << 20)) {      // 64 wide channels, large volumes: 8 lanes x 2 slices (half the per-pixel set-up per
+                                                           // plane; at small volumes the lower occupancy costs more than that saves)
     const int nb = (D + 7) / 8;
     if (nb <= 4) NRGBD_SWEEP2(8, 2, 4); else if (nb <= 8) NRGBD_SWEEP2(8, 2, 8); else if (nb <= 16) NRGBD_SWEEP2(8, 2, 16); else NRGBD_SWEEP2(8, 2, 32);
     return NRGBD_OK;

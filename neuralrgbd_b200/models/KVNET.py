@@ -4,7 +4,7 @@ Same constructor / forward signatures, attribute names and state_dict keys (so
 kvnet_scannet.tar / kvnet_kitti.tar load, with or without the DataParallel 'module.'
 prefix), same return tuple. forward() does no math in Python: it hands the frame to the
 native engine (include/nrgbd.h nrgbd_kvnet_*), which runs D-Net -> R-Net -> (K-Net -> R-Net)
-as hand-written sm_100a kernels on the current CUDA stream. No CPU path.
+as hand-written sm_90a kernels on the current CUDA stream. No CPU path.
 """
 import ctypes
 import math
@@ -62,7 +62,7 @@ def _init_tensor(name, shape, kind, gen):
 
 class KVNET(nn.Module):
     r'''
-    The full KV-Net pipeline on the B200 engine:
+    The full KV-Net pipeline on the H100 engine:
     * D-Net (feature extraction + plane sweep + BV_cur estimation)
     * R-Net DPV refinement / up-sampling
     * KV-Net Bayesian update against the propagated DPV
@@ -91,8 +91,8 @@ class KVNET(nn.Module):
         self.if_upsample_d = if_upsample_d
         self.cam_intrinsics = cam_intrinsics          # captured at construction: used by D-Net (KVNET.py:64-67)
         self.feat_dist = 'L2'                         # basic.py:146 default, never overridden by KVNET
-        # convolution arithmetic: 'f16x3' (default; tcgen05 kind::f16 on split-fp16 operand pairs, 22-bit products, fp32 accumulate -
-        # the fastest AND the closest to the reference of the tensor paths), 'tf32x3' (tcgen05 3xTF32), 'fp32' (exact CUDA-core FFMA)
+        # convolution arithmetic: 'f16x3' (default; wgmma on split-fp16 operand pairs, 22-bit products, fp32 accumulate -
+        # the fastest AND the closest to the reference of the tensor paths), 'tf32x3' (wgmma 3xTF32), 'fp32' (exact CUDA-core FFMA)
         self.conv_math = 'f16x3'
 
         D = len(d_candi)

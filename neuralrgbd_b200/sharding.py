@@ -3,7 +3,7 @@ windows sharded across ranks, weights broadcast once, no per-frame collective.
 
 Replaces what `torch.nn.DataParallel` does implicitly in the reference (`test_KVNet.py:163-164`,
 `train_KVNet.py:261-262`: replicate weights every forward, scatter one video per GPU, gather).
-Backend-agnostic (`nccl` on the B200 box, `gloo` in the CPU tests)."""
+Backend-agnostic (`nccl` on the GPU machines, `gloo` in the CPU tests)."""
 import torch
 import torch.distributed as dist
 

@@ -3,7 +3,7 @@
 Same names, positional order, argument meaning (numpy float64 `d_candi`, dict intrinsics,
 list-or-tensor R/t), return shapes/dtypes and error behaviour as
 /root/reference/code/warping/homography.py; every function dispatches to the hand-written
-sm_100a kernels in libnrgbd.so through the C ABI of include/nrgbd.h. torch is used for
+sm_90a kernels in libnrgbd.so through the C ABI of include/nrgbd.h. torch is used for
 device memory and the current stream only. There is no CPU path: tensors must live on a
 CUDA device and the library must be built.
 """

@@ -1,4 +1,4 @@
-"""Runs the reference's OWN inference step (baseline/_ref/code/test_utils/test_KVNet.py:test, unmodified) on the
+"""Runs the reference's OWN inference step (test_utils/test_KVNet.py:test of an unmodified checkout) on the
 engine through neuralrgbd_b200.install_as_reference_modules(), the way test_KVNet.py:159-168,190-250 does:
 construct models.KVNET.KVNET by keyword, wrap in nn.DataParallel, .cuda(), load weights, then stream frames feeding
 each step the prior the previous one returned. Prints one JSON line with the outputs' deviation from the committed

@@ -8,19 +8,44 @@ import subprocess
 import sys
 
 import numpy as np
-import pytest
 import torch
 
 from tests import cases
 from tests.conftest import ROOT
 
-REF_CODE = os.path.join(ROOT, 'baseline', '_ref', 'code')
+# the reference's code/ directory: the copy build() places in oracle/_ref (or $NRGBD_REFERENCE_CODE); without one the install
+# logic is exercised on a stand-in tree with the reference's package layout (written below)
+
+# module -> source of the stand-in: the package layout and the names install_as_reference_modules() and the reference's own
+# inference step rely on (the patched symbols, the helpers that must survive, the cross-module imports), no arithmetic
+STANDIN = {
+    'warping/__init__.py': '',
+    'warping/View.py': 'def normalised_pixel_to_ray_array(*a, **k):\n    raise NotImplementedError\n',
+    'warping/homography.py': ''.join('def %s(*a, **k):\n    raise NotImplementedError\n' % n for n in (
+        'est_swp_volume_v4', 'warp_img_feats_v3', 'warp_img_feats_mgpu', 'resample_vol_cuda', 'get_rel_extrinsicM',
+        'back_warp_th_Rt', 'back_warp_th_Rt_msrc')),
+    'mutils/__init__.py': '',
+    'mutils/misc.py': ''.join('def %s(*a, **k):\n    raise NotImplementedError\n' % n for n in (
+        'depth_val_regression', 'valid_dpv', 'get_entries_list_dict', 'm_makedir', 'save_ScenePathInfo', 'split_frame_list')),
+    'models/__init__.py': '',
+    'models/KVNET.py': 'class KVNET(object):\n    pass\n',
+    'test_utils/__init__.py': '',
+    'test_utils/test_KVNet.py': 'import warping.homography as warp_homo\n\n\ndef test(*a, **k):\n    raise NotImplementedError\n',
+    'mdataloader/__init__.py': '',
+    'mdataloader/scanNet.py': 'import warping.View as View\n',
+}
 
 
-def _have_ref():
-    if not os.path.isdir(REF_CODE) and os.path.isdir('/root/reference/code'):
-        subprocess.run([sys.executable, os.path.join(ROOT, 'baseline', 'fetch_reference.py')], check=True, capture_output=True)
-    return os.path.isdir(REF_CODE)
+def _reference_code(tmp_path):
+    from oracle import fetch_reference
+    if fetch_reference.code_dir():
+        return fetch_reference.code_dir()
+    root = str(tmp_path / 'code')
+    for rel, src in STANDIN.items():
+        os.makedirs(os.path.dirname(os.path.join(root, rel)), exist_ok=True)
+        with open(os.path.join(root, rel), 'w') as f:
+            f.write(src)
+    return root
 
 
 INSTALL_PROBE = r'''
@@ -48,15 +73,14 @@ print(json.dumps(out))
 '''
 
 
-def test_install_patches_the_reference_modules_in_place():
-    if not _have_ref():
-        pytest.skip('baseline/_ref not present (run baseline/fetch_reference.py in the build container)')
-    r = subprocess.run([sys.executable, '-c', INSTALL_PROBE % dict(root=ROOT, ref=REF_CODE)], capture_output=True, text=True,
+def test_install_patches_the_reference_modules_in_place(tmp_path):
+    ref_code = _reference_code(tmp_path)
+    r = subprocess.run([sys.executable, '-c', INSTALL_PROBE % dict(root=ROOT, ref=ref_code)], capture_output=True, text=True,
                        timeout=600)
     assert r.returncode == 0, r.stderr[-2000:]
     out = json.loads(r.stdout.strip().splitlines()[-1])
-    assert out['homography_file'].startswith(REF_CODE) and out['misc_file'].startswith(REF_CODE)      # reference modules stay
-    assert out['step_file'].startswith(REF_CODE)
+    assert out['homography_file'].startswith(ref_code) and out['misc_file'].startswith(ref_code)      # reference modules stay
+    assert out['step_file'].startswith(ref_code)
     assert all(m == 'neuralrgbd_b200.warping.homography' for m in out['patched_h'])
     assert out['patched_misc'] == 'neuralrgbd_b200.mutils.misc' and out['patched_kvnet'] == 'neuralrgbd_b200.models.KVNET'
     assert all(out['kept']) and out['view']

@@ -1,4 +1,4 @@
-"""GPU parity of the second-generation tensor-core convolution (csrc/conv_f16.cu: tcgen05 kind::f16 on split-fp16
+"""GPU parity of the second-generation tensor-core convolution (csrc/conv_f16.cu: wgmma on split-fp16
 operand pairs, halo tile) against the fp32 numpy oracle, op level. The pair product keeps 22 significand bits per
 operand like 3xTF32, so the same 6e-6 gate (relative to the output scale) applies."""
 import math

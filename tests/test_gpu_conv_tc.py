@@ -1,7 +1,6 @@
-"""GPU parity of the tcgen05 3xTF32 convolution path against the fp32 numpy oracle, op level.
+"""GPU parity of the wgmma 3xTF32 convolution path against the fp32 numpy oracle, op level.
 Expected error of the error-compensated product: ~2^-22 relative per term (vs 2^-11 for plain
-TF32), i.e. the same order as an fp32 FFMA chain; gate 6e-6 relative to the output scale
-(measured: profiles/r1_conv_microbench.json)."""
+TF32), i.e. the same order as an fp32 FFMA chain; gate 6e-6 relative to the output scale."""
 import math
 
 import numpy as np
@@ -106,7 +105,7 @@ def test_tc_matches_fp32_simt_path():
 
 @pytest.mark.parametrize('shape', [(1, 64, 480, 640, 64), (1, 96, 240, 320, 96), (5, 128, 120, 160, 128)])
 def test_tc2_large_images_repeatable(shape):
-    """Many waves of CTAs on HBM-resident inputs: the shared-memory rings and TMEM operand buffers are recycled
+    """Many waves of CTAs on HBM-resident inputs: the shared-memory rings are recycled
     hundreds of times per SM with irregular TMA latencies. A slot released before its readers had finished
     showed up only here (a few corrupt tiles per launch), never on the small oracle-sized cases."""
     from neuralrgbd_b200 import convops

@@ -135,7 +135,7 @@ def test_kvnet_forward_streaming_vs_reference(golden, name, conv_math):
     c = cases.kvnet_case(name)
     cam = cam_torch(cases.cam_for(O.make_cam_intrinsics, c['W'] // 4, c['H'] // 4))
     base = build_model(c, cam)
-    base.conv_math = conv_math        # exact fp32 CUDA-core path / tcgen05 3xTF32 tensor-core path: same gates
+    base.conv_math = conv_math        # exact fp32 CUDA-core path / wgmma 3xTF32 tensor-core path: same gates
     model = torch.nn.DataParallel(base, device_ids=[0])      # as test_KVNet.py:163
     n_steps = len(c['frames']) - 4
     bv_pred = None

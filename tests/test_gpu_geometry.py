@@ -1,5 +1,5 @@
 """GPU parity of the geometry kernels (SURVEY §8 a1-a3, a7, a9, a11, a12) through the
-reference-named Python surface -> C ABI -> sm_100a kernels, against (i) the numpy oracle on the
+reference-named Python surface -> C ABI -> sm_90a kernels, against (i) the numpy oracle on the
 same seeded inputs and (ii) the committed outputs of the live reference.
 
 Tolerances (float32 path; see DESIGN.md 'tolerance domain'):

@@ -1,5 +1,5 @@
 """Conv micro-benchmark at the real layer shapes of the 640x480 workload: fp32 FFMA implicit GEMM
-(nrgbd_conv_nhwc) vs tcgen05 3xTF32 (nrgbd_conv_nhwc_tc, split time reported separately).
+(nrgbd_conv_nhwc) vs wgmma 3xTF32 (nrgbd_conv_nhwc_tc, split time reported separately).
 CUDA events, 256 MiB L2 flush between iterations. Development aid."""
 import ctypes
 import json
@@ -49,11 +49,6 @@ SHAPES = [  # name, N, D, H, W, Cin, Cout, k(kd), stride, pad, dil
 def main():
     out = []
     for a in sys.argv[1:]:
-        if a.startswith('nacc='):
-            L.nrgbd_conv_tc_set_nacc(int(a[5:]))
-        if a.startswith('dev='):
-            st_, fl_ = a[4:].split(',')
-            L.nrgbd_conv_tc_set_dev(int(st_), int(fl_))
         if a.startswith('h2flags='):
             L.nrgbd_dev_conv_h2_set_flags(int(a[8:]))
     only = [a[5:] for a in sys.argv[1:] if a.startswith('only=')]
