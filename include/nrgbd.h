@@ -158,6 +158,37 @@ int nrgbd_lba_back_warp_backward(const float* grad_out, const float* imgs, const
                                  const float* ts, const float* K, const float* rays, int N, int C, int H, int W,
                                  float* g_imgs, float* g_R, float* g_t, double* ws, nrgbd_stream_t stream);
 
+/* ---- the LBA pose optimiser (replaces ICP/opt_pose_numerical.py local_BA_direct(_parallel): Adam on the unit-quaternion
+ * rotation u and / or the translation t of every source view, L1 photometric loss of the back-warp, 3 pyramid levels) ----
+ * Per-view state: NRGBD_LBA_STATE_FLOATS floats, owned by the caller and updated in place. u (unitQ parameter, 3), t (3),
+ * R = UnitQ2Rotation(u) (row-major 3x3, the rotation the warp uses), Adam's exp_avg / exp_avg_sq of u and of t, and the
+ * gradients of the last iteration. */
+#define NRGBD_LBA_STATE_FLOATS 40
+#define NRGBD_LBA_U 0
+#define NRGBD_LBA_T 3
+#define NRGBD_LBA_R 6
+#define NRGBD_LBA_M_U 15
+#define NRGBD_LBA_V_U 18
+#define NRGBD_LBA_M_T 21
+#define NRGBD_LBA_V_T 24
+#define NRGBD_LBA_G_U 27
+#define NRGBD_LBA_G_T 30
+#define NRGBD_LBA_OPT_R 1 /* mode bits: which parameters Adam updates */
+#define NRGBD_LBA_OPT_T 2
+/* F.avg_pool2d(x, k) of N planes [N][H][W] -> out [N][H/k][W/k] (floor), bit-exact with ATen. */
+int nrgbd_lba_avgpool(const float* x, int N, int H, int W, int k, float* out, nrgbd_stream_t stream);
+/* Bytes of device workspace nrgbd_lba_pose_opt_scale needs for V views of H x W (-1 for bad sizes). */
+long long nrgbd_lba_pose_opt_workspace_bytes(int V, int H, int W);
+/* n_iter Adam iterations at one pyramid level, enqueued on `stream` with no host synchronisation (one kernel each).
+ * ref [3][H][W], conf [H][W], dmap [H][W], srcs [V][3][H][W], K 3x3, rays [3][H*W]; mode = NRGBD_LBA_OPT_R | NRGBD_LBA_OPT_T;
+ * loss_scale = 1 / (number of residuals the reference's mean runs over); lr: this level's learning rate; first_step: Adam
+ * steps taken before this call. state [V][NRGBD_LBA_STATE_FLOATS] is updated in place; losses [n_iter][V] (double)
+ * receives each iteration's sum of |residual| per view, evaluated before the step. ws: workspace_bytes(V, H, W) bytes,
+ * 8-byte aligned; one call at a time per workspace. */
+int nrgbd_lba_pose_opt_scale(const float* ref, const float* conf, const float* dmap, const float* srcs, const float* K,
+                             const float* rays, int V, int H, int W, int mode, double loss_scale, double lr, int first_step,
+                             int n_iter, float* state, double* losses, void* ws, nrgbd_stream_t stream);
+
 /* ---- f-4: input stage (replaces mdataloader/scanNet.py:368-369 PIL nearest resize and
  * mdataloader/m_preprocess.py:15-21 ToTensor + Normalize, both host-side per frame) ------------------------------
  * dst[c][y][x] = ((float)src[ys[y]][xs[x]][c] / 255 - mean[c]) / std[c], each op rounded in fp32 (bit-exact with

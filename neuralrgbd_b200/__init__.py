@@ -17,7 +17,10 @@ _PATCHES = (
       'back_warp_th_Rt', 'back_warp_th_Rt_msrc')),
     ('mutils.misc', 'neuralrgbd_b200.mutils.misc', ('depth_val_regression', 'valid_dpv')),
     ('models.KVNET', 'neuralrgbd_b200.models.KVNET', ('KVNET',)),
+    ('ICP.opt_pose_numerical', 'neuralrgbd_b200.ICP.opt_pose_numerical', ('local_BA_direct', 'local_BA_direct_parallel')),
 )
+# packages a checkout may lack (the LBA pose optimiser): without one, only its patch is skipped
+_OPTIONAL = ('ICP',)
 
 
 def install_as_reference_modules(reference_code_dir=None):
@@ -35,7 +38,11 @@ def install_as_reference_modules(reference_code_dir=None):
     Without a reference checkout (reference_code_dir=None and `warping` not importable) the mirrors themselves are
     registered under the reference's names - enough for code that only needs the mirrored symbols.
 
-    Returns a namespace with the three patched (or registered) modules and `patched`: {module: [symbols]}.
+    `ICP.opt_pose_numerical.local_BA_direct(_parallel)` (the LBA pose optimiser) is patched too when the checkout has an
+    `ICP` package; a checkout without one skips only that patch.
+
+    Returns a namespace with the patched (or registered) modules (`opt_pose_numerical` is None when that patch was
+    skipped) and `patched`: {module: [symbols]}.
     """
     if reference_code_dir is not None:
         reference_code_dir = os.path.abspath(reference_code_dir)
@@ -45,6 +52,10 @@ def install_as_reference_modules(reference_code_dir=None):
             sys.path.insert(0, reference_code_dir)
     mods, patched = {}, {}
     for ref_name, mirror_name, symbols in _PATCHES:
+        pkg_name = ref_name.split('.')[0]
+        if (pkg_name in _OPTIONAL and reference_code_dir is not None
+                and not os.path.isdir(os.path.join(reference_code_dir, pkg_name))):
+            continue
         mirror = importlib.import_module(mirror_name)
         ref_mod = sys.modules.get(ref_name)
         if ref_mod is None or (getattr(ref_mod, '__name__', '') or '').startswith('neuralrgbd_b200'):
@@ -59,7 +70,6 @@ def install_as_reference_modules(reference_code_dir=None):
                 ref_mod = None
         if ref_mod is None:
             # no reference on the path: register the mirror (and its package) under the reference's names
-            pkg_name = ref_name.split('.')[0]
             if pkg_name not in sys.modules:
                 sys.modules[pkg_name] = importlib.import_module('neuralrgbd_b200.' + pkg_name)
             sys.modules[ref_name] = mirror
@@ -73,7 +83,8 @@ def install_as_reference_modules(reference_code_dir=None):
         mods[ref_name] = ref_mod
         patched[ref_name] = list(symbols)
     return types.SimpleNamespace(homography=mods['warping.homography'], misc=mods['mutils.misc'],
-                                 KVNET=mods['models.KVNET'], patched=patched)
+                                 KVNET=mods['models.KVNET'], opt_pose_numerical=mods.get('ICP.opt_pose_numerical'),
+                                 patched=patched)
 
 
 def uninstall_reference_patches():

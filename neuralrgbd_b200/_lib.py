@@ -89,6 +89,10 @@ SIGNATURES = {
     'nrgbd_lba_back_warp': (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     'nrgbd_lba_back_warp_backward': (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp,
                                              c_vp]),
+    'nrgbd_lba_avgpool': (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
+    'nrgbd_lba_pose_opt_workspace_bytes': (c_ll, [c_int, c_int, c_int]),
+    'nrgbd_lba_pose_opt_scale': (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, ctypes.c_double, ctypes.c_double,
+                                         c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
     'nrgbd_preprocess_rgb_u8': (c_int, [c_vp, c_int, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
     'nrgbd_export_depth_conf': (c_int, [c_vp, c_vp, c_int, c_ll, c_float, c_float, c_vp, c_vp, c_vp, c_vp, c_vp]),
     'nrgbd_write_pgm16': (c_int, [ctypes.c_char_p, c_vp, c_int, c_int]),

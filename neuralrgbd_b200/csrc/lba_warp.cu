@@ -7,36 +7,10 @@
 // respect to R and t (60 Adam iterations x 3 scales per frame): the backward kernel is grid_sampler_2d_backward with
 // respect to the grid chained through the perspective division and the two small matmuls, plus the scatter-add of the
 // image gradient. One thread per (view, reference pixel); no N x H x W x 2 grid tensor, no homogeneous point matrices.
-#include "common.cuh"
+#include "lba_common.cuh"
 #include "../../include/nrgbd.h"
 
 namespace {
-
-struct LbaGeom {
-  float ix, iy;        // un-normalised sampling location
-  float X0, X1, X2;    // back-projected point
-  float Px, Py, Pz;    // K (R X + t)
-};
-
-// Coordinate chain in the reference's op order (:546-567): elementwise d * ray, 4x4 matmuls as sgemm FMA chains over k
-// (the homogeneous 1 contributes fma(t, 1, acc) = acc + t; the zero last column of the 4x4 intrinsic matrix nothing),
-// division by P_z WITHOUT an epsilon, (u - cx) / cx, ATen's un-normalisation.
-__device__ __forceinline__ LbaGeom lba_project(float d, float r0, float r1, float r2, const float* __restrict__ R, const float* __restrict__ t,
-                                               const float* __restrict__ K, float Wf, float Hf) {
-  LbaGeom g;
-  g.X0 = __fmul_rn(d, r0); g.X1 = __fmul_rn(d, r1); g.X2 = __fmul_rn(d, r2);
-  const float c0 = __fadd_rn(dot3_chain(R[0], R[1], R[2], g.X0, g.X1, g.X2), t[0]);
-  const float c1 = __fadd_rn(dot3_chain(R[3], R[4], R[5], g.X0, g.X1, g.X2), t[1]);
-  const float c2 = __fadd_rn(dot3_chain(R[6], R[7], R[8], g.X0, g.X1, g.X2), t[2]);
-  g.Px = dot3_chain(K[0], K[1], K[2], c0, c1, c2);
-  g.Py = dot3_chain(K[3], K[4], K[5], c0, c1, c2);
-  g.Pz = dot3_chain(K[6], K[7], K[8], c0, c1, c2);
-  const float u = __fdiv_rn(g.Px, g.Pz), v = __fdiv_rn(g.Py, g.Pz);
-  const float cx = K[2], cy = K[5];
-  g.ix = unnormalize(__fdiv_rn(__fsub_rn(u, cx), cx), Wf);
-  g.iy = unnormalize(__fdiv_rn(__fsub_rn(v, cy), cy), Hf);
-  return g;
-}
 
 __global__ void __launch_bounds__(256)
 lba_warp_forward_kernel(const float* __restrict__ imgs, const float* __restrict__ dmap, const float* __restrict__ Rs,
@@ -92,9 +66,7 @@ lba_warp_backward_kernel(const float* __restrict__ grad_out, const float* __rest
         const float* s = src + (long long)c * hw;
         const float nw = (vx0 && vy0) ? __ldg(s + y0 * W + x0) : 0.f, ne = (vx1 && vy0) ? __ldg(s + y0 * W + x1) : 0.f;
         const float sw = (vx0 && vy1) ? __ldg(s + y1 * W + x0) : 0.f, se = (vx1 && vy1) ? __ldg(s + y1 * W + x1) : 0.f;
-        // ATen grid_sampler_2d_backward: d out / d ix, d out / d iy
-        gix += gv * (-nw * ay + ne * ay - sw * by + se * by);
-        giy += gv * (-nw * ax - ne * bx + sw * ax + se * bx);
+        lba_grid_grad(gv, nw, ne, sw, se, ax, bx, ay, by, gix, giy);
         if (gi) {
           float* d = gi + (long long)c * hw;
           if (vx0 && vy0) atomicAdd(d + y0 * W + x0, gv * ax * ay);
@@ -103,19 +75,7 @@ lba_warp_backward_kernel(const float* __restrict__ grad_out, const float* __rest
           if (vx1 && vy1) atomicAdd(d + y1 * W + x1, gv * bx * by);
         }
       }
-      // ix = ((u - cx) / cx + 1) W / 2 - 1 / 2  ->  d ix / d u = W / (2 cx); u = Px / Pz
-      const float cx = K[2], cy = K[5];
-      const float gu = gix * (Wf * 0.5f) / cx, gvv = giy * (Hf * 0.5f) / cy;
-      const float iz = 1.f / g.Pz;
-      const float gPx = gu * iz, gPy = gvv * iz, gPz = -(gu * g.Px + gvv * g.Py) * iz * iz;
-      // g_Xc = K^T g_P
-      const float gc0 = K[0] * gPx + K[3] * gPy + K[6] * gPz;
-      const float gc1 = K[1] * gPx + K[4] * gPy + K[7] * gPz;
-      const float gc2 = K[2] * gPx + K[5] * gPy + K[8] * gPz;
-      acc[0] = gc0 * g.X0; acc[1] = gc0 * g.X1; acc[2] = gc0 * g.X2;
-      acc[3] = gc1 * g.X0; acc[4] = gc1 * g.X1; acc[5] = gc1 * g.X2;
-      acc[6] = gc2 * g.X0; acc[7] = gc2 * g.X1; acc[8] = gc2 * g.X2;
-      acc[9] = gc0; acc[10] = gc1; acc[11] = gc2;
+      lba_pose_grad(g, gix, giy, K, Wf, Hf, acc);
     }
   }
   // block reduction of the 12 pose-gradient terms (double from the warp level on)
