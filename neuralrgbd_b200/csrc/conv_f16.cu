@@ -11,20 +11,26 @@
 // fused BatchNorm pass), so both operands go TMA -> shared memory -> tensor core.
 //
 // Halo tile. One (TH + 2p) x (TW + 2p) pixel halo box per (depth tap, 32-channel chunk) is staged once and all in-plane
-// taps read it through shifted wgmma descriptors: the output tile is 16 rows x 8 columns, so one 8-row core-matrix group
-// is exactly one tile row, a tap (dy, dx) is a start-address offset of (dy * pitch + dx) pixel rows and the stride-byte-
-// offset between groups is the halo pitch (pitch * row bytes, not a multiple of the swizzle atom: the swizzle is a
-// function of the absolute shared-memory address, as is TMA's, so any 16-byte-aligned row offset stays consistent).
-// A 3x3 convolution reads its input tile 1.4x instead of 9x. Strided convolutions use one box per tap ("tap mode").
+// taps read it through shifted wgmma descriptors: the output tile is TH x TW = 16 x 8 or 8 x 16 pixels, and each
+// warpgroup's 64 GEMM rows are 8 core-matrix groups of 8 pixels that are each a piece of one tile row (16 x 8: rows
+// [8 cw, 8 cw + 8); 8 x 16: columns [8 cw, 8 cw + 8) of all 8 rows, a start offset of 8 pixels). A tap (dy, dx) is a
+// start-address offset of (dy * pitch + dx) pixel rows and the stride-byte-offset between groups is the halo pitch
+// (pitch * row bytes, not a multiple of the swizzle atom: the swizzle is a function of the absolute shared-memory
+// address, as is TMA's, so any 16-byte-aligned row offset stays consistent). A 3x3 convolution reads its input tile 1.4x
+// instead of 9x. Strided convolutions use one box per tap ("tap mode"). The launch takes the orientation that pads fewer
+// output positions: 8 x 16 divides the 120-row planes of the 1/4-resolution layers, 16 x 8 leaves a 1/16 ragged row.
 //
-// Roles (one 128-pixel x BN-channel tile per CTA, grid.y = Cout chunks of BN <= 128 channels):
-//   warps 0-7   two consumer warpgroups, 64 pixels (8 tile rows) each: per K step and tap, wgmma a_hi x b_hi -> main,
-//               a_hi x b_lo and a_lo x b_hi -> cross; the ring slots of step s are released once step s + 1 is issued
-//               and step s has retired (wgmma.wait_group 1); then the epilogue straight from the registers: main +
-//               scale * cross, bias / LeakyReLU, fp32 or fp16-pair stores, BatchNorm column sums (one pair of fp64
-//               atomics per column and CTA).
+// Roles (persistent CTAs over 128-pixel x BN-channel tiles, grid.y = Cout chunks of BN <= 128 channels):
+//   warps 0-7   two consumer warpgroups, 64 pixels each: per K step and tap, wgmma a_hi x b_hi -> main, a_hi x b_lo and
+//               a_lo x b_hi -> cross; the ring slots of step s are released once step s + 1 is issued and step s has
+//               retired (wgmma.wait_group 1), the last step's at the end of the tile; then the epilogue straight from the
+//               registers: main + scale * cross, bias / LeakyReLU, fp32 or fp16-pair stores, BatchNorm column sums
+//               (summed per CTA over its tiles, then one pair of fp64 atomics per column and CTA).
+//               (a_hi x [b_hi | b_lo] as one wgmma of N = 2 BN would read a_hi once, but its accumulators overlap those of
+//               a_lo x b_hi in part, and ptxas then serialises every wgmma (C7511): 8-15 % slower on H100.)
 //   warp 8      TMA producer: halo / tap box of the hi and the lo activation planes into the A ring, G taps of the hi and
-//               lo K-major weight tiles into the B ring; expect-tx mbarriers.
+//               lo K-major weight tiles into the B ring; expect-tx mbarriers. It runs on into the next tile's stages, so
+//               that tile's first loads overlap this tile's last steps and epilogue.
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -35,19 +41,18 @@
 
 namespace {
 
-constexpr int TH = 16, TW = 8;         // output tile: 16 rows x 8 columns = 128 GEMM rows
 constexpr int WG_THREADS = 288;        // warps 0-7: two consumer warpgroups, warp 8: TMA producer
 constexpr int BKC = 32;                // input channels per K chunk
 
 struct WgParams {
   float* y; const float* bias; double* stats;
   __half *y_hi, *y_lo;
-  int N, Dz, Hy, Wx, tiles_x, tiles_y;
+  int N, Dz, Hy, Wx, tiles_x, tiles_y, n_tiles, wide;   // wide: 8 x 16 output tile (else 16 x 8)
   int cin_chunks, n_kz, n_tap, halo, in_stride, org_y, org_x;
   int Cout, c_first;                     // logical output channels; first channel of this launch's chunk 0
   int Dout, Hout, Wout, Cs_out, c_off, out_stride, out_off_y, out_off_x, leaky;
   int stages_a, stages_b, box_w, box_h;  // ring depths; activation box in pixels (halo pitch x halo rows, or the tile)
-  uint32_t a_tile_bytes, a_stage_bytes, a_tx_bytes, b_stage_bytes, wg_row16;   // wg_row16: 8 tile rows down the A tile, 16-byte units
+  uint32_t a_tile_bytes, a_stage_bytes, a_tx_bytes, b_stage_bytes, wg_row16;   // wg_row16: second warpgroup's A offset, 16-byte units
   uint32_t a_desc_hi, b_desc_hi;         // high words of the shared-memory descriptors (SBO, swizzle mode)
   signed char dz[3];
   signed char dy[WG_MAX_TAP2D], dx[WG_MAX_TAP2D];
@@ -112,14 +117,16 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
   constexpr float SCALE = TF32 ? 1.f : 1.f / 2048.f;
   constexpr uint32_t B_HALF = (uint32_t)(G * BN * RB);
   constexpr int NJ = BN / 8;                          // 8-column accumulator blocks
-  // shared memory: [A ring: stages_a x (hi | lo)][B ring: stages_b x (hi G taps | lo G taps)][column sums 8 x 2 x BN][barriers]
+  // shared memory: [A ring: stages_a x (hi | lo)][B ring: stages_b x (hi G taps | lo G taps)][column sums 8 x 2 x BN floats]
+  //                [CTA column sums 2 x BN doubles][barriers]
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t base = smem_u32(smem_raw);
   if (base & 1023u) __trap();
   const uint32_t b_ring = base + (uint32_t)p.stages_a * p.a_stage_bytes;
   const uint32_t sums_off = (uint32_t)p.stages_a * p.a_stage_bytes + (uint32_t)p.stages_b * p.b_stage_bytes;
   float* part = reinterpret_cast<float*>(smem_raw + sums_off);
-  const uint32_t bars = base + sums_off + 8u * 2u * BN * 4u;
+  double* cta_sums = reinterpret_cast<double*>(smem_raw + sums_off + 8u * 2u * BN * 4u);
+  const uint32_t bars = base + sums_off + 8u * 2u * BN * 4u + 2u * BN * 8u;
   const uint32_t bar_afull = bars, bar_aempty = bars + 64, bar_bfull = bars + 128, bar_bempty = bars + 192;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -128,13 +135,12 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
     for (int s = 0; s < p.stages_b; ++s) { mbar_init(bar_bfull + 8 * s, 1); mbar_init(bar_bempty + 8 * s, 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
+  if (threadIdx.x < 2 * BN) cta_sums[threadIdx.x] = 0.0;
   __syncthreads();
 
-  int t = blockIdx.x;
-  const int tx = t % p.tiles_x; t /= p.tiles_x;
-  const int ty = t % p.tiles_y; t /= p.tiles_y;
-  const int z0 = t % p.Dz, n0 = t / p.Dz;
-  const int ox0 = tx * TW, oy0 = ty * TH;
+  // Persistent CTAs: tiles blockIdx.x, blockIdx.x + gridDim.x, ... The rings and their phases run on across tiles, so
+  // the producer loads the next tile's first stages while the consumers run this tile's epilogue.
+  const int th = p.wide ? 8 : 16, tw = p.wide ? 16 : 8;
   const int cbase = p.c_first + (int)blockIdx.y * BN;
   const int n_steps = p.n_kz * p.cin_chunks * (p.n_tap / G);
 
@@ -143,27 +149,33 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
     if (lane == 0) {
       int sa = 0, sb = 0;
       uint32_t pha = 0, phb = 0;
-      for (int kz = 0; kz < p.n_kz; ++kz) {
-        const int cz = z0 + p.dz[kz];
-        for (int cc = 0; cc < p.cin_chunks; ++cc) {
-          for (int tap = 0; tap < p.n_tap; tap += G) {
-            if (!p.halo || tap == 0) {
-              const int cx = ox0 * p.in_stride + (p.halo ? p.org_x : (int)p.dx[tap]);
-              const int cy = oy0 * p.in_stride + (p.halo ? p.org_y : (int)p.dy[tap]);
-              mbar_wait(bar_aempty + 8 * sa, pha ^ 1u);
-              mbar_expect_tx(bar_afull + 8 * sa, p.a_tx_bytes);
-              const uint32_t dst = base + (uint32_t)sa * p.a_stage_bytes;
-              tma_load_5d(dst, &tm_a_hi, bar_afull + 8 * sa, cc * BKC, cx, cy, cz, n0);
-              tma_load_5d(dst + p.a_tile_bytes, &tm_a_lo, bar_afull + 8 * sa, cc * BKC, cx, cy, cz, n0);
-              if (++sa == p.stages_a) { sa = 0; pha ^= 1u; }
+      for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
+        int t = tile;
+        const int ox0 = (t % p.tiles_x) * tw; t /= p.tiles_x;
+        const int oy0 = (t % p.tiles_y) * th; t /= p.tiles_y;
+        const int z0 = t % p.Dz, n0 = t / p.Dz;
+        for (int kz = 0; kz < p.n_kz; ++kz) {
+          const int cz = z0 + p.dz[kz];
+          for (int cc = 0; cc < p.cin_chunks; ++cc) {
+            for (int tap = 0; tap < p.n_tap; tap += G) {
+              if (!p.halo || tap == 0) {
+                const int cx = ox0 * p.in_stride + (p.halo ? p.org_x : (int)p.dx[tap]);
+                const int cy = oy0 * p.in_stride + (p.halo ? p.org_y : (int)p.dy[tap]);
+                mbar_wait(bar_aempty + 8 * sa, pha ^ 1u);
+                mbar_expect_tx(bar_afull + 8 * sa, p.a_tx_bytes);
+                const uint32_t dst = base + (uint32_t)sa * p.a_stage_bytes;
+                tma_load_5d(dst, &tm_a_hi, bar_afull + 8 * sa, cc * BKC, cx, cy, cz, n0);
+                tma_load_5d(dst + p.a_tile_bytes, &tm_a_lo, bar_afull + 8 * sa, cc * BKC, cx, cy, cz, n0);
+                if (++sa == p.stages_a) { sa = 0; pha ^= 1u; }
+              }
+              mbar_wait(bar_bempty + 8 * sb, phb ^ 1u);
+              mbar_expect_tx(bar_bfull + 8 * sb, 2 * B_HALF);
+              const uint32_t dst = b_ring + (uint32_t)sb * p.b_stage_bytes;
+              const int ws = p.wsel[kz * p.n_tap + tap];
+              tma_load_3d(dst, &tm_b_hi, bar_bfull + 8 * sb, cc * BKC, cbase, ws);
+              tma_load_3d(dst + B_HALF, &tm_b_lo, bar_bfull + 8 * sb, cc * BKC, cbase, ws);
+              if (++sb == p.stages_b) { sb = 0; phb ^= 1u; }
             }
-            mbar_wait(bar_bempty + 8 * sb, phb ^ 1u);
-            mbar_expect_tx(bar_bfull + 8 * sb, 2 * B_HALF);
-            const uint32_t dst = b_ring + (uint32_t)sb * p.b_stage_bytes;
-            const int ws = p.wsel[kz * p.n_tap + tap];
-            tma_load_3d(dst, &tm_b_hi, bar_bfull + 8 * sb, cc * BKC, cbase, ws);
-            tma_load_3d(dst + B_HALF, &tm_b_lo, bar_bfull + 8 * sb, cc * BKC, cbase, ws);
-            if (++sb == p.stages_b) { sb = 0; phb ^= 1u; }
           }
         }
       }
@@ -171,140 +183,156 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
     return;
   }
 
-  // ===== consumers: warpgroup cw owns tile rows [8 cw, 8 cw + 8) =====
-  const int cw = warp >> 2;
+  // ===== consumers: 64 GEMM rows per warpgroup; 16x8 tile: cw owns tile rows [8 cw, 8 cw + 8), 8x16 tile: columns
+  // [8 cw, 8 cw + 8) of all 8 rows. Either way core-matrix group g is one tile row, one halo pitch down. =====
+  const int cw = warp >> 2, w4 = warp & 3;
   float acc_m[BN / 2], acc_c[BN / 2];
-#pragma unroll
-  for (int k = 0; k < BN / 2; ++k) { acc_m[k] = 0.f; acc_c[k] = 0.f; }
   const uint32_t wg_off = (uint32_t)cw * p.wg_row16 * 16u;
   int sa = 0, sb = 0, sa_cur = 0, tap = 0;
   uint32_t pha = 0, phb = 0;
-  int rel_a = -1, rel_b = -1;                         // slots of the previous step, released once it has retired
-  for (int step = 0; step < n_steps; ++step) {
-    const bool new_a = !p.halo || tap == 0;
-    if (new_a) {
-      mbar_wait(bar_afull + 8 * sa, pha);
-      sa_cur = sa;
-      if (++sa == p.stages_a) { sa = 0; pha ^= 1u; }
-    }
-    mbar_wait(bar_bfull + 8 * sb, phb);
-    const uint32_t a_hi = base + (uint32_t)sa_cur * p.a_stage_bytes + wg_off;
-    const uint32_t b_hi = b_ring + (uint32_t)sb * p.b_stage_bytes;
-    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+  for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
 #pragma unroll
-    for (int g = 0; g < G; ++g) {
-      const uint32_t ao = a_hi + (p.halo ? (uint32_t)p.a_off16[tap + g] * 16u : 0u);
-#pragma unroll
-      for (int ks = 0; ks < KS; ++ks) {
-        const uint32_t ah = ao + 32u * ks, al = ah + p.a_tile_bytes;
-        const uint32_t bh = b_hi + (uint32_t)(g * BN * RB) + 32u * ks, bl = bh + B_HALF;
-        wg_mma<BN, TF32>(acc_m, wg_desc(ah, p.a_desc_hi), wg_desc(bh, p.b_desc_hi));
-        wg_mma<BN, TF32>(acc_c, wg_desc(ah, p.a_desc_hi), wg_desc(bl, p.b_desc_hi));
-        wg_mma<BN, TF32>(acc_c, wg_desc(al, p.a_desc_hi), wg_desc(bh, p.b_desc_hi));
+    for (int k = 0; k < BN / 2; ++k) { acc_m[k] = 0.f; acc_c[k] = 0.f; }
+    int rel_a = -1, rel_b = -1;                       // slots of the previous step, released once it has retired
+    for (int step = 0; step < n_steps; ++step) {
+      const bool new_a = !p.halo || tap == 0;
+      if (new_a) {
+        mbar_wait(bar_afull + 8 * sa, pha);
+        sa_cur = sa;
+        if (++sa == p.stages_a) { sa = 0; pha ^= 1u; }
       }
-    }
-    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
-    asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
-    if (lane == 0) {
-      if (rel_b >= 0) mbar_arrive(bar_bempty + 8 * rel_b);
-      if (rel_a >= 0) mbar_arrive(bar_aempty + 8 * rel_a);
-    }
-    tap += G;
-    const bool last_of_a = !p.halo || tap == p.n_tap;
-    if (tap == p.n_tap) tap = 0;
-    rel_b = sb; rel_a = last_of_a ? sa_cur : -1;
-    if (++sb == p.stages_b) { sb = 0; phb ^= 1u; }
-  }
-  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
-  // (the producer issues no further loads: the last slots need no release)
-
-  // ===== epilogue from the accumulator registers =====
-  const int w4 = warp & 3;
-  const int n_here = min(BN, p.Cout - cbase);
-  const bool pair = p.y_hi != nullptr;
-  const bool vec2 = ((p.Cs_out | (p.c_off + cbase)) & 1) == 0;
-  float* dst_row[2] = {nullptr, nullptr};
-  long long pix[2] = {0, 0};
-  bool valid[2];
+      mbar_wait(bar_bfull + 8 * sb, phb);
+      const uint32_t a_hi = base + (uint32_t)sa_cur * p.a_stage_bytes + wg_off;
+      const uint32_t b_hi = b_ring + (uint32_t)sb * p.b_stage_bytes;
+      asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const int r = 16 * w4 + (lane >> 2) + 8 * i;      // GEMM row within the warpgroup
-    const int iy = oy0 + 8 * cw + (r >> 3), ix = ox0 + (r & 7);
-    valid[i] = iy < p.Hy && ix < p.Wx;
-    const int oy = iy * p.out_stride + p.out_off_y, ox = ix * p.out_stride + p.out_off_x;
-    pix[i] = (((long long)n0 * p.Dout + z0) * p.Hout + oy) * p.Wout + ox;
-    if (!pair) dst_row[i] = p.y + pix[i] * (long long)p.Cs_out + p.c_off + cbase;
-  }
-  constexpr int NJ_PAIR = ((BN + 31) / 32) * 4;       // pair output: pad channels up to the next 32 are stored as zeros
-  const int nj_store = pair ? NJ_PAIR : NJ;
+      for (int g = 0; g < G; ++g) {
+        const uint32_t ao = a_hi + (p.halo ? (uint32_t)p.a_off16[tap + g] * 16u : 0u);
 #pragma unroll
-  for (int j = 0; j < NJ_PAIR; ++j) {
-    if (j >= nj_store) break;
-    const int c = 8 * j + 2 * (lane & 3);
-    float v[2][2];
-#pragma unroll
-    for (int i = 0; i < 2; ++i)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        float f = 0.f;
-        if (j < NJ && c + e < n_here && valid[i]) {
-          f = fmaf(acc_c[4 * j + 2 * i + e], SCALE, acc_m[4 * j + 2 * i + e]);
-          if (p.bias) f += __ldg(p.bias + cbase + c + e);
-          if (p.leaky) f = f >= 0.f ? f : f * 0.01f;
+        for (int ks = 0; ks < KS; ++ks) {
+          const uint32_t ah = ao + 32u * ks, al = ah + p.a_tile_bytes;
+          const uint32_t bh = b_hi + (uint32_t)(g * BN * RB) + 32u * ks, bl = bh + B_HALF;
+          wg_mma<BN, TF32>(acc_m, wg_desc(ah, p.a_desc_hi), wg_desc(bh, p.b_desc_hi));
+          wg_mma<BN, TF32>(acc_c, wg_desc(ah, p.a_desc_hi), wg_desc(bl, p.b_desc_hi));
+          wg_mma<BN, TF32>(acc_c, wg_desc(al, p.a_desc_hi), wg_desc(bh, p.b_desc_hi));
         }
-        v[i][e] = f;
       }
+      asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+      asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+      if (lane == 0) {
+        if (rel_b >= 0) mbar_arrive(bar_bempty + 8 * rel_b);
+        if (rel_a >= 0) mbar_arrive(bar_aempty + 8 * rel_a);
+      }
+      tap += G;
+      const bool last_of_a = !p.halo || tap == p.n_tap;
+      if (tap == p.n_tap) tap = 0;
+      rel_b = sb; rel_a = last_of_a ? sa_cur : -1;
+      if (++sb == p.stages_b) { sb = 0; phb ^= 1u; }
+    }
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    // the last step's slots: the producer may already be waiting on them for the next tile
+    if (lane == 0) {
+      mbar_arrive(bar_bempty + 8 * rel_b);
+      mbar_arrive(bar_aempty + 8 * rel_a);
+    }
+
+    // ===== epilogue from the accumulator registers (its indices are computed here, not held through the K loop) =====
+    int t = tile;
+    const int ox0 = (t % p.tiles_x) * tw; t /= p.tiles_x;
+    const int oy0 = (t % p.tiles_y) * th; t /= p.tiles_y;
+    const int z0 = t % p.Dz, n0 = t / p.Dz;
+    const int n_here = min(BN, p.Cout - cbase);
+    const bool pair = p.y_hi != nullptr;
+    const bool vec2 = ((p.Cs_out | (p.c_off + cbase)) & 1) == 0;
+    float* dst_row[2] = {nullptr, nullptr};
+    long long pix[2] = {0, 0};
+    bool valid[2];
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-      if (!valid[i]) continue;
-      if (pair) {
-        __half h0, l0, h1, l1;
-        nrgbd_split_pair(v[i][0], h0, l0); nrgbd_split_pair(v[i][1], h1, l1);
-        const long long o = pix[i] * (long long)p.Cs_out + cbase + c;
-        *reinterpret_cast<__half2*>(p.y_hi + o) = __halves2half2(h0, h1);
-        *reinterpret_cast<__half2*>(p.y_lo + o) = __halves2half2(l0, l1);
-      } else if (vec2 && c + 1 < n_here) {
-        *reinterpret_cast<float2*>(dst_row[i] + c) = make_float2(v[i][0], v[i][1]);
-      } else {
-        if (c < n_here) dst_row[i][c] = v[i][0];
-        if (c + 1 < n_here) dst_row[i][c + 1] = v[i][1];
-      }
+      const int r = 16 * w4 + (lane >> 2) + 8 * i;    // GEMM row within the warpgroup: tile row r / 8, column r % 8
+      const int iy = oy0 + (r >> 3) + (p.wide ? 0 : 8 * cw), ix = ox0 + (r & 7) + (p.wide ? 8 * cw : 0);
+      valid[i] = iy < p.Hy && ix < p.Wx;
+      const int oy = iy * p.out_stride + p.out_off_y, ox = ix * p.out_stride + p.out_off_x;
+      pix[i] = (((long long)n0 * p.Dout + z0) * p.Hout + oy) * p.Wout + ox;
+      if (!pair) dst_row[i] = p.y + pix[i] * (long long)p.Cs_out + p.c_off + cbase;
     }
-    if (p.stats && j < NJ) {
-      // column sums over this warp's 16 rows: the thread's two rows, then across the 8 lane quads
-      float s1[2], s2[2];
+    constexpr int NJ_PAIR = ((BN + 31) / 32) * 4;     // pair output: pad channels up to the next 32 are stored as zeros
+    const int nj_store = pair ? NJ_PAIR : NJ;
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        s1[e] = v[0][e] + v[1][e];
-        s2[e] = fmaf(v[0][e], v[0][e], v[1][e] * v[1][e]);
+    for (int j = 0; j < NJ_PAIR; ++j) {
+      if (j >= nj_store) break;
+      const int c = 8 * j + 2 * (lane & 3);
+      float v[2][2];
 #pragma unroll
-        for (int m = 4; m < 32; m <<= 1) {
-          s1[e] += __shfl_xor_sync(0xffffffffu, s1[e], m);
-          s2[e] += __shfl_xor_sync(0xffffffffu, s2[e], m);
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float f = 0.f;
+          if (j < NJ && c + e < n_here && valid[i]) {
+            f = fmaf(acc_c[4 * j + 2 * i + e], SCALE, acc_m[4 * j + 2 * i + e]);
+            if (p.bias) f += __ldg(p.bias + cbase + c + e);
+            if (p.leaky) f = f >= 0.f ? f : f * 0.01f;
+          }
+          v[i][e] = f;
+        }
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        if (!valid[i]) continue;
+        if (pair) {
+          __half h0, l0, h1, l1;
+          nrgbd_split_pair(v[i][0], h0, l0); nrgbd_split_pair(v[i][1], h1, l1);
+          const long long o = pix[i] * (long long)p.Cs_out + cbase + c;
+          *reinterpret_cast<__half2*>(p.y_hi + o) = __halves2half2(h0, h1);
+          *reinterpret_cast<__half2*>(p.y_lo + o) = __halves2half2(l0, l1);
+        } else if (vec2 && c + 1 < n_here) {
+          *reinterpret_cast<float2*>(dst_row[i] + c) = make_float2(v[i][0], v[i][1]);
+        } else {
+          if (c < n_here) dst_row[i][c] = v[i][0];
+          if (c + 1 < n_here) dst_row[i][c + 1] = v[i][1];
         }
       }
-      if (lane < 4) {
+      if (p.stats && j < NJ) {
+        // column sums over this warp's 16 rows: the thread's two rows, then across the 8 lane quads
+        float s1[2], s2[2];
 #pragma unroll
-        for (int e = 0; e < 2; ++e) { part[(warp * 2) * BN + c + e] = s1[e]; part[(warp * 2 + 1) * BN + c + e] = s2[e]; }
+        for (int e = 0; e < 2; ++e) {
+          s1[e] = v[0][e] + v[1][e];
+          s2[e] = fmaf(v[0][e], v[0][e], v[1][e] * v[1][e]);
+#pragma unroll
+          for (int m = 4; m < 32; m <<= 1) {
+            s1[e] += __shfl_xor_sync(0xffffffffu, s1[e], m);
+            s2[e] += __shfl_xor_sync(0xffffffffu, s2[e], m);
+          }
+        }
+        if (lane < 4) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) { part[(warp * 2) * BN + c + e] = s1[e]; part[(warp * 2 + 1) * BN + c + e] = s2[e]; }
+        }
       }
     }
-  }
-  if (p.stats) {
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    const int c = threadIdx.x;
-    if (c < n_here) {
-      double a1 = 0.0, a2 = 0.0;
+    if (p.stats) {
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      const int c = threadIdx.x;
+      if (c < n_here) {
+        double a1 = 0.0, a2 = 0.0;
 #pragma unroll
-      for (int w = 0; w < 8; ++w) { a1 += (double)part[(w * 2) * BN + c]; a2 += (double)part[(w * 2 + 1) * BN + c]; }
-      atomicAdd(p.stats + cbase + c, a1);
-      atomicAdd(p.stats + p.Cout + cbase + c, a2);
+        for (int w = 0; w < 8; ++w) { a1 += (double)part[(w * 2) * BN + c]; a2 += (double)part[(w * 2 + 1) * BN + c]; }
+        cta_sums[c] += a1; cta_sums[BN + c] += a2;
+      }
+      asm volatile("bar.sync 1, 256;" ::: "memory");   // the next tile overwrites the partial sums
     }
+  }
+  const int c = threadIdx.x;
+  if (p.stats && c < min(BN, p.Cout - cbase) && (int)blockIdx.x < p.n_tiles) {
+    atomicAdd(p.stats + cbase + c, cta_sums[c]);
+    atomicAdd(p.stats + p.Cout + cbase + c, cta_sums[BN + c]);
   }
 }
 
 int g_h2_smem_cap_kb = 0;   // development: cap on the dynamic shared memory per CTA (0 = chosen by the plan below)
 int g_h2_flags = 0;         // development knobs (nrgbd_dev_conv_h2_set_flags), all off in production:
-                            //   4 one box per tap (no halo tile)   128 one tap per pipeline step
+                            //   4 one box per tap (no halo tile)   8 always the 16 x 8 output tile
+                            //   32 one tile per CTA (no persistent CTAs)   128 one tap per pipeline step
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -405,7 +433,7 @@ int launch_chunks(const WgConv& c, WgParams p, int BN, int n_chunks, int c_first
     if (consecutive) G = 3;
   }
   // shared memory: two CTAs per SM when BN <= 64 and two A + two B stages fit half of the SM's 228 KB
-  const size_t extra = (size_t)8 * 2 * BN * 4 + 256;
+  const size_t extra = (size_t)8 * 2 * BN * 4 + (size_t)2 * BN * 8 + 256;
   auto plan = [&](size_t cap, int g, int& sa, int& sb) {
     const size_t b_stage = (size_t)2 * g * BN * RB;
     sa = 2;
@@ -441,8 +469,14 @@ int launch_chunks(const WgConv& c, WgParams p, int BN, int n_chunks, int c_first
     if (e != cudaSuccess) { nrgbd_set_error("conv_wgmma: cannot opt in to %zu bytes of shared memory: %s", smem, cudaGetErrorString(e)); return NRGBD_ERR_CUDA; }
     conf = smem;
   }
-  const long long tiles = (long long)p.N * p.Dz * p.tiles_x * p.tiles_y;
-  fn<<<dim3((unsigned)tiles, (unsigned)n_chunks), WG_THREADS, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, p);
+  // persistent CTAs: one per resident slot (the smem plan and __launch_bounds__ give the CTAs per SM), shared out
+  // among the Cout chunks
+  int grid_x = p.n_tiles;
+  if (!(g_h2_flags & 32)) {
+    const int per_sm = (int)std::min<size_t>(BN <= 64 ? 2 : 1, 233472 / (smem + 1024));
+    grid_x = std::min(grid_x, ceil_div(nrgbd_sm_count() * per_sm, n_chunks));
+  }
+  fn<<<dim3((unsigned)grid_x, (unsigned)n_chunks), WG_THREADS, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, p);
   return NRGBD_OK;
 }
 
@@ -456,7 +490,13 @@ int conv_wgmma(const WgConv& c, cudaStream_t st) {
   p.y = c.y; p.bias = c.bias; p.stats = c.stats;
   p.y_hi = reinterpret_cast<__half*>(c.y_hi); p.y_lo = reinterpret_cast<__half*>(c.y_lo);
   p.N = c.N; p.Dz = c.Din; p.Hy = c.Hy; p.Wx = c.Wx;
+  // output tile 8 x 16 when it pads fewer positions than 16 x 8 (120-row planes), else 16 x 8
+  const long long pad_tall = (long long)ceil_div(c.Hy, 16) * ceil_div(c.Wx, 8), pad_wide = (long long)ceil_div(c.Hy, 8) * ceil_div(c.Wx, 16);
+  p.wide = (pad_wide < pad_tall && !(g_h2_flags & 8)) ? 1 : 0;
+  const int TH = p.wide ? 8 : 16, TW = p.wide ? 16 : 8;
   p.tiles_x = ceil_div(c.Wx, TW); p.tiles_y = ceil_div(c.Hy, TH);
+  NRGBD_REQUIRE((long long)p.N * p.Dz * p.tiles_x * p.tiles_y < (1ll << 31), "too many output tiles");
+  p.n_tiles = p.N * p.Dz * p.tiles_x * p.tiles_y;
   p.cin_chunks = c.Cin_pad / BKC; p.n_kz = c.n_kz; p.n_tap = c.n_tap; p.in_stride = c.in_stride;
   p.Cout = c.Cout; p.Dout = c.Dout; p.Hout = c.Hout; p.Wout = c.Wout; p.Cs_out = c.Cs_out; p.c_off = c.c_off;
   p.out_stride = c.out_stride; p.out_off_y = c.out_off_y; p.out_off_x = c.out_off_x; p.leaky = c.leaky;
@@ -473,7 +513,7 @@ int conv_wgmma(const WgConv& c, cudaStream_t st) {
       min_dx = c.dx[t] < min_dx ? c.dx[t] : min_dx; max_dx = c.dx[t] > max_dx ? c.dx[t] : max_dx;
     }
     pitch = TW + (max_dx - min_dx); halo_rows = TH + (max_dy - min_dy);
-    if (pitch > 16 || halo_rows > TH + 16) { p.halo = 0; pitch = TW; halo_rows = TH; }
+    if (pitch > TW + 16 || halo_rows > TH + 16) { p.halo = 0; pitch = TW; halo_rows = TH; }
     else {
       p.org_y = min_dy; p.org_x = min_dx;
       for (int t = 0; t < c.n_tap; ++t) p.a_off16[t] = (unsigned short)((((c.dy[t] - min_dy) * pitch + (c.dx[t] - min_dx)) * RB) >> 4);
@@ -482,7 +522,7 @@ int conv_wgmma(const WgConv& c, cudaStream_t st) {
   const uint32_t swz_mode = c.tf32 ? 1u : 2u;                    // 128-byte / 64-byte swizzle = one pixel row
   p.a_desc_hi = (uint32_t)((pitch * RB) >> 4) | (swz_mode << 30);  // SBO = one row of the (halo) tile
   p.b_desc_hi = (uint32_t)((8 * RB) >> 4) | (swz_mode << 30);
-  p.wg_row16 = (uint32_t)((8 * pitch * RB) >> 4);
+  p.wg_row16 = (uint32_t)((8 * (p.wide ? 1 : pitch) * RB) >> 4);   // 8 pixels right / 8 (halo) rows down
   p.box_w = pitch; p.box_h = halo_rows;
   p.a_tx_bytes = 2u * (uint32_t)(halo_rows * pitch * RB);
   p.a_tile_bytes = round_up((uint32_t)(halo_rows * pitch * RB), 1024);

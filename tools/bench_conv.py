@@ -1,6 +1,11 @@
 """Conv micro-benchmark at the real layer shapes of the 640x480 workload: fp32 FFMA implicit GEMM
 (nrgbd_conv_nhwc) vs wgmma 3xTF32 (nrgbd_conv_nhwc_tc, split time reported separately).
-CUDA events, 256 MiB L2 flush between iterations. Development aid."""
+CUDA events, 256 MiB L2 flush between iterations. Development aid.
+
+    python tools/bench_conv.py abflags [only=<name part>] [rounds=N] [out=<file.json>]
+times the split-fp16 convolution (nrgbd_conv_nhwc_h2) at each shape with all schedule features on (flags 0) and with
+each one switched off (8: 16 x 8 tile only, 32: one tile per CTA, 40: both), the arms
+alternating round by round, and writes the medians to the JSON file `out` (default: bench_conv_ab.json)."""
 import ctypes
 import json
 import os
@@ -99,6 +104,23 @@ def main():
                 return timeit(fn, iters)
             except _lib.NrgbdError:
                 return float('nan')
+        if 'abflags' in sys.argv:
+            arms = (0, 8, 32, 40)
+            rounds = int(next((a[7:] for a in sys.argv if a.startswith('rounds=')), 5))
+            ts = {a: [] for a in arms}
+            for _ in range(rounds):
+                for a in arms:
+                    L.nrgbd_dev_conv_h2_set_flags(a)
+                    ts[a].append(timeit(h2, 5))
+            L.nrgbd_dev_conv_h2_set_flags(0)
+            med = {a: float(np.median(v)) for a, v in ts.items()}
+            rec = dict(layer=name, gflop=flops / 1e9, us={str(a): med[a] for a in arms},
+                       tflops={str(a): flops / med[a] / 1e6 for a in arms},
+                       spread={str(a): float((max(v) - min(v)) / np.median(v)) for a, v in ts.items()},
+                       gain_vs_off={str(a): med[a] / med[0] - 1.0 for a in arms[1:]})
+            out.append(rec)
+            print(json.dumps(rec), flush=True)
+            continue
         if 'h2only' in sys.argv:
             t_h2 = safe(h2)
             print(json.dumps(dict(layer=name, h2_us=t_h2, h2_tflops=flops / t_h2 / 1e6)), flush=True)
@@ -113,6 +135,11 @@ def main():
                    h2_vs_simt_relerr=float((y - y4).abs().max() / y.abs().max()))
         out.append(rec)
         print(json.dumps(rec), flush=True)
+    if 'abflags' in sys.argv:
+        path = next((a[4:] for a in sys.argv[1:] if a.startswith('out=')), 'bench_conv_ab.json')
+        with open(path, 'w') as f:
+            json.dump(out, f, indent=1)
+        return
     os.makedirs('gpurun_out', exist_ok=True)
     json.dump(out, open('gpurun_out/bench_conv.json', 'w'), indent=1)
 
