@@ -258,6 +258,10 @@ int nrgbd_bn_apply_stats_pair(const float* x, double* stats, double count, const
  * Q has Cs >= kd*k*k floats per position; k = 3, kd in {1, 3}. */
 int nrgbd_tap_gather_sum(const float* Q, int N, int D, int H, int W, int Cs, int kd, int k, float bias, float* out,
                          nrgbd_stream_t stream);
+/* Eval-mode BatchNorm coefficients from the running statistics (only read), ATen's order of operations:
+ * scale = (1 / sqrt(running_var + eps)) * gamma, shift = beta - running_mean * scale, C channels. */
+int nrgbd_bn_eval_coeffs(const float* gamma, const float* beta, const float* running_mean, const float* running_var,
+                         float eps, int C, float* scale, float* shift, nrgbd_stream_t stream);
 /* y = [relu](x*scale + shift) [+ res] over n_pos positions of Cs channels (C logical). */
 int nrgbd_bn_apply(const float* x, const float* scale, const float* shift, const float* res, int relu,
                    long long n_pos, int Cs, int C, float* y, nrgbd_stream_t stream);
@@ -329,6 +333,19 @@ int nrgbd_conv_nhwc_h2_pair(const void* x_hi, const void* x_lo, int N, int Din, 
                             const void* w, const float* bias, int Cout, int Cout_pad, int BN, int kd, int kh, int kw, int stride,
                             int pad, int dilation, void* y_hi, void* y_lo, int Hout, int Wout, int Cs_out, int leaky,
                             nrgbd_stream_t stream);
+/* Eval-mode Conv + BatchNorm (running statistics) [+ residual] [+ ReLU] in ONE pass: nrgbd_conv_nhwc_h2 without bias whose
+ * epilogue computes, per output element, v = acc * scale[c] + shift[c]; v += residual (optional); v = max(v, 0) (relu != 0).
+ * scale / shift [Cout]: nrgbd_bn_eval_coeffs. The residual has the output's layout ([N][D][Hout][Wout][Cs_out], channels from
+ * c_off) and is either the fp32 tensor `res` or the operand pair (res_hi, res_lo: value hi + lo * 2^-11); at most one form.
+ * The output is either fp32 (y, channels [c_off, c_off + Cout)) or the split-fp16 operand pair of the next convolution
+ * (y_hi / y_lo as in nrgbd_conv_nhwc_h2_pair: Cs_out % 32 == 0, c_off == 0, pad channels stored as zeros). No statistics and
+ * no atomics: the output is identical from run to run. (K-Net's convbn_3d layers, models/basic.py:71-94, and the feature
+ * CNN's downsample shortcuts, models/psm_submodule.py:128-131, with the module in .eval().) */
+int nrgbd_conv_nhwc_h2_affine(const void* x_hi, const void* x_lo, int N, int Din, int Hin, int Win, int Cin_pad, int Cs_in,
+                              const void* w, int Cout, int Cout_pad, int BN, int kd, int kh, int kw, int stride, int pad,
+                              int dilation, const float* scale, const float* shift, const float* res, const void* res_hi,
+                              const void* res_lo, int relu, float* y, void* y_hi, void* y_lo, int Hout, int Wout, int Cs_out,
+                              int c_off, nrgbd_stream_t stream);
 int nrgbd_conv_transpose2d_k4s2_nhwc_h2(const void* x_hi, const void* x_lo, int N, int Hin, int Win, int Cin_pad, int Cs_in,
                                         const void* w, const float* bias, int Cout, int Cout_pad, int BN, float* y, int Cs_out,
                                         int c_off, int leaky, nrgbd_stream_t stream);
@@ -362,7 +379,7 @@ int nrgbd_kvnet_set_param(nrgbd_kvnet* e, const char* name, const float* data, l
 int nrgbd_kvnet_set_camera(nrgbd_kvnet* e, int slot, const float* K_host, const float* rays_host, float cx,
                            float cy, double hfov_deg, double vfov_deg);
 int nrgbd_kvnet_set_planes(nrgbd_kvnet* e, const float* d_host, int D);   /* float32(d_candi) */
-int nrgbd_kvnet_set_option(nrgbd_kvnet* e, const char* key, int value);   /* "bn_update_running", "profile", "conv_math" (0 fp32 FFMA, 1 wgmma 3xTF32, 2 wgmma split-fp16 pairs), "use_graph" (CUDA-graph replay, default 1) */
+int nrgbd_kvnet_set_option(nrgbd_kvnet* e, const char* key, int value);   /* "bn_update_running", "profile", "conv_math" (0 fp32 FFMA, 1 wgmma 3xTF32, 2 wgmma split-fp16 pairs), "use_graph" (CUDA-graph replay, default 1), "bn_eval" (1: the module is in .eval(): BatchNorm layers with running statistics normalise with them and update nothing, the others keep batch statistics; default 0) */
 /* with option "profile"=1 the engine brackets its conv (category 0, work = flops) and plane-sweep
  * (category 1, work = algorithmic bytes) launches with CUDA events; this returns and clears the sums. */
 int nrgbd_kvnet_profile_read(nrgbd_kvnet* e, int category, double* ms, double* work, long long* launches);

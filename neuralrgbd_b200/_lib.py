@@ -67,6 +67,9 @@ SIGNATURES = {
                                    c_vp]),
     'nrgbd_conv_nhwc_h2_pair': (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_int, c_int, c_int,
                                         c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp]),
+    'nrgbd_conv_nhwc_h2_affine': (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
+                                          c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp,
+                                          c_int, c_int, c_int, c_int, c_vp]),
     'nrgbd_conv_transpose2d_k4s2_nhwc_h2': (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_int, c_int,
                                                     c_int, c_vp, c_int, c_int, c_int, c_vp]),
     'nrgbd_bn_finalize': (c_int, [c_vp, c_int, ctypes.c_double, c_vp, c_vp, c_float, c_vp, c_vp, c_vp, c_vp,
@@ -76,6 +79,7 @@ SIGNATURES = {
     'nrgbd_tap_gather_sum': (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_vp, c_vp]),
     'nrgbd_bn_apply_stats_pair': (c_int, [c_vp, c_vp, ctypes.c_double, c_vp, c_vp, c_float, c_vp, c_vp, c_float, c_vp, c_vp, c_vp, c_int,
                                           c_ll, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    'nrgbd_bn_eval_coeffs': (c_int, [c_vp, c_vp, c_vp, c_vp, c_float, c_int, c_vp, c_vp, c_vp]),
     'nrgbd_bn_apply': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_ll, c_int, c_int, c_vp, c_vp]),
     'nrgbd_nchw_to_nhwc': (c_int, [c_vp, c_int, c_int, c_ll, c_vp, c_int, c_int, c_vp]),
     'nrgbd_nhwc_to_nchw': (c_int, [c_vp, c_int, c_int, c_ll, c_int, c_int, c_vp, c_vp]),

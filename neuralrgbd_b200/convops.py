@@ -336,6 +336,55 @@ def conv_h2_pair_out(x, w, bias=None, stride=1, pad=0, dilation=1, leaky=False):
     return from_cl(val.contiguous(), Cout), yh, yl
 
 
+def bn_eval_coeffs(gamma, beta, running_mean, running_var, eps=1e-5):
+    """Eval-mode BatchNorm coefficients on the device (nrgbd_bn_eval_coeffs) -> (scale, shift)."""
+    L = _lib.lib()
+    C = gamma.numel()
+    scale = torch.empty(C, device=gamma.device, dtype=torch.float32); shift = torch.empty_like(scale)
+    check(L.nrgbd_bn_eval_coeffs(ptr(gamma.float().contiguous()), ptr(beta.float().contiguous()), ptr(running_mean.float().contiguous()),
+                                 ptr(running_var.float().contiguous()), _F(eps), C, ptr(scale), ptr(shift), _st()))
+    return scale, shift
+
+
+def conv_h2_affine(x, w, scale, shift, stride=1, pad=0, dilation=1, res=None, res_pair=False, relu=False, pair_out=False):
+    """Eval-mode convbn in one kernel (nrgbd_conv_nhwc_h2_affine): relu(conv(x, w) * scale + shift + res). res (NCHW / NCDHW,
+    the output's shape) is passed as fp32 or, with res_pair, as its split-fp16 operand pair. pair_out: the result is written
+    only as the operand pair of the next convolution; returned as its fp32 value hi + lo * 2^-11 plus the raw (hi, lo)."""
+    L = _lib.lib()
+    is3d = x.dim() == 5
+    N = x.shape[0]
+    Din = x.shape[2] if is3d else 1
+    Hin, Win = x.shape[-2], x.shape[-1]
+    Cout = w.shape[0]
+    wp, Cin_pad, Cout_pad, BN = pack_weight_h2(w)
+    xh, xl = split_f16_pair(to_cl_padded(x, Cin_pad))
+    kd = w.shape[2] if is3d else 1
+    kh, kw = w.shape[-2], w.shape[-1]
+    Ho = (Hin + 2 * pad - dilation * (kh - 1) - 1) // stride + 1
+    Wo = (Win + 2 * pad - dilation * (kw - 1) - 1) // stride + 1
+    Cs = pad_to(Cout, 32) if pair_out else pad4(Cout)
+    shape = (N,) + ((Din,) if is3d else ()) + (Ho, Wo, Cs)
+    r = rh = rl = None
+    if res is not None:
+        rc = to_cl_padded(res, Cs)
+        if res_pair:
+            rh, rl = split_f16_pair(rc)
+        else:
+            r = rc
+    y = yh = yl = None
+    if pair_out:
+        yh = torch.full(shape, float('nan'), device=x.device, dtype=torch.float16)     # every element must be written
+        yl = torch.full(shape, float('nan'), device=x.device, dtype=torch.float16)
+    else:
+        y = torch.zeros(shape, device=x.device, dtype=torch.float32)
+    check(L.nrgbd_conv_nhwc_h2_affine(ptr(xh), ptr(xl), N, Din, Hin, Win, Cin_pad, Cin_pad, ptr(wp), Cout, Cout_pad, BN, kd, kh, kw,
+                                      stride, pad, dilation, ptr(scale), ptr(shift), ptr(r), ptr(rh), ptr(rl), 1 if relu else 0,
+                                      ptr(y), ptr(yh), ptr(yl), Ho, Wo, Cs, 0, _st()))
+    if pair_out:
+        return from_cl((yh.float() + yl.float() * (1.0 / 2048.0)).contiguous(), Cout), yh, yl
+    return from_cl(y, Cout)
+
+
 def conv_cout1_h2(x, w, bias=0.0):
     """Single-output-channel k3 convolution (K-Net's last layer, models/basic.py:136-137) the way the engine runs it:
     a pointwise f16-pair conv to one channel per tap + nrgbd_tap_gather_sum. x [N, C, D, H, W] (or [N, C, H, W]),

@@ -45,6 +45,22 @@ static inline int nrgbd_sm_count() {
   return n;
 }
 
+// Eval-mode BatchNorm coefficients of several layers in one launch (conv.cu): per layer l and channel c < C[l],
+// scale = (1 / sqrt(var + eps)) * gamma, shift = beta - mean * scale, from the running statistics (only read).
+constexpr int NRGBD_BN_EVAL_MAX = 16;
+struct BnEvalTable {
+  const float* gamma[NRGBD_BN_EVAL_MAX];
+  const float* beta[NRGBD_BN_EVAL_MAX];
+  const float* mean[NRGBD_BN_EVAL_MAX];
+  const float* var[NRGBD_BN_EVAL_MAX];
+  float* scale[NRGBD_BN_EVAL_MAX];
+  float* shift[NRGBD_BN_EVAL_MAX];
+  int C[NRGBD_BN_EVAL_MAX];
+  int n;
+  float eps;
+};
+int bn_eval_coeffs(const BnEvalTable& t, cudaStream_t st);
+
 // launch counter (bench.py reports it as gpu_launches)
 extern "C" void nrgbd_count_launch(int n);
 #define NRGBD_COUNT(n) nrgbd_count_launch(n)

@@ -262,6 +262,18 @@ __global__ void bn_finalize_kernel(const double* __restrict__ stats, int C, doub
   }
 }
 
+// Eval-mode coefficients (ATen's CPU order: invstd = 1 / sqrt(var + eps), scale = invstd * gamma, shift = beta - mean * scale),
+// one block per layer
+__global__ void bn_eval_coeffs_kernel(const BnEvalTable t) {
+  const int l = blockIdx.x;
+  for (int c = threadIdx.x; c < t.C[l]; c += blockDim.x) {
+    const float invstd = __fdiv_rn(1.f, __fsqrt_rn(__fadd_rn(t.var[l][c], t.eps)));
+    const float sc = __fmul_rn(invstd, t.gamma[l][c]);
+    t.scale[l][c] = sc;
+    t.shift[l][c] = __fsub_rn(t.beta[l][c], __fmul_rn(t.mean[l][c], sc));
+  }
+}
+
 // y = act(x * scale[c] + shift[c]) (+ res), channels-last with stride Cs; pad channels stay 0.
 __global__ void __launch_bounds__(256)
 bn_apply_kernel(const float* __restrict__ x, const float* __restrict__ scale, const float* __restrict__ shift,
@@ -420,6 +432,14 @@ int g_bn_unroll = 0;           // development override of the vectors in flight 
 int g_bn_blocks_per_sm = 0;    // development override of the grid cap in blocks per SM (0 = by size; nrgbd_dev_set_bn_blocks_per_sm)
 
 }  // namespace
+
+int bn_eval_coeffs(const BnEvalTable& t, cudaStream_t st) {
+  NRGBD_REQUIRE(t.n >= 1 && t.n <= NRGBD_BN_EVAL_MAX, "bad layer count");
+  bn_eval_coeffs_kernel<<<t.n, 128, 0, st>>>(t);
+  NRGBD_COUNT(1);
+  NRGBD_LAUNCH_CHECK();
+  return NRGBD_OK;
+}
 
 extern "C" {
 
@@ -606,6 +626,15 @@ int nrgbd_tap_gather_sum(const float* Q, int N, int D, int H, int W, int Cs, int
 }
 
 // y = [relu](x*scale + shift) [+ res]; n_pos positions of Cs channels (C logical). In place allowed.
+int nrgbd_bn_eval_coeffs(const float* gamma, const float* beta, const float* running_mean, const float* running_var, float eps, int C,
+                         float* scale, float* shift, cudaStream_t st) {
+  NRGBD_REQUIRE(gamma && beta && running_mean && running_var && scale && shift && C > 0, "bad arguments");
+  BnEvalTable t{};
+  t.gamma[0] = gamma; t.beta[0] = beta; t.mean[0] = running_mean; t.var[0] = running_var;
+  t.scale[0] = scale; t.shift[0] = shift; t.C[0] = C; t.n = 1; t.eps = eps;
+  return bn_eval_coeffs(t, st);
+}
+
 int nrgbd_bn_apply(const float* x, const float* scale, const float* shift, const float* res, int relu,
                    long long n_pos, int Cs, int C, float* y, cudaStream_t st) {
   NRGBD_REQUIRE(x && scale && shift && y && Cs % 4 == 0 && C <= Cs && n_pos > 0, "bad arguments");

@@ -25,7 +25,9 @@
 //               a_lo x b_hi -> cross; the ring slots of step s are released once step s + 1 is issued and step s has
 //               retired (wgmma.wait_group 1), the last step's at the end of the tile; then the epilogue straight from the
 //               registers: main + scale * cross, bias / LeakyReLU, fp32 or fp16-pair stores, BatchNorm column sums
-//               (summed per CTA over its tiles, then one pair of fp64 atomics per column and CTA).
+//               (summed per CTA over its tiles, then one pair of fp64 atomics per column and CTA). The affine form (AFF,
+//               eval-mode BatchNorm with fixed coefficients) applies per-channel scale / shift, an optional residual and
+//               ReLU instead, and accumulates nothing: no atomics, the same output on every run.
 //               (a_hi x [b_hi | b_lo] as one wgmma of N = 2 BN would read a_hi once, but its accumulators overlap those of
 //               a_lo x b_hi in part, and ptxas then serialises every wgmma (C7511): 8-15 % slower on H100.)
 //   warp 8      TMA producer: halo / tap box of the hi and the lo activation planes into the A ring, G taps of the hi and
@@ -47,6 +49,9 @@ constexpr int BKC = 32;                // input channels per K chunk
 struct WgParams {
   float* y; const float* bias; double* stats;
   __half *y_hi, *y_lo;
+  const float *aff_scale, *aff_shift, *res;   // affine epilogue (AFF instantiations only)
+  const __half *res_hi, *res_lo;
+  int relu;
   int N, Dz, Hy, Wx, tiles_x, tiles_y, n_tiles, wide;   // wide: 8 x 16 output tile (else 16 x 8)
   int cin_chunks, n_kz, n_tap, halo, in_stride, org_y, org_x;
   int Cout, c_first;                     // logical output channels; first channel of this launch's chunk 0
@@ -107,8 +112,8 @@ __device__ __forceinline__ void wg_mma(float* d, uint64_t a, uint64_t b) {
 }
 
 // BN: output channels per CTA (16..128). TF32: operand kind. G: in-plane taps per pipeline step (one weight box and one
-// barrier round trip per G taps).
-template <int BN, bool TF32, int G>
+// barrier round trip per G taps). AFF: affine epilogue (see WgConv).
+template <int BN, bool TF32, int G, bool AFF>
 __global__ void __launch_bounds__(WG_THREADS, BN <= 64 ? 2 : 1)
 conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo, const WgParams p) {
@@ -136,6 +141,11 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (threadIdx.x < 2 * BN) cta_sums[threadIdx.x] = 0.0;
+  if constexpr (AFF) {
+    // the affine form keeps no column sums: the partial-sum area holds this CTA's scale [BN] | shift [BN] instead
+    const int c0 = p.c_first + (int)blockIdx.y * BN, t = threadIdx.x % BN;
+    if (threadIdx.x < 2 * BN) part[threadIdx.x] = c0 + t < p.Cout ? __ldg((threadIdx.x < BN ? p.aff_scale : p.aff_shift) + c0 + t) : 0.f;
+  }
   __syncthreads();
 
   // Persistent CTAs: tiles blockIdx.x, blockIdx.x + gridDim.x, ... The rings and their phases run on across tiles, so
@@ -256,6 +266,12 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
       pix[i] = (((long long)n0 * p.Dout + z0) * p.Hout + oy) * p.Wout + ox;
       if (!pair) dst_row[i] = p.y + pix[i] * (long long)p.Cs_out + p.c_off + cbase;
     }
+    if constexpr (AFF) {
+      // main + scale * cross for every column first: the cross accumulators die here, which leaves registers for the
+      // residual loads of the store loop (no spills at BN = 64)
+#pragma unroll
+      for (int k = 0; k < BN / 2; ++k) acc_m[k] = fmaf(acc_c[k], SCALE, acc_m[k]);
+    }
     constexpr int NJ_PAIR = ((BN + 31) / 32) * 4;     // pair output: pad channels up to the next 32 are stored as zeros
     const int nj_store = pair ? NJ_PAIR : NJ;
 #pragma unroll
@@ -269,15 +285,31 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
         for (int e = 0; e < 2; ++e) {
           float f = 0.f;
           if (j < NJ && c + e < n_here && valid[i]) {
-            f = fmaf(acc_c[4 * j + 2 * i + e], SCALE, acc_m[4 * j + 2 * i + e]);
-            if (p.bias) f += __ldg(p.bias + cbase + c + e);
-            if (p.leaky) f = f >= 0.f ? f : f * 0.01f;
+            if constexpr (AFF) {
+              f = fmaf(acc_m[4 * j + 2 * i + e], part[c + e], part[BN + c + e]);      // residual and ReLU: in the store loop below
+            } else {
+              f = fmaf(acc_c[4 * j + 2 * i + e], SCALE, acc_m[4 * j + 2 * i + e]);
+              if (p.bias) f += __ldg(p.bias + cbase + c + e);
+              if (p.leaky) f = f >= 0.f ? f : f * 0.01f;
+            }
           }
           v[i][e] = f;
         }
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         if (!valid[i]) continue;
+        if constexpr (AFF) {
+          // residual (the output's layout: the pair output has c_off 0, so o is also the store offset), then ReLU
+          const long long o = pix[i] * (long long)p.Cs_out + p.c_off + cbase + c;
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            if (j < NJ && c + e < n_here) {
+              if (p.res) v[i][e] += __ldg(p.res + o + e);
+              else if (p.res_hi) v[i][e] += fmaf(__half2float(p.res_lo[o + e]), 1.f / 2048.f, __half2float(p.res_hi[o + e]));
+              if (p.relu) v[i][e] = fmaxf(v[i][e], 0.f);
+            }
+          }
+        }
         if (pair) {
           __half h0, l0, h1, l1;
           nrgbd_split_pair(v[i][0], h0, l0); nrgbd_split_pair(v[i][1], h1, l1);
@@ -291,7 +323,7 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
           if (c + 1 < n_here) dst_row[i][c + 1] = v[i][1];
         }
       }
-      if (p.stats && j < NJ) {
+      if (!AFF && p.stats && j < NJ) {
         // column sums over this warp's 16 rows: the thread's two rows, then across the 8 lane quads
         float s1[2], s2[2];
 #pragma unroll
@@ -310,7 +342,7 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
         }
       }
     }
-    if (p.stats) {
+    if (!AFF && p.stats) {
       asm volatile("bar.sync 1, 256;" ::: "memory");
       const int c = threadIdx.x;
       if (c < n_here) {
@@ -323,7 +355,7 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
     }
   }
   const int c = threadIdx.x;
-  if (p.stats && c < min(BN, p.Cout - cbase) && (int)blockIdx.x < p.n_tiles) {
+  if (!AFF && p.stats && c < min(BN, p.Cout - cbase) && (int)blockIdx.x < p.n_tiles) {
     atomicAdd(p.stats + cbase + c, cta_sums[c]);
     atomicAdd(p.stats + p.Cout + cbase + c, cta_sums[BN + c]);
   }
@@ -405,17 +437,17 @@ inline uint32_t round_up(uint32_t v, uint32_t m) { return (v + m - 1) / m * m; }
 
 typedef void (*WgKernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const WgParams);
 
-template <bool TF32, int G>
+template <bool TF32, int G, bool AFF = false>
 WgKernel pick_kernel(int BN) {
   switch (BN) {
-    case 16: return conv_wg_kernel<16, TF32, G>;
-    case 32: return conv_wg_kernel<32, TF32, G>;
-    case 48: return conv_wg_kernel<48, TF32, G>;
-    case 64: return conv_wg_kernel<64, TF32, G>;
-    case 80: return conv_wg_kernel<80, TF32, G>;
-    case 96: return conv_wg_kernel<96, TF32, G>;
-    case 112: return conv_wg_kernel<112, TF32, G>;
-    case 128: return conv_wg_kernel<128, TF32, G>;
+    case 16: return conv_wg_kernel<16, TF32, G, AFF>;
+    case 32: return conv_wg_kernel<32, TF32, G, AFF>;
+    case 48: return conv_wg_kernel<48, TF32, G, AFF>;
+    case 64: return conv_wg_kernel<64, TF32, G, AFF>;
+    case 80: return conv_wg_kernel<80, TF32, G, AFF>;
+    case 96: return conv_wg_kernel<96, TF32, G, AFF>;
+    case 112: return conv_wg_kernel<112, TF32, G, AFF>;
+    case 128: return conv_wg_kernel<128, TF32, G, AFF>;
   }
   return nullptr;
 }
@@ -460,10 +492,14 @@ int launch_chunks(const WgConv& c, WgParams p, int BN, int n_chunks, int c_first
   rc = encode_act_map(&ta_hi, c.x_hi, esize, c.N, c.Din, c.Hin, c.Win, c.Cin_pad, c.Cs_in, p.box_w, p.box_h, p.in_stride);
   if (rc == NRGBD_OK) rc = encode_act_map(&ta_lo, c.x_lo, esize, c.N, c.Din, c.Hin, c.Win, c.Cin_pad, c.Cs_in, p.box_w, p.box_h, p.in_stride);
   if (rc != NRGBD_OK) return rc;
-  WgKernel fn = tf32 ? (G == 3 ? pick_kernel<true, 3>(BN) : pick_kernel<true, 1>(BN)) : (G == 3 ? pick_kernel<false, 3>(BN) : pick_kernel<false, 1>(BN));
+  const bool aff = p.aff_scale != nullptr;
+  if (aff && tf32) { nrgbd_set_error("conv_wgmma: the affine epilogue is built for split-fp16 operands only"); return NRGBD_ERR_UNSUPPORTED; }
+  WgKernel fn = aff ? (G == 3 ? pick_kernel<false, 3, true>(BN) : pick_kernel<false, 1, true>(BN))
+                    : tf32 ? (G == 3 ? pick_kernel<true, 3>(BN) : pick_kernel<true, 1>(BN))
+                           : (G == 3 ? pick_kernel<false, 3>(BN) : pick_kernel<false, 1>(BN));
   if (!fn) { nrgbd_set_error("conv_wgmma: unsupported chunk width %d", BN); return NRGBD_ERR_UNSUPPORTED; }
-  static size_t configured[2][2][8] = {};
-  size_t& conf = configured[tf32][G == 3][BN / 16 - 1];
+  static size_t configured[2][2][2][8] = {};
+  size_t& conf = configured[aff][tf32][G == 3][BN / 16 - 1];
   if (smem > conf) {
     cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { nrgbd_set_error("conv_wgmma: cannot opt in to %zu bytes of shared memory: %s", smem, cudaGetErrorString(e)); return NRGBD_ERR_CUDA; }
@@ -489,6 +525,8 @@ int conv_wgmma(const WgConv& c, cudaStream_t st) {
   WgParams p{};
   p.y = c.y; p.bias = c.bias; p.stats = c.stats;
   p.y_hi = reinterpret_cast<__half*>(c.y_hi); p.y_lo = reinterpret_cast<__half*>(c.y_lo);
+  p.aff_scale = c.aff_scale; p.aff_shift = c.aff_shift; p.res = c.res; p.relu = c.relu;
+  p.res_hi = reinterpret_cast<const __half*>(c.res_hi); p.res_lo = reinterpret_cast<const __half*>(c.res_lo);
   p.N = c.N; p.Dz = c.Din; p.Hy = c.Hy; p.Wx = c.Wx;
   // output tile 8 x 16 when it pads fewer positions than 16 x 8 (120-row planes), else 16 x 8
   const long long pad_tall = (long long)ceil_div(c.Hy, 16) * ceil_div(c.Wx, 8), pad_wide = (long long)ceil_div(c.Hy, 8) * ceil_div(c.Wx, 16);
@@ -616,7 +654,8 @@ int nrgbd_pack_conv_weight_h2(const float* w, int transposed, int Cout, int Cin,
 
 static int conv_nhwc_h2_impl(const void* x_hi, const void* x_lo, int N, int Din, int Hin, int Win, int Cin_pad, int Cs_in, const void* w,
                              const float* bias, int Cout, int Cout_pad, int BN, int kd, int kh, int kw, int stride, int pad, int dilation, float* y,
-                             void* y_hi, void* y_lo, int Hout, int Wout, int Cs_out, int c_off, int leaky, double* stats, cudaStream_t st);
+                             void* y_hi, void* y_lo, int Hout, int Wout, int Cs_out, int c_off, int leaky, double* stats, cudaStream_t st,
+                             const WgConv* aff = nullptr);
 
 int nrgbd_conv_nhwc_h2(const void* x_hi, const void* x_lo, int N, int Din, int Hin, int Win, int Cin_pad, int Cs_in, const void* w,
                        const float* bias, int Cout, int Cout_pad, int BN, int kd, int kh, int kw, int stride, int pad, int dilation, float* y,
@@ -640,7 +679,8 @@ int nrgbd_conv_nhwc_h2_pair(const void* x_hi, const void* x_lo, int N, int Din, 
 
 static int conv_nhwc_h2_impl(const void* x_hi, const void* x_lo, int N, int Din, int Hin, int Win, int Cin_pad, int Cs_in, const void* w,
                              const float* bias, int Cout, int Cout_pad, int BN, int kd, int kh, int kw, int stride, int pad, int dilation, float* y,
-                             void* y_hi, void* y_lo, int Hout, int Wout, int Cs_out, int c_off, int leaky, double* stats, cudaStream_t st) {
+                             void* y_hi, void* y_lo, int Hout, int Wout, int Cs_out, int c_off, int leaky, double* stats, cudaStream_t st,
+                             const WgConv* aff) {
   NRGBD_REQUIRE(x_hi && x_lo && w, "null pointer");
   NRGBD_REQUIRE(Cin_pad % 32 == 0 && Cin_pad >= 32 && Cin_pad <= Cs_in && Cs_in % 8 == 0 && Cout_pad % 16 == 0 && Cout <= Cout_pad && Cout > Cout_pad - 16 &&
                     BN == (Cout_pad < 128 ? Cout_pad : 128), "channel counts not supported by the f16-pair tensor-core path");
@@ -660,6 +700,7 @@ static int conv_nhwc_h2_impl(const void* x_hi, const void* x_lo, int N, int Din,
   c.bias = bias; c.stats = stats; c.y = y; c.y_hi = y_hi; c.y_lo = y_lo;
   c.Cout = Cout; c.Dout = Din; c.Hout = Hout; c.Wout = Wout; c.Cs_out = Cs_out; c.c_off = c_off;
   c.out_stride = 1; c.out_off_y = 0; c.out_off_x = 0; c.leaky = leaky;
+  if (aff) { c.aff_scale = aff->aff_scale; c.aff_shift = aff->aff_shift; c.res = aff->res; c.res_hi = aff->res_hi; c.res_lo = aff->res_lo; c.relu = aff->relu; }
   c.Hy = Hout; c.Wx = Wout; c.in_stride = stride; c.n_kz = kd; c.n_tap = kh * kw;
   for (int a = 0; a < kd; ++a) c.dz[a] = (signed char)(a - kd / 2);
   int t = 0;
@@ -671,6 +712,22 @@ static int conv_nhwc_h2_impl(const void* x_hi, const void* x_lo, int N, int Din,
   NRGBD_COUNT(1);
   NRGBD_LAUNCH_CHECK();
   return NRGBD_OK;
+}
+
+// Eval-mode convbn in one pass: the convolution, then per output channel v = acc * scale + shift (+ residual) (ReLU), written
+// either as fp32 (y, channel offset c_off) or as the operand pair of the next convolution (y_hi / y_lo, as
+// nrgbd_conv_nhwc_h2_pair). No bias, no statistics.
+int nrgbd_conv_nhwc_h2_affine(const void* x_hi, const void* x_lo, int N, int Din, int Hin, int Win, int Cin_pad, int Cs_in, const void* w,
+                              int Cout, int Cout_pad, int BN, int kd, int kh, int kw, int stride, int pad, int dilation,
+                              const float* scale, const float* shift, const float* res, const void* res_hi, const void* res_lo, int relu,
+                              float* y, void* y_hi, void* y_lo, int Hout, int Wout, int Cs_out, int c_off, cudaStream_t st) {
+  NRGBD_REQUIRE(scale && shift, "null scale / shift");
+  NRGBD_REQUIRE((y != nullptr) != (y_hi != nullptr) && (y_hi == nullptr) == (y_lo == nullptr), "the output is either fp32 (y) or a pair (y_hi, y_lo)");
+  NRGBD_REQUIRE((res_hi == nullptr) == (res_lo == nullptr) && !(res && res_hi), "the residual is either an fp32 tensor or an operand pair");
+  WgConv aff{};
+  aff.aff_scale = scale; aff.aff_shift = shift; aff.res = res; aff.res_hi = res_hi; aff.res_lo = res_lo; aff.relu = relu ? 1 : 0;
+  return conv_nhwc_h2_impl(x_hi, x_lo, N, Din, Hin, Win, Cin_pad, Cs_in, w, nullptr, Cout, Cout_pad, BN, kd, kh, kw, stride, pad, dilation, y,
+                           y_hi, y_lo, Hout, Wout, Cs_out, c_off, 0, nullptr, st, &aff);
 }
 
 // nn.ConvTranspose2d(kernel 4, stride 2, padding 1) as four output-parity classes of 2x2-tap convolutions

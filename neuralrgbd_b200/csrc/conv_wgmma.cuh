@@ -23,6 +23,12 @@ struct WgConv {
   float* y;                              // fp32 output [N][Dout][Hout][Wout][Cs_out] at channel offset c_off ...
   void *y_hi, *y_lo;                     // ... or (when non-null) the fp16 operand pair of the next convolution
   int Cout, Dout, Hout, Wout, Cs_out, c_off, out_stride, out_off_y, out_off_x, leaky;
+  // affine epilogue (split-fp16 only; replaces bias / LeakyReLU / statistics when aff_scale is set):
+  // v = acc * aff_scale[c] + aff_shift[c], + residual (fp32 `res`, or the pair res_hi + res_lo * 2^-11, laid out like the output),
+  // then max(v, 0) when relu
+  const float *aff_scale, *aff_shift, *res;
+  const void *res_hi, *res_lo;
+  int relu;
   int Hy, Wx, in_stride;                 // output positions per plane (before the parity interleave), conv stride
   int n_kz, n_tap;                       // depth taps, in-plane taps
   signed char dz[3], dy[WG_MAX_TAP2D], dx[WG_MAX_TAP2D];

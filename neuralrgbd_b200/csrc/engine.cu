@@ -7,6 +7,7 @@
 // stream: no Python between layers, no allocation after warm-up, activations channels-last.
 // Parameters are registered by their reference state_dict names (borrowed device pointers or
 // engine-owned copies of host arrays), so kvnet_*.tar checkpoints map one to one.
+#include <algorithm>
 #include <array>
 #include <cmath>
 #include <cstdio>
@@ -76,6 +77,9 @@ struct nrgbd_kvnet {
   float sigma;
   int metric = 0;
   int bn_update_running = 1;
+  int bn_eval = 0;                  // the module is in .eval(): BatchNorm layers with running statistics normalise with them
+  float* eval_coef = nullptr;       // [NRGBD_BN_EVAL_MAX][scale 512 | shift 512] of those layers, recomputed by every forward
+  std::unordered_map<std::string, int> eval_slot;   // BatchNorm prefix -> row of eval_coef (empty in train mode)
   std::unordered_map<std::string, ParamRef> params;
   std::unordered_map<std::string, Packed> packed;
   std::unordered_map<std::string, PackedTc> packed_tc;
@@ -378,6 +382,101 @@ Act conv(Eng* e, const Act& x, const std::string& wname, int Cout, int kd, int k
   return y;
 }
 
+// Eval mode: scale / shift of every BatchNorm that tracks running statistics (its running_mean is registered), computed on
+// the device by one launch at the start of each forward. The launch is part of the captured graph, so a replay reads the
+// running statistics as they are then (a train-mode forward in between may have updated them in place).
+void eval_coeffs(Eng* e) {
+  e->eval_slot.clear();
+  if (!e->bn_eval || e->rc) return;
+  const std::string suf = ".running_mean";
+  std::vector<std::string> pres;
+  for (auto& kv : e->params) {
+    const std::string& k = kv.first;
+    if (k.size() > suf.size() && k.compare(k.size() - suf.size(), suf.size(), suf) == 0) pres.push_back(k.substr(0, k.size() - suf.size()));
+  }
+  if (pres.empty()) return;
+  if ((int)pres.size() > NRGBD_BN_EVAL_MAX) {
+    nrgbd_set_error("engine: %d BatchNorm layers with running statistics, at most %d supported", (int)pres.size(), NRGBD_BN_EVAL_MAX);
+    e->rc = NRGBD_ERR_UNSUPPORTED; return;
+  }
+  std::sort(pres.begin(), pres.end());
+  BnEvalTable t{};
+  t.n = (int)pres.size(); t.eps = 1e-5f;
+  for (int i = 0; i < t.n; ++i) {
+    const std::string& pre = pres[i];
+    t.gamma[i] = param(e, pre + ".weight"); t.beta[i] = param(e, pre + ".bias");
+    t.mean[i] = param(e, pre + ".running_mean"); t.var[i] = param(e, pre + ".running_var");
+    if (e->rc) return;
+    t.C[i] = (int)e->params[pre + ".weight"].n;
+    if (t.C[i] > 512 || e->params[pre + ".running_mean"].n != t.C[i] || e->params[pre + ".running_var"].n != t.C[i]) {
+      nrgbd_set_error("engine: BatchNorm '%s' has inconsistent or more than 512 channels", pre.c_str());
+      e->rc = NRGBD_ERR_BAD_ARG; return;
+    }
+    t.scale[i] = e->eval_coef + (size_t)i * 1024; t.shift[i] = t.scale[i] + 512;
+    e->eval_slot[pre] = i;
+  }
+  ENG_CALL(e, bn_eval_coeffs(t, e->st));
+}
+
+// eval-mode scale of BatchNorm `pre` (its shift is 512 floats further), or null: train mode, or a layer without running
+// statistics (it keeps batch statistics in eval mode too)
+const float* eval_coef(Eng* e, const std::string& pre) {
+  auto it = e->eval_slot.find(pre);
+  return it == e->eval_slot.end() ? nullptr : e->eval_coef + (size_t)it->second * 1024;
+}
+
+// Eval-mode Conv (no bias) + BatchNorm(running statistics) [+ residual] [+ ReLU] of a tracked layer. f16-pair mode: ONE
+// convolution with the affine epilogue, written as the operand pair of the next convolution when only convolutions read it
+// (out_use 2), else as fp32. Other modes: the convolution without statistics, then nrgbd_bn_apply. No statistic is read or
+// written, no running buffer updated.
+Act convbn_eval(Eng* e, const Act& x, const std::string& wname, int Cout, int kd, int k, int stride, int pad, int dil, bool relu,
+                const Act* res, int out_use, const float* scale) {
+  const float* shift = scale + 512;
+  if (use_h2(e, x)) {
+    const int Ho = (x.H + 2 * pad - dil * (k - 1) - 1) / stride + 1, Wo = (x.W + 2 * pad - dil * (k - 1) - 1) / stride + 1;
+    const PackedH2* ph = packw_h2(e, wname, Cout, x.C, kd * k * k, false);
+    const PairBuf* pin = pair_of(e, x);
+    Act y;
+    if (e->rc) return y;
+    PairBuf pb; pb.hi = pb.lo = nullptr;
+    if (out_use == 2) {
+      y.N = x.N; y.D = x.D; y.H = Ho; y.W = Wo; y.C = Cout; y.Cs = pad32(Cout); y.pair_only = true;
+      y.p = e->pool.acquire(16);                                    // key of the pair buffers
+      pb.hi = e->pool.acquire((size_t)y.floats() * 2);
+      pb.lo = e->pool.acquire((size_t)y.floats() * 2);
+      if (!y.p || !pb.hi || !pb.lo) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; return y; }
+      e->pairs[y.p] = pb;
+    } else {
+      y = acquire(e, x.N, x.D, Ho, Wo, Cout);
+      if (e->rc) return y;
+    }
+    const float* res_f = nullptr;
+    const void *res_hi = nullptr, *res_lo = nullptr;
+    if (res) {
+      if (res->Cs != y.Cs || res->pos() != y.pos()) { nrgbd_set_error("engine: residual layout differs from the output's"); e->rc = NRGBD_ERR_BAD_ARG; return y; }
+      if (res->pair_only) {
+        auto it = e->pairs.find(res->p);
+        if (it == e->pairs.end()) { nrgbd_set_error("engine: residual has neither an fp32 copy nor an operand pair"); e->rc = NRGBD_ERR_BAD_ARG; return y; }
+        res_hi = it->second.hi; res_lo = it->second.lo;
+      } else {
+        res_f = res->p;
+      }
+    }
+    char tag[56];
+    snprintf(tag, sizeof(tag), "conv%dd k%d s%d d%d %d->%d %dx%dx%dx%d", kd > 1 ? 3 : 2, k, stride, dil, x.C, Cout, x.N, x.D, Ho, Wo);
+    ProfScope ps(e, 0, 2.0 * (double)x.N * x.D * Ho * Wo * Cout * x.C * kd * k * k, tag);
+    ENG_CALL(e, nrgbd_conv_nhwc_h2_affine(pin->hi, pin->lo, x.N, x.D, x.H, x.W, ph->Cin_pad, x.Cs, ph->w, Cout, ph->Cout_pad, ph->BN, kd, k, k,
+                                          stride, pad, dil, scale, shift, res_f, res_hi, res_lo, relu ? 1 : 0, out_use == 2 ? nullptr : y.p,
+                                          pb.hi, pb.lo, Ho, Wo, y.Cs, 0, (nrgbd_stream_t)e->st));
+    return y;
+  }
+  if (res && res->pair_only) { nrgbd_set_error("engine: residual exists only as an operand pair"); e->rc = NRGBD_ERR_BAD_ARG; return Act(); }
+  Act y = conv(e, x, wname, Cout, kd, k, stride, pad, dil, nullptr, false, false);
+  if (!e->rc)
+    ENG_CALL(e, nrgbd_bn_apply(y.p, scale, shift, res ? res->p : nullptr, relu ? 1 : 0, y.pos(), y.Cs, y.C, y.p, (nrgbd_stream_t)e->st));
+  return y;
+}
+
 // Conv (no bias) + BatchNorm(batch statistics) [+ ReLU] [+ residual]; BN applied in place.
 // `pre` is the Sequential(Conv, BN) prefix: weights pre.0.weight, pre.1.{weight,bias,running_*}.
 // out_use (f16-pair mode only): 0 = the result is read as fp32 only; 1 = also by a convolution (the BatchNorm pass emits the
@@ -387,6 +486,7 @@ Act conv(Eng* e, const Act& x, const std::string& wname, int Cout, int kd, int k
 Act convbn(Eng* e, const Act& x, const std::string& pre, int Cout, int kd, int k, int stride, int pad, int dil,
            bool relu, const Act* res, int out_use = 0) {
   int p = (kd == 1 && dil > 1) ? dil : pad;          // psm_submodule.convbn :13
+  if (const float* sc = eval_coef(e, pre + ".1")) return convbn_eval(e, x, pre + ".0.weight", Cout, kd, k, stride, p, dil, relu, res, out_use, sc);
   Act y = conv(e, x, pre + ".0.weight", Cout, kd, k, stride, p, dil, nullptr, false, true);
   float* g = param(e, pre + ".1.weight");
   float* b = param(e, pre + ".1.bias");
@@ -438,7 +538,11 @@ Act basic_block(Eng* e, Act& x, const std::string& pre, int planes, int stride, 
   if (fused) t = conv(e, x, pre + ".conv1.0.0.weight", planes, 1, 3, stride, p1, dil, nullptr, false, true, nullptr, 0, -1, e->stats_b);
   else t = convbn(e, x, pre + ".conv1.0", planes, 1, 3, stride, 1, dil, true, nullptr, 2);
   Act sc; const Act* res = &x;
-  if (down) {
+  const float* down_eval = down ? eval_coef(e, pre + ".downsample.1") : nullptr;
+  if (down_eval) {
+    sc = convbn_eval(e, x, pre + ".downsample.0.weight", planes, 1, 1, stride, 0, 1, false, nullptr, 0, down_eval);
+    res = &sc;
+  } else if (down) {
     // downsample = Sequential(Conv2d 1x1 stride, BatchNorm2d) :125-131 -> names downsample.0 / downsample.1
     sc = conv(e, x, pre + ".downsample.0.weight", planes, 1, 1, stride, 0, 1, nullptr, false, true);
     float* g = param(e, pre + ".downsample.1.weight"); float* b = param(e, pre + ".downsample.1.bias");
@@ -731,6 +835,7 @@ int nrgbd_kvnet_create(int H, int W, int D, int V, int feature_dim, int kv_featu
             cudaMalloc((void**)&e->bn_counter, sizeof(unsigned int)) == cudaSuccess &&
             cudaMalloc((void**)&e->scale, sizeof(float) * 512) == cudaSuccess &&
             cudaMalloc((void**)&e->shift, sizeof(float) * 512) == cudaSuccess &&
+            cudaMalloc((void**)&e->eval_coef, sizeof(float) * 1024 * NRGBD_BN_EVAL_MAX) == cudaSuccess &&
             cudaMalloc((void**)&e->ws_sweep, sizeof(float) * 12 * V) == cudaSuccess &&
             cudaMalloc((void**)&e->bv_cur_hwd, sizeof(float) * hw * D) == cudaSuccess &&
             cudaMalloc((void**)&e->dpv_hwd, sizeof(float) * hw * D) == cudaSuccess &&
@@ -750,7 +855,7 @@ int nrgbd_kvnet_destroy(nrgbd_kvnet* e) {
   for (auto& kv : e->packed_tc) { cudaFree(kv.second.hi); cudaFree(kv.second.lo); }
   for (auto& kv : e->packed_h2) cudaFree(kv.second.w);
   for (int i = 0; i < 2; ++i) { cudaFree(e->cam[i].K); cudaFree(e->cam[i].rays); }
-  cudaFree(e->d_planes); cudaFree(e->stats); cudaFree(e->stats_b); cudaFree(e->bn_counter); cudaFree(e->scale); cudaFree(e->shift); cudaFree(e->ws_sweep);
+  cudaFree(e->d_planes); cudaFree(e->stats); cudaFree(e->stats_b); cudaFree(e->bn_counter); cudaFree(e->scale); cudaFree(e->shift); cudaFree(e->eval_coef); cudaFree(e->ws_sweep);
   cudaFree(e->bv_cur_hwd); cudaFree(e->dpv_hwd); cudaFree(e->prior_hwd); cudaFree(e->depth); cudaFree(e->conf);
   cudaFree(e->x0_buf); cudaFree(e->rt_buf); cudaFree(e->ref_cur_hwd); cudaFree(e->ref_kv_hwd);
   drop_graphs(e);
@@ -828,6 +933,7 @@ int nrgbd_kvnet_set_option(nrgbd_kvnet* e, const char* key, int value) {
   std::string k(key);
   if (k == "bn_update_running") { drop_graphs(e); e->bn_update_running = value; return NRGBD_OK; }
   if (k == "profile") { e->profile = value; return NRGBD_OK; }
+  if (k == "bn_eval") { drop_graphs(e); e->bn_eval = value ? 1 : 0; return NRGBD_OK; }
   if (k == "fuse_bn") { if (e->fuse_bn != value) drop_graphs(e); e->fuse_bn = value; return NRGBD_OK; }
   if (k == "use_graph") { drop_graphs(e); e->use_graph = value; return NRGBD_OK; }
   if (k == "conv_math") {            // 0: exact fp32 (CUDA cores); 1: wgmma 3xTF32; 2: wgmma split-fp16 pairs
@@ -1001,6 +1107,7 @@ int nrgbd_kvnet_forward(nrgbd_kvnet* e, const float* frames, const float* poses,
 static int forward_core(nrgbd_kvnet* e, bool steady, bool need_cur_refined, bool need_kv_refined, nrgbd_stream_t stream) {
   e->st = (cudaStream_t)stream; e->rc = 0;
   nrgbd_stream_t st = stream;
+  eval_coeffs(e);
   const int H = e->H, W = e->W, D = e->D, V = e->V, h = e->h, w = e->w, F = e->F, N = V + 1;
   const long long hw = (long long)h * w, HW = (long long)H * W;
 

@@ -126,7 +126,7 @@ class KVNET(nn.Module):
                                        ctypes.byref(hnd)))
             d32 = np.ascontiguousarray(np.asarray(self.d_candi).astype(np.float32))
             check(L.nrgbd_kvnet_set_planes(hnd, d32.ctypes.data_as(ctypes.c_void_p), len(d32)))
-            ent = {'h': hnd, 'params': {}, 'cams': [None, None], 'keep': {}, 'conv_math': None}
+            ent = {'h': hnd, 'params': {}, 'cams': [None, None], 'keep': {}, 'conv_math': None, 'bn_eval': False}
             self._engines[key] = ent
         return ent
 
@@ -222,9 +222,6 @@ class KVNET(nn.Module):
         '''
         if not ref_frame.is_cuda:
             raise _lib.NrgbdError('neuralrgbd_b200.KVNET has no CPU path: inputs must be CUDA tensors')
-        if not self.training:
-            raise NotImplementedError('eval-mode BatchNorm (running statistics) is not implemented: the reference '
-                                      'never calls .eval(), every BN layer normalises with batch statistics')
         if isinstance(BV_predict, torch.Tensor):
             if m_misc.valid_dpv(BV_predict):
                 assert BV_predict.shape[0] == 1
@@ -243,6 +240,12 @@ class KVNET(nn.Module):
                     raise ValueError("conv_math must be 'fp32', 'tf32x3' or 'f16x3'")
                 check(L.nrgbd_kvnet_set_option(ent['h'], b'conv_math', modes[self.conv_math]))
                 ent['conv_math'] = self.conv_math
+            # .eval(): the 13 BatchNorm layers with running statistics (K-Net's BatchNorm3d, the feature CNN's downsample
+            # BatchNorm2d) normalise with them and nothing is updated; the others keep batch statistics, as in PyTorch
+            bn_eval = not self.training
+            if ent['bn_eval'] != bn_eval:
+                check(L.nrgbd_kvnet_set_option(ent['h'], b'bn_eval', int(bn_eval)))
+                ent['bn_eval'] = bn_eval
             self._set_camera(ent, 0, cam=self.cam_intrinsics)
             prior = None
             if isinstance(BV_predict, torch.Tensor) and m_misc.valid_dpv(BV_predict):
@@ -267,10 +270,10 @@ class KVNET(nn.Module):
             st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
             check(L.nrgbd_kvnet_forward(ent['h'], ptr(frames), ptr(poses), ptr(prior), ptr(dmap_cur), ptr(dmap_kv),
                                         ptr(bv_cur), ptr(dpv), ptr(depth), ptr(conf), st))
-            # BatchNorm's num_batches_tracked side effect, applied lazily; a replica shares the counters' owner
+            # BatchNorm's num_batches_tracked side effect (train mode only), applied lazily; a replica shares the counters' owner
             owner = self.__dict__.get('_owner_ref', None)
             owner = owner() if owner is not None else self
-            if owner is not None:
+            if owner is not None and self.training:
                 owner.__dict__['_nb_pending'] = owner.__dict__.get('_nb_pending', 0) + 1
                 if prior is not None:
                     owner.__dict__['_nb_pending_kv'] = owner.__dict__.get('_nb_pending_kv', 0) + 1
