@@ -362,6 +362,17 @@ int nrgbd_upsample_bilinear_ac_nhwc(const float* x, int N, int Hi, int Wi, int C
 int nrgbd_copy_channels(const float* x, long long P, int Cs_in, int c_off_in, int C, int op, float* y,
                         int Cs_out, int c_off_out, nrgbd_stream_t stream);
 
+/* ---- guided-filter depth refinement: models/Refine.py:620-641 RefineNet_DGF.forward with
+ * models/GF/guided_filter.py GuidedFilter(r, eps) (KVNET(refineNet_name='DGF') uses r = 1, eps = 1e-8).
+ * dmap [h][w] low-resolution depth; img: channel c (0..2) of pixel p at img[c * img_sc + p * img_sp], [H][W];
+ * w0 [64][3], b0 [64], w1 [64], b1 [1] = r_net.feature_ext.{0,2}.{weight,bias}; out [H][W].
+ * H / h == W / w > 1. ws: nrgbd_guided_filter_workspace_floats(H, W) floats. Box sums use the reference's
+ * cumulative-sum form (double-accumulated prefixes rounded to fp32); no atomics, identical from run to run. */
+long long nrgbd_guided_filter_workspace_floats(int H, int W);
+int nrgbd_guided_filter_refine(const float* dmap, int h, int w, const float* img, long long img_sc, long long img_sp,
+                               int H, int W, const float* w0, const float* b0, const float* w1, const float* b1,
+                               int r, float eps, float* ws, float* out, nrgbd_stream_t stream);
+
 /* ---- a4, a6: whole-frame engine -------------------------------------------------------------
  * replaces models/KVNET.py:35-185 (KVNET.__init__/forward with if_refined=True, refineNet_name='DPV')
  * + models/basic.py:223-323 (D_NET_BASIC.forward) + the DPV propagation of
@@ -379,7 +390,7 @@ int nrgbd_kvnet_set_param(nrgbd_kvnet* e, const char* name, const float* data, l
 int nrgbd_kvnet_set_camera(nrgbd_kvnet* e, int slot, const float* K_host, const float* rays_host, float cx,
                            float cy, double hfov_deg, double vfov_deg);
 int nrgbd_kvnet_set_planes(nrgbd_kvnet* e, const float* d_host, int D);   /* float32(d_candi) */
-int nrgbd_kvnet_set_option(nrgbd_kvnet* e, const char* key, int value);   /* "bn_update_running", "profile", "conv_math" (0 fp32 FFMA, 1 wgmma 3xTF32, 2 wgmma split-fp16 pairs), "use_graph" (CUDA-graph replay, default 1), "bn_eval" (1: the module is in .eval(): BatchNorm layers with running statistics normalise with them and update nothing, the others keep batch statistics; default 0) */
+int nrgbd_kvnet_set_option(nrgbd_kvnet* e, const char* key, int value);   /* "bn_update_running", "profile", "conv_math" (0 fp32 FFMA, 1 wgmma 3xTF32, 2 wgmma split-fp16 pairs), "use_graph" (CUDA-graph replay, default 1), "bn_eval" (1: the module is in .eval(): BatchNorm layers with running statistics normalise with them and update nothing, the others keep batch statistics; default 0), "refine" (refined outputs: 0 the DPV R-Net, default; 1 the guided filter of refineNet_name='DGF', [H][W] depth maps; 2 none, if_refined=False), "refine_upsample_d" (1: the DPV R-Net of if_upsample_d=True, refined log-DPVs of 4D planes; default 0) */
 /* with option "profile"=1 the engine brackets its conv (category 0, work = flops) and plane-sweep
  * (category 1, work = algorithmic bytes) launches with CUDA events; this returns and clears the sums. */
 int nrgbd_kvnet_profile_read(nrgbd_kvnet* e, int category, double* ms, double* work, long long* launches);
@@ -389,7 +400,8 @@ int nrgbd_kvnet_profile_read(nrgbd_kvnet* e, int category, double* ms, double* w
 int nrgbd_kvnet_profile_table(nrgbd_kvnet* e, int category, char* buf, long long cap);
 long long nrgbd_kvnet_workspace_bytes(nrgbd_kvnet* e);
 /* frames [V+1][3][H][W] (sources then reference), poses [V][4][4], bv_predict [D][h][w] or NULL
- * (first window). Outputs (any may be NULL): dmap_cur_refined, dmap_refined [D][H][W] log-DPV;
+ * (first window). Outputs (any may be NULL): dmap_cur_refined, dmap_refined [D][H][W] log-DPV
+ * (option "refine" 1: [H][W] depth; 2: both must be NULL; "refine_upsample_d" 1: [4D][H][W]);
  * bv_cur, dpv [D][h][w] log-DPV; depth_lowres, conf_lowres [h][w]. All device pointers. */
 int nrgbd_kvnet_forward(nrgbd_kvnet* e, const float* frames, const float* poses, const float* bv_predict,
                         float* dmap_cur_refined, float* dmap_refined, float* bv_cur, float* dpv,

@@ -87,6 +87,9 @@ SIGNATURES = {
     'nrgbd_upsample_bilinear_ac_nhwc': (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int,
                                                 c_int, c_vp]),
     'nrgbd_copy_channels': (c_int, [c_vp, c_ll, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp]),
+    'nrgbd_guided_filter_workspace_floats': (c_ll, [c_int, c_int]),
+    'nrgbd_guided_filter_refine': (c_int, [c_vp, c_int, c_int, c_vp, c_ll, c_ll, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_int,
+                                           c_float, c_vp, c_vp, c_vp]),
     'nrgbd_plane_sweep_backward_packed': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp,
                                                   c_vp, c_vp, c_float, c_float, c_float, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     'nrgbd_unpack_features': (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp]),

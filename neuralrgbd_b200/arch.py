@@ -65,33 +65,52 @@ def kv_net_specs(pre, cin, f):
     return s
 
 
-def r_net_specs(pre, C0, C1, C2, D):
-    """Refine.RefineNet_DPV_upsample.__init__ :30-77 (upsample_D=False)."""
+def r_net_specs(pre, C0, C1, C2, D, upsample_D=False):
+    """Refine.RefineNet_DPV_upsample.__init__ :30-77. upsample_D widens the two transposed convolutions' outputs to
+    D0 = 2D and D1 = 4D planes (:44-48): the refined DPV then has 4D planes."""
     def c(p, a, b):
         return [(p + '.weight', (b, a, 3, 3), 'conv2d'), (p + '.bias', (b,), 'bias')]
 
     def t(p, a, b):
         return [(p + '.weight', (a, b, 4, 4), 'convT2d'), (p + '.bias', (b,), 'bias')]
     i0 = D + C0
-    return (c(pre + '.conv0.0', i0, i0) + c(pre + '.conv0_1.0', i0, i0) + t(pre + '.trans_conv0.0', i0, D)
-            + c(pre + '.conv1.0', D + C1, D + C1) + c(pre + '.conv1_1.0', D + C1, D + C1)
-            + t(pre + '.trans_conv1.0', D + C1, D)
-            + c(pre + '.conv2.0', D + C2, D + C2) + c(pre + '.conv2_1.0', D + C2, D)
-            + c(pre + '.conv2_2', D, D))
+    D0, D1 = (2 * D, 4 * D) if upsample_D else (D, D)
+    return (c(pre + '.conv0.0', i0, i0) + c(pre + '.conv0_1.0', i0, i0) + t(pre + '.trans_conv0.0', i0, D0)
+            + c(pre + '.conv1.0', D0 + C1, D0 + C1) + c(pre + '.conv1_1.0', D0 + C1, D0 + C1)
+            + t(pre + '.trans_conv1.0', D0 + C1, D1)
+            + c(pre + '.conv2.0', D1 + C2, D1 + C2) + c(pre + '.conv2_1.0', D1 + C2, D1)
+            + c(pre + '.conv2_2', D1, D1))
 
 
-def kvnet_param_specs(feature_dim=64, D=64, t_win_r=2, kv_feature_dim=64):
+def dgf_specs(pre):
+    """Refine.RefineNet_DGF.__init__ :587-598: feature_ext = Conv2d(3, 64, 1), ReLU, Conv2d(64, 1, 1). The guided filter
+    itself has no parameters, and refine_channel does not change these shapes."""
+    return [(pre + '.feature_ext.0.weight', (64, 3, 1, 1), 'conv2d'), (pre + '.feature_ext.0.bias', (64,), 'bias'),
+            (pre + '.feature_ext.2.weight', (1, 64, 1, 1), 'conv2d'), (pre + '.feature_ext.2.bias', (1,), 'bias')]
+
+
+def kvnet_param_specs(feature_dim=64, D=64, t_win_r=2, kv_feature_dim=64, refine='DPV', upsample_d=False):
     """Every entry of KVNET(...).state_dict() in registration order. The feature CNN
     appears twice (the extractor object is registered under both `feature_extractor`
-    and `d_net.feature_extraction`, KVNET.py:63-67) -- same tensors, two names."""
+    and `d_net.feature_extraction`, KVNET.py:63-67) -- same tensors, two names; its
+    parameters do not depend on multi_scale, so every refinement shares them.
+    refine: 'DPV' (default), 'DGF' or None (if_refined=False); upsample_d: the DPV R-Net's if_upsample_d (ignored
+    unless refine is 'DPV', as in the reference)."""
     fe = feature_cnn_specs('feature_extractor.feature_extraction', feature_dim)
     fe2 = [('d_net.feature_extraction.' + n[len('feature_extractor.'):], shp, kind) for n, shp, kind in fe]
     kv = kv_net_specs('kv_net', 3 * (2 * t_win_r + 1) + 1, kv_feature_dim)
-    rn = r_net_specs('r_net', feature_dim, feature_dim // 2, 3, D)
+    if refine == 'DPV':
+        rn = r_net_specs('r_net', feature_dim, feature_dim // 2, 3, D, upsample_d)
+    elif refine == 'DGF':
+        rn = dgf_specs('r_net')
+    elif refine is None:
+        rn = []
+    else:
+        raise ValueError(refine)
     return fe + fe2 + kv + rn
 
 
-def synth_state_dict(seed, feature_dim=64, D=64, t_win_r=2, kv_feature_dim=64):
+def synth_state_dict(seed, feature_dim=64, D=64, t_win_r=2, kv_feature_dim=64, refine='DPV', upsample_d=False):
     """Random-initialised weights in the reference's style (He-normal convs,
     basic.py:28-40) with non-trivial BN affine terms so those paths are exercised.
     Transposed convs get the reference's bilinear kernel (Refine.py:121-132) times a
@@ -99,7 +118,7 @@ def synth_state_dict(seed, feature_dim=64, D=64, t_win_r=2, kv_feature_dim=64):
     are wget-only and unavailable offline). Returns {name: float32 ndarray}."""
     rng = np.random.RandomState(seed)
     sd = {}
-    for name, shp, kind in kvnet_param_specs(feature_dim, D, t_win_r, kv_feature_dim):
+    for name, shp, kind in kvnet_param_specs(feature_dim, D, t_win_r, kv_feature_dim, refine, upsample_d):
         if name.startswith('d_net.feature_extraction.'):
             sd[name] = sd['feature_extractor.' + name[len('d_net.feature_extraction.'):]]
             continue

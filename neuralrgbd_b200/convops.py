@@ -421,3 +421,18 @@ def conv_transpose2d_h2(x, w, bias=None, leaky=False):
     check(L.nrgbd_conv_transpose2d_k4s2_nhwc_h2(ptr(xh), ptr(xl), N, Hin, Win, Cin_pad, Cin_pad, ptr(wp), ptr(bias), Cout,
                                                 Cout_pad, BN, ptr(y), Cs_out, 0, 1 if leaky else 0, _st()))
     return from_cl(y, Cout)
+
+
+def guided_filter_refine(dmap, img, w0, b0, w1, b1, r=1, eps=1e-8):
+    """RefineNet_DGF.forward (models/Refine.py:620-641) through nrgbd_guided_filter_refine: dmap [h,w], img [3,H,W]
+    (CUDA float32), feature_ext weights as in the state_dict -> [H,W]."""
+    L = _lib.lib()
+    h, w = dmap.shape
+    _, H, W = img.shape
+    dmap = dmap.float().contiguous(); img = img.float().contiguous()
+    ws = torch.empty(L.nrgbd_guided_filter_workspace_floats(H, W), device=img.device, dtype=torch.float32)
+    out = torch.empty((H, W), device=img.device, dtype=torch.float32)
+    check(L.nrgbd_guided_filter_refine(ptr(dmap), h, w, ptr(img), H * W, 1, H, W, ptr(w0.float().contiguous()),
+                                       ptr(b0.float().contiguous()), ptr(w1.float().contiguous()), ptr(b1.float().contiguous()), r,
+                                       _F(eps), ptr(ws), ptr(out), _st()))
+    return out

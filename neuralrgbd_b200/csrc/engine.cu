@@ -86,6 +86,8 @@ struct nrgbd_kvnet {
   std::unordered_map<std::string, PackedH2> packed_h2;
   std::unordered_map<const float*, PairBuf> pairs;   // activations that currently have a split-fp16 copy (conv_math 2)
   int conv_math = 0;                // 0: exact fp32 FFMA implicit GEMM; 1: wgmma 3xTF32; 2: wgmma split-fp16 pairs (conv_f16.cu)
+  int refine = 0;                   // refinement of KVNET(...): 0 the DPV R-Net, 1 the guided filter ('DGF'), 2 none (if_refined=False)
+  int refine_up = 0;                // DPV R-Net with if_upsample_d: widths D0 = 2D, D1 = 4D (Refine.py:44-48)
   bool packed_dirty = true;
   Camera cam[2];
   float* d_planes = nullptr;
@@ -117,8 +119,11 @@ struct nrgbd_kvnet {
   struct GraphEnt { int variant; cudaStream_t stream; cudaGraphExec_t exec; long long launches; };
   float* x0_buf = nullptr;          // [V+1][H][W][4] input frames, channels-last
   float* rt_buf = nullptr;          // [V][3][3] rotations then [V][3] translations
-  float* ref_cur_hwd = nullptr;     // [HW][D] refined log-DPV of the measurement
-  float* ref_kv_hwd = nullptr;      // [HW][D] refined log-DPV of the filtered DPV (steady state)
+  float* ref_cur_hwd = nullptr;     // [HW][refined_planes()] refined output of the measurement (log-DPV, or guided-filter depth)
+  float* ref_kv_hwd = nullptr;      // [HW][refined_planes()] refined output of the filtered DPV (steady state)
+  long long ref_floats = 0;         // floats allocated for each of the two
+  // planes of a refined output: the DPV R-Net's D (4D with if_upsample_d), 1 for the guided filter, 0 without refinement
+  int refined_planes() const { return refine == 0 ? (refine_up ? 4 * D : D) : (refine == 1 ? 1 : 0); }
   std::vector<GraphEnt> graphs;
   unsigned long long graph_clock = 0;
   int profile = 0;
@@ -719,9 +724,11 @@ void conv_transpose(Eng* e, const Act& x, const std::string& wname, const char* 
   ENG_CALL(e, nrgbd_conv_transpose2d_k4s2_nhwc(x.p, x.N, x.H, x.W, pk->Cin_pad, x.Cs, pk->w, tb, Cout, pk->Cout_pad, dst.p, dst.Cs, 0, 1, st));
 }
 
-// models/Refine.py:79-107. prob source: log-DPV pixel-major [hw][D]; returns log-DPV [H*W][D].
+// models/Refine.py:79-107. prob source: log-DPV pixel-major [hw][D]; returns log-DPV [H*W][D1]. The transposed convolutions
+// widen the DPV to D0 and D1 planes: D0 = D1 = D, or with if_upsample_d D0 = 2D, D1 = 4D (Refine.py:44-48).
 void r_net(Eng* e, const float* bv_hwd, const float* feat_ref, int feat_Cs, const float* l1_ref, int l1_Cs, const Act& frame_ref, Act& out) {
   const int D = e->D, h = e->h, w = e->w, H = e->H, W = e->W, F = e->F;
+  const int D0 = e->refine_up ? 2 * D : D, D1 = e->refine_up ? 4 * D : D;
   const long long hw = (long long)h * w;
   nrgbd_stream_t st = (nrgbd_stream_t)e->st;
   Act in0 = acquire(e, 1, 1, h, w, D + F);
@@ -731,22 +738,44 @@ void r_net(Eng* e, const float* bv_hwd, const float* feat_ref, int feat_Cs, cons
   }
   Act a = conv(e, in0, "r_net.conv0.0.weight", D + F, 1, 3, 1, 1, 1, "r_net.conv0.0.bias", true, false, nullptr, 0, -1, nullptr, nullptr, true); release(e, in0);
   Act b = conv(e, a, "r_net.conv0_1.0.weight", D + F, 1, 3, 1, 1, 1, "r_net.conv0_1.0.bias", true, false, nullptr, 0, -1, nullptr, nullptr, true); release(e, a);
-  Act t0 = acquire(e, 1, 1, 2 * h, 2 * w, D + F / 2);
-  conv_transpose(e, b, "r_net.trans_conv0.0.weight", "r_net.trans_conv0.0.bias", D, t0);
-  if (!e->rc) ENG_CALL(e, nrgbd_copy_channels(l1_ref, 4 * hw, l1_Cs, 0, F / 2, 0, t0.p, t0.Cs, D, st));
+  Act t0 = acquire(e, 1, 1, 2 * h, 2 * w, D0 + F / 2);
+  conv_transpose(e, b, "r_net.trans_conv0.0.weight", "r_net.trans_conv0.0.bias", D0, t0);
+  if (!e->rc) ENG_CALL(e, nrgbd_copy_channels(l1_ref, 4 * hw, l1_Cs, 0, F / 2, 0, t0.p, t0.Cs, D0, st));
   release(e, b);
-  Act c = conv(e, t0, "r_net.conv1.0.weight", D + F / 2, 1, 3, 1, 1, 1, "r_net.conv1.0.bias", true, false, nullptr, 0, -1, nullptr, nullptr, true); release(e, t0);
-  Act d = conv(e, c, "r_net.conv1_1.0.weight", D + F / 2, 1, 3, 1, 1, 1, "r_net.conv1_1.0.bias", true, false, nullptr, 0, -1, nullptr, nullptr, true); release(e, c);
-  Act t1 = acquire(e, 1, 1, H, W, D + 3);
-  conv_transpose(e, d, "r_net.trans_conv1.0.weight", "r_net.trans_conv1.0.bias", D, t1);
-  if (!e->rc) ENG_CALL(e, nrgbd_copy_channels(frame_ref.p, (long long)H * W, frame_ref.Cs, 0, 3, 0, t1.p, t1.Cs, D, st));
+  Act c = conv(e, t0, "r_net.conv1.0.weight", D0 + F / 2, 1, 3, 1, 1, 1, "r_net.conv1.0.bias", true, false, nullptr, 0, -1, nullptr, nullptr, true); release(e, t0);
+  Act d = conv(e, c, "r_net.conv1_1.0.weight", D0 + F / 2, 1, 3, 1, 1, 1, "r_net.conv1_1.0.bias", true, false, nullptr, 0, -1, nullptr, nullptr, true); release(e, c);
+  Act t1 = acquire(e, 1, 1, H, W, D1 + 3);
+  conv_transpose(e, d, "r_net.trans_conv1.0.weight", "r_net.trans_conv1.0.bias", D1, t1);
+  if (!e->rc) ENG_CALL(e, nrgbd_copy_channels(frame_ref.p, (long long)H * W, frame_ref.Cs, 0, 3, 0, t1.p, t1.Cs, D1, st));
   release(e, d);
-  Act f = conv(e, t1, "r_net.conv2.0.weight", D + 3, 1, 3, 1, 1, 1, "r_net.conv2.0.bias", true, false, nullptr, 0, -1, nullptr, nullptr, true); release(e, t1);
-  Act g = conv(e, f, "r_net.conv2_1.0.weight", D, 1, 3, 1, 1, 1, "r_net.conv2_1.0.bias", true, false, nullptr, 0, -1, nullptr, nullptr, true); release(e, f);
-  conv(e, g, "r_net.conv2_2.weight", D, 1, 3, 1, 1, 1, "r_net.conv2_2.bias", false, false, &out, 0, D); release(e, g);
-  // F.log_softmax(conv2_2_out, dim=1): channels are contiguous per pixel (Cs == D)
+  Act f = conv(e, t1, "r_net.conv2.0.weight", D1 + 3, 1, 3, 1, 1, 1, "r_net.conv2.0.bias", true, false, nullptr, 0, -1, nullptr, nullptr, true); release(e, t1);
+  Act g = conv(e, f, "r_net.conv2_1.0.weight", D1, 1, 3, 1, 1, 1, "r_net.conv2_1.0.bias", true, false, nullptr, 0, -1, nullptr, nullptr, true); release(e, f);
+  conv(e, g, "r_net.conv2_2.weight", D1, 1, 3, 1, 1, 1, "r_net.conv2_2.bias", false, false, &out, 0, D1); release(e, g);
+  // F.log_softmax(conv2_2_out, dim=1): channels are contiguous per pixel (Cs == D1); above 256 planes dpv_normalize takes
+  // its thread-per-pixel path
   if (!e->rc)
-    ENG_CALL(e, nrgbd_dpv_normalize(out.p, 1, D, nullptr, 0, 0, 1.f, H * W, D, out.p, 1, D, nullptr, nullptr, nullptr, st));
+    ENG_CALL(e, nrgbd_dpv_normalize(out.p, 1, D1, nullptr, 0, 0, 1.f, H * W, D1, out.p, 1, D1, nullptr, nullptr, nullptr, st));
+}
+
+// models/KVNET.py:129-132,176-178 with refineNet_name='DGF': expected depth of the low-resolution log-DPV in
+// depth_val_regression's sequential order (mutils/misc.py:541-546; dpv_normalize's warp-reduced depth is not that order),
+// then RefineNet_DGF (Refine.py:620-641) guided by the reference frame; out [H][W] depth.
+void dgf_refine(Eng* e, const float* bv_hwd, const Act& frame_ref, float* out) {
+  const int D = e->D, h = e->h, w = e->w, H = e->H, W = e->W;
+  const long long hw = (long long)h * w;
+  nrgbd_stream_t st = (nrgbd_stream_t)e->st;
+  const float* w0 = param(e, "r_net.feature_ext.0.weight");
+  const float* b0 = param(e, "r_net.feature_ext.0.bias");
+  const float* w1 = param(e, "r_net.feature_ext.2.weight");
+  const float* b1 = param(e, "r_net.feature_ext.2.bias");
+  if (e->rc) return;
+  float* dmap = e->pool.acquire((size_t)hw * sizeof(float));
+  float* ws = e->pool.acquire((size_t)nrgbd_guided_filter_workspace_floats(H, W) * sizeof(float));
+  if (!dmap || !ws) { nrgbd_set_error("engine: out of device memory (guided filter)"); e->rc = NRGBD_ERR_NOMEM; }
+  ENG_CALL(e, nrgbd_depth_regression(bv_hwd, (int)hw, D, 1, D, e->d_planes, 1, dmap, nullptr, st));
+  ENG_CALL(e, nrgbd_guided_filter_refine(dmap, h, w, frame_ref.p, 1, frame_ref.Cs, H, W, w0, b0, w1, b1, 1, 1e-8f, ws, out, st));
+  if (dmap) e->pool.release(dmap);
+  if (ws) e->pool.release(ws);
 }
 
 // models/basic.py:113-139 on a channels-last volume [D][h][w][CK] -> gain [D][hw] (DHW, Cs = 1)
@@ -936,6 +965,17 @@ int nrgbd_kvnet_set_option(nrgbd_kvnet* e, const char* key, int value) {
   if (k == "bn_eval") { drop_graphs(e); e->bn_eval = value ? 1 : 0; return NRGBD_OK; }
   if (k == "fuse_bn") { if (e->fuse_bn != value) drop_graphs(e); e->fuse_bn = value; return NRGBD_OK; }
   if (k == "use_graph") { drop_graphs(e); e->use_graph = value; return NRGBD_OK; }
+  if (k == "refine") {               // 0: DPV R-Net (default); 1: guided filter (DGF); 2: none
+    if (value < 0 || value > 2) { nrgbd_set_error("refine must be 0 (DPV), 1 (DGF) or 2 (none)"); return NRGBD_ERR_BAD_ARG; }
+    if (e->refine != value) drop_graphs(e);
+    e->refine = value;
+    return NRGBD_OK;
+  }
+  if (k == "refine_upsample_d") {    // DPV R-Net with if_upsample_d: refined outputs of 4D planes
+    if (e->refine_up != (value ? 1 : 0)) drop_graphs(e);
+    e->refine_up = value ? 1 : 0;
+    return NRGBD_OK;
+  }
   if (k == "conv_math") {            // 0: exact fp32 (CUDA cores); 1: wgmma 3xTF32; 2: wgmma split-fp16 pairs
     if (value < 0 || value > 2) { nrgbd_set_error("conv_math must be 0 (fp32), 1 (tf32x3) or 2 (f16x3)"); return NRGBD_ERR_BAD_ARG; }
     drop_graphs(e); e->conv_math = value;
@@ -997,21 +1037,33 @@ int nrgbd_kvnet_profile_table(nrgbd_kvnet* e, int category, char* buf, long long
 //  poses   [V][4][4]       relative poses E_src.E_ref^-1, device
 //  bv_predict [D][h][w] or NULL: NULL -> first-window branch (:138-140). (The NaN-sentinel test of
 //  :142 reads one element on the host and is done by the caller.)
-//  outputs (device, any may be NULL): dmap_cur_refined [D][H][W], dmap_refined [D][H][W],
+//  outputs (device, any may be NULL): dmap_cur_refined [D][H][W], dmap_refined [D][H][W] (option "refine" 1: [H][W] depth;
+//  2: both must be NULL),
 //  bv_cur [D][h][w], dpv [D][h][w]; depth_lowres/conf_lowres [h][w] = expected depth / max prob of dpv.
 // ---- one depth frame = eager head -> core (CUDA graph) -> eager tail --------------------------------
 // head: caller inputs -> engine-owned buffers (frames to channels-last, R|t gather, prior to pixel-major)
 // core: D-Net, R-Net, [K-Net, R-Net] entirely on engine-owned memory (graph-captured per branch/need-set)
 // tail: engine results -> caller tensors in the reference layouts ([D][H][W] / [D][h][w])
+// The refined-output buffers are sized by the refinement option; a change of option drops the graphs that captured them.
 static int ensure_io_buffers(nrgbd_kvnet* e) {
-  if (e->x0_buf) return NRGBD_OK;
   const size_t HW = (size_t)e->H * e->W;
-  bool ok = cudaMalloc((void**)&e->x0_buf, sizeof(float) * (e->V + 1) * HW * 4) == cudaSuccess &&
-            cudaMalloc((void**)&e->rt_buf, sizeof(float) * 12 * e->V) == cudaSuccess &&
-            cudaMalloc((void**)&e->ref_cur_hwd, sizeof(float) * HW * e->D) == cudaSuccess &&
-            cudaMalloc((void**)&e->ref_kv_hwd, sizeof(float) * HW * e->D) == cudaSuccess;
-  if (!ok) { nrgbd_set_error("engine: cudaMalloc failed for the I/O staging buffers"); return NRGBD_ERR_NOMEM; }
-  cudaMemset(e->x0_buf, 0, sizeof(float) * (e->V + 1) * HW * 4);      // pad channel stays 0
+  if (!e->x0_buf) {
+    bool ok = cudaMalloc((void**)&e->x0_buf, sizeof(float) * (e->V + 1) * HW * 4) == cudaSuccess &&
+              cudaMalloc((void**)&e->rt_buf, sizeof(float) * 12 * e->V) == cudaSuccess;
+    if (!ok) { nrgbd_set_error("engine: cudaMalloc failed for the I/O staging buffers"); return NRGBD_ERR_NOMEM; }
+    cudaMemset(e->x0_buf, 0, sizeof(float) * (e->V + 1) * HW * 4);      // pad channel stays 0
+  }
+  const long long need = (long long)HW * e->refined_planes();
+  if (need != e->ref_floats) {
+    cudaFree(e->ref_cur_hwd); cudaFree(e->ref_kv_hwd);
+    e->ref_cur_hwd = e->ref_kv_hwd = nullptr; e->ref_floats = 0;
+    if (need > 0) {
+      bool ok = cudaMalloc((void**)&e->ref_cur_hwd, sizeof(float) * need) == cudaSuccess &&
+                cudaMalloc((void**)&e->ref_kv_hwd, sizeof(float) * need) == cudaSuccess;
+      if (!ok) { nrgbd_set_error("engine: cudaMalloc failed for the refined outputs"); return NRGBD_ERR_NOMEM; }
+      e->ref_floats = need;
+    }
+  }
   return NRGBD_OK;
 }
 
@@ -1036,8 +1088,16 @@ static int forward_tail(nrgbd_kvnet* e, bool steady, float* dmap_cur_refined, fl
   int rc = NRGBD_OK;
   if (bv_cur && !rc) rc = nrgbd_transpose2d(e->bv_cur_hwd, (int)hw, D, bv_cur, st);
   if (dpv && !rc) rc = nrgbd_transpose2d(e->dpv_hwd, (int)hw, D, dpv, st);
-  if (dmap_cur_refined && !rc) rc = nrgbd_transpose2d(e->ref_cur_hwd, (int)HW, D, dmap_cur_refined, st);
-  if (dmap_refined && !rc) rc = nrgbd_transpose2d(steady ? e->ref_kv_hwd : e->ref_cur_hwd, (int)HW, D, dmap_refined, st);
+  if (e->refine == 1) {              // guided filter: [H][W] depth maps, already in the caller's layout
+    if (dmap_cur_refined) NRGBD_CUDA_CHECK(cudaMemcpyAsync(dmap_cur_refined, e->ref_cur_hwd, sizeof(float) * HW, cudaMemcpyDeviceToDevice, (cudaStream_t)st));
+    if (dmap_refined)
+      NRGBD_CUDA_CHECK(cudaMemcpyAsync(dmap_refined, steady ? e->ref_kv_hwd : e->ref_cur_hwd, sizeof(float) * HW, cudaMemcpyDeviceToDevice,
+                                       (cudaStream_t)st));
+  } else {
+    const int Dr = e->refined_planes();
+    if (dmap_cur_refined && !rc) rc = nrgbd_transpose2d(e->ref_cur_hwd, (int)HW, Dr, dmap_cur_refined, st);
+    if (dmap_refined && !rc) rc = nrgbd_transpose2d(steady ? e->ref_kv_hwd : e->ref_cur_hwd, (int)HW, Dr, dmap_refined, st);
+  }
   if (rc) return rc;
   if (depth_lowres) NRGBD_CUDA_CHECK(cudaMemcpyAsync(depth_lowres, e->depth, sizeof(float) * hw, cudaMemcpyDeviceToDevice, (cudaStream_t)st));
   if (conf_lowres) NRGBD_CUDA_CHECK(cudaMemcpyAsync(conf_lowres, e->conf, sizeof(float) * hw, cudaMemcpyDeviceToDevice, (cudaStream_t)st));
@@ -1050,6 +1110,7 @@ int nrgbd_kvnet_forward(nrgbd_kvnet* e, const float* frames, const float* poses,
   NRGBD_REQUIRE(e && frames && poses, "null input");
   NRGBD_REQUIRE(e->cam[0].set && e->d_planes, "camera / depth planes not set");
   NRGBD_REQUIRE(!bv_predict || e->cam[1].set, "per-call camera (slot 1) not set");
+  NRGBD_REQUIRE(e->refine != 2 || (!dmap_cur_refined && !dmap_refined), "refine option 2 (none) has no refined outputs: pass NULL");
   cudaStream_t st = (cudaStream_t)stream;
   int rc = ensure_io_buffers(e);
   if (rc) return rc;
@@ -1136,9 +1197,13 @@ static int forward_core(nrgbd_kvnet* e, bool steady, bool need_cur_refined, bool
   const float* feat_ref = feat.p ? feat.p + (size_t)V * featS : nullptr;
   const float* l1_ref = l1.p ? l1.p + (size_t)V * 4 * hw * l1.Cs : nullptr;
   Act frame_ref = x0; frame_ref.N = 1; frame_ref.p = x0.p + (size_t)V * HW * x0.Cs;
-  Act out_cur; out_cur.p = e->ref_cur_hwd; out_cur.N = 1; out_cur.D = 1; out_cur.H = H; out_cur.W = W; out_cur.C = D; out_cur.Cs = D;
+  Act out_cur; out_cur.p = e->ref_cur_hwd; out_cur.N = 1; out_cur.D = 1; out_cur.H = H; out_cur.W = W;
+  out_cur.C = out_cur.Cs = e->refined_planes();
   Act out_kv = out_cur; out_kv.p = e->ref_kv_hwd;
-  if (need_cur_refined) r_net(e, e->bv_cur_hwd, feat_ref, feat.Cs, l1_ref, l1.Cs, frame_ref, out_cur);
+  if (need_cur_refined) {
+    if (e->refine == 1) dgf_refine(e, e->bv_cur_hwd, frame_ref, out_cur.p);
+    else r_net(e, e->bv_cur_hwd, feat_ref, feat.Cs, l1_ref, l1.Cs, frame_ref, out_cur);
+  }
   if (!steady) {
     // first window: DPV = BV_cur (KVNET.py:138-140)
     if (!e->rc) cudaMemcpyAsync(e->dpv_hwd, e->bv_cur_hwd, sizeof(float) * hw * D, cudaMemcpyDeviceToDevice, e->st);
@@ -1172,7 +1237,10 @@ static int forward_core(nrgbd_kvnet* e, bool steady, bool need_cur_refined, bool
     ENG_CALL(e, nrgbd_dpv_normalize(gain.p, hw, 1, e->prior_hwd, 1, D, 1.f, (int)hw, D, e->dpv_hwd, 1, D, e->d_planes, e->depth,
                                     e->conf, st));
     release(e, gain);
-    if (need_kv_refined) r_net(e, e->dpv_hwd, feat_ref, feat.Cs, l1_ref, l1.Cs, frame_ref, out_kv);
+    if (need_kv_refined) {
+      if (e->refine == 1) dgf_refine(e, e->dpv_hwd, frame_ref, out_kv.p);
+      else r_net(e, e->dpv_hwd, feat_ref, feat.Cs, l1_ref, l1.Cs, frame_ref, out_kv);
+    }
   }
   release(e, l1); release(e, feat); release(e, rgbq);
   if (e->rc == 0) { cudaError_t ce = cudaGetLastError(); if (ce != cudaSuccess) { nrgbd_set_error("nrgbd_kvnet_forward: %s", cudaGetErrorString(ce)); e->rc = NRGBD_ERR_CUDA; } }

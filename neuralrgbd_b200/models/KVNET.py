@@ -5,6 +5,11 @@ kvnet_scannet.tar / kvnet_kitti.tar load, with or without the DataParallel 'modu
 prefix), same return tuple. forward() does no math in Python: it hands the frame to the
 native engine (include/nrgbd.h nrgbd_kvnet_*), which runs D-Net -> R-Net -> (K-Net -> R-Net)
 as hand-written sm_90a kernels on the current CUDA stream. No CPU path.
+
+Refinement (KVNET.py:80-85, 126-136, 175-180): refineNet_name='DPV' (default) refines the DPV to image size, with
+4D planes when if_upsample_d=True (Refine.py:44-48; regress it with 4D candidates, e.g. the loaders' dup4_candi);
+'DGF' refines the expected depth with the guided filter of Refine.py:583-641 ([1,1,H,W] depth maps); if_refined=False
+runs no R-Net at all and returns -1 for both refined outputs.
 """
 import ctypes
 import math
@@ -73,13 +78,12 @@ class KVNET(nn.Module):
                  if_refined=True, refineNet_name='DPV',
                  t_win_r=2, refine_channel=3, if_upsample_d=False):
         super(KVNET, self).__init__()
-        if not (if_refined and refineNet_name == 'DPV'):
-            raise NotImplementedError("neuralrgbd_b200.KVNET implements the configuration every reference driver "
-                                      "uses (if_refined=True, refineNet_name='DPV'); got if_refined=%r, "
-                                      "refineNet_name=%r" % (if_refined, refineNet_name))
-        if d_upsample_ratio_KV_net is not None or if_upsample_d:
-            raise NotImplementedError('depth-dimension up-sampling (d_upsample_ratio_KV_net / if_upsample_d) is unused '
-                                      'by the reference drivers and not implemented')
+        if if_refined and refineNet_name not in ('DPV', 'DGF'):
+            raise NotImplementedError("refineNet_name must be 'DPV' or 'DGF' (models/KVNET.py:81-85); got %r" % (refineNet_name,))
+        if d_upsample_ratio_KV_net is not None:
+            raise NotImplementedError('d_upsample_ratio_KV_net is not implemented: for a ratio other than 1 the reference '
+                                      'itself fails with a shape error where K-Net\'s gain is added to BV_predict '
+                                      '(models/KVNET.py:172)')
         self.t_win_r = t_win_r
         self.feature_dim = feature_dim
         self.KVNet_feature_dim = KVNet_feature_dim
@@ -89,6 +93,9 @@ class KVNET(nn.Module):
         self.if_refined = if_refined
         self.refineNet_name = refineNet_name
         self.if_upsample_d = if_upsample_d
+        self.refine_channel = refine_channel
+        self._refine = refineNet_name if if_refined else None     # 'DPV', 'DGF' or None
+        self._upsample_d = bool(if_refined and refineNet_name == 'DPV' and if_upsample_d)   # refined DPVs of 4D planes
         self.cam_intrinsics = cam_intrinsics          # captured at construction: used by D-Net (KVNET.py:64-67)
         self.feat_dist = 'L2'                         # basic.py:146 default, never overridden by KVNET
         # convolution arithmetic: 'f16x3' (default; wgmma on split-fp16 operand pairs, 22-bit products, fp32 accumulate -
@@ -97,7 +104,7 @@ class KVNET(nn.Module):
 
         D = len(d_candi)
         gen = torch.Generator().manual_seed(0)
-        specs = arch.kvnet_param_specs(feature_dim, D, t_win_r, KVNet_feature_dim)
+        specs = arch.kvnet_param_specs(feature_dim, D, t_win_r, KVNet_feature_dim, self._refine, self._upsample_d)
         self._specs = [(n, s, k) for n, s, k in specs if not n.startswith('d_net.feature_extraction.')]
         for name, shape, kind in self._specs:
             _register(self, name, _init_tensor(name, tuple(shape), kind, gen), kind in ('bn_rm', 'bn_rv', 'bn_nb'))
@@ -106,13 +113,14 @@ class KVNET(nn.Module):
         self.d_net.add_module('feature_extraction', self.feature_extractor)
         # reference order of state_dict(): feature_extractor, d_net, kv_net, r_net
         for k in ('kv_net', 'r_net'):
-            m = self._modules.pop(k)
-            self._modules[k] = m
+            if k in self._modules:
+                self._modules[k] = self._modules.pop(k)
         self._engines = {}
         self.register_state_dict_pre_hook(KVNET._flush_batches_tracked)
         print('KV-Net initialization:')
         print('with R-net: %r' % (self.if_refined))
-        print('\trefinement name: %s' % (self.refineNet_name))
+        if self.if_refined:
+            print('\trefinement name: %s' % (self.refineNet_name))
 
     # ------------------------------------------------------------------ engine plumbing
     def _engine(self, H, W, V, device):
@@ -126,7 +134,8 @@ class KVNET(nn.Module):
                                        ctypes.byref(hnd)))
             d32 = np.ascontiguousarray(np.asarray(self.d_candi).astype(np.float32))
             check(L.nrgbd_kvnet_set_planes(hnd, d32.ctypes.data_as(ctypes.c_void_p), len(d32)))
-            ent = {'h': hnd, 'params': {}, 'cams': [None, None], 'keep': {}, 'conv_math': None, 'bn_eval': False}
+            ent = {'h': hnd, 'params': {}, 'cams': [None, None], 'keep': {}, 'conv_math': None, 'bn_eval': False, 'refine': 0,
+                   'upsample_d': False}
             self._engines[key] = ent
         return ent
 
@@ -218,8 +227,13 @@ class KVNET(nn.Module):
         cam_intrinsics - list of cam_intrinsics dict.
         BV_predict - NDHW tensor, the predicted BV, from the last reference frame, N=1
 
-        Outputs: dmap_cur_refined, dmap_kv_refined, BV_cur, BV_KV (refined entries are log-DPVs at image size)
+        Outputs: dmap_cur_refined, dmap_kv_refined, BV_cur, BV_KV. The refined entries are log-DPVs at image size
+        ('DPV'; 4D planes with if_upsample_d), depth maps 1 x 1 x H x W ('DGF'), or -1 (if_refined=False).
         '''
+        if self._refine == 'DGF':
+            # RefineNet_DGF.forward's input checks (Refine.py:627-628), as the reference meets them in its first R-Net call
+            assert ref_frame.dim() == 4, 'input format is wrong'
+            assert self.refine_channel == ref_frame.shape[1]
         if not ref_frame.is_cuda:
             raise _lib.NrgbdError('neuralrgbd_b200.KVNET has no CPU path: inputs must be CUDA tensors')
         if isinstance(BV_predict, torch.Tensor):
@@ -242,6 +256,13 @@ class KVNET(nn.Module):
                 ent['conv_math'] = self.conv_math
             # .eval(): the 13 BatchNorm layers with running statistics (K-Net's BatchNorm3d, the feature CNN's downsample
             # BatchNorm2d) normalise with them and nothing is updated; the others keep batch statistics, as in PyTorch
+            refine = {'DPV': 0, 'DGF': 1, None: 2}[self._refine]
+            if ent['refine'] != refine:
+                check(L.nrgbd_kvnet_set_option(ent['h'], b'refine', refine))
+                ent['refine'] = refine
+            if ent['upsample_d'] != self._upsample_d:
+                check(L.nrgbd_kvnet_set_option(ent['h'], b'refine_upsample_d', int(self._upsample_d)))
+                ent['upsample_d'] = self._upsample_d
             bn_eval = not self.training
             if ent['bn_eval'] != bn_eval:
                 check(L.nrgbd_kvnet_set_option(ent['h'], b'bn_eval', int(bn_eval)))
@@ -257,11 +278,12 @@ class KVNET(nn.Module):
             frames = torch.cat((src_frames[0], ref_frame), dim=0).float().contiguous()
             poses = src_cam_poses[0].to(device=dev, dtype=torch.float32).contiguous()
             h, w = H // 4, W // 4
-            dmap_cur = torch.empty((1, D, H, W), device=dev, dtype=torch.float32)
+            Dr = {'DPV': 4 * D if self._upsample_d else D, 'DGF': 1, None: 0}[self._refine]     # planes of a refined output
+            dmap_cur = torch.empty((1, Dr, H, W), device=dev, dtype=torch.float32) if Dr else None
             bv_cur = torch.empty((1, D, h, w), device=dev, dtype=torch.float32)
             dmap_kv = dpv = None
             if prior is not None:
-                dmap_kv = torch.empty((1, D, H, W), device=dev, dtype=torch.float32)
+                dmap_kv = torch.empty((1, Dr, H, W), device=dev, dtype=torch.float32) if Dr else None
                 dpv = torch.empty((1, D, h, w), device=dev, dtype=torch.float32)
             depth = conf = None
             if return_depth:
@@ -277,6 +299,8 @@ class KVNET(nn.Module):
                 owner.__dict__['_nb_pending'] = owner.__dict__.get('_nb_pending', 0) + 1
                 if prior is not None:
                     owner.__dict__['_nb_pending_kv'] = owner.__dict__.get('_nb_pending_kv', 0) + 1
+        if self._refine is None:
+            dmap_cur = dmap_kv = -1                         # KVNET.py:136, 182
         if prior is None:
             out = (dmap_cur, dmap_cur, bv_cur, bv_cur)     # KVNET.py:138-143
         else:
