@@ -291,9 +291,12 @@ const PackedH2* packw_h2_taps(Eng* e, const std::string& name, int Cin, int taps
   return &e->packed_h2[key];
 }
 
-// f16-pair tensor path: any conv with >= 16 input channels whose activation carries the 32-channel padding
+// f16-pair tensor path: any conv whose activation carries its channels padded to the packed weight's Cin_pad = pad32(C).
+// Channels [C, Cs) are zero in every activation (acquire() clears them, pair outputs and the K-Net volume rows store
+// zeros there) and the packed weight's rows [C, Cin_pad) are zero, so the padding adds exact zeros to every sum. This
+// is also the one condition under which an activation may exist only as its operand pair (the K-Net input volume).
 bool use_h2(Eng* e, const Act& x) {
-  return e->conv_math == 2 && x.C >= 16 && pad32(x.C) <= x.Cs && x.Cs % 8 == 0;
+  return e->conv_math == 2 && pad32(x.C) <= x.Cs && x.Cs % 8 == 0;
 }
 
 bool use_tc(Eng* e, const Act& x, int Cout) {
@@ -317,6 +320,10 @@ Act conv(Eng* e, const Act& x, const std::string& wname, int Cout, int kd, int k
          const char* bias_name, bool leaky, bool want_stats, Act* dst = nullptr, int c_off = 0, int out_Cs = -1,
          double* stats_buf = nullptr, const nrgbd_bn_input* in_bn = nullptr, bool pair_out = false) {
   if (!stats_buf) stats_buf = e->stats;
+  if (x.pair_only && !use_h2(e, x)) {          // x.p is no fp32 tensor: only the f16-pair path can read x
+    if (!e->rc) { nrgbd_set_error("engine: '%s' reads an activation that exists only as an operand pair", wname.c_str()); e->rc = NRGBD_ERR_BAD_ARG; }
+    return Act();
+  }
   int Ho = (x.H + 2 * pad - dil * (k - 1) - 1) / stride + 1;
   int Wo = (x.W + 2 * pad - dil * (k - 1) - 1) / stride + 1;
   Act y;
@@ -1212,10 +1219,13 @@ static int forward_core(nrgbd_kvnet* e, bool steady, bool need_cur_refined, bool
     const Camera& c1 = e->cam[1];
     const int CK = 3 * V + 4;
     Act vol;
-    if (e->conv_math == 2 && pad32(CK) == 32) {
+    vol.N = 1; vol.D = D; vol.H = h; vol.W = w; vol.C = CK; vol.Cs = pad32(CK);
+    if (vol.Cs == 32 && use_h2(e, vol)) {
       // f16-pair mode: the volume is written directly as the operand pair of dres0.0 (no fp32 volume, no split pass);
-      // vol.p is only the key of the pair buffers (a 16-byte block)
-      vol.N = 1; vol.D = D; vol.H = h; vol.W = w; vol.C = CK; vol.Cs = 32;
+      // vol.p is only the key of the pair buffers (a 16-byte block). dres0.0 decides its path by the same use_h2(vol),
+      // so it reads the pair: CK = 10 (t_win_r = 1) runs at Cin_pad = 32 like CK = 16 and 28. The row kernel stores
+      // 32 channels, the zeros [CK, 32) included.
+      vol.pair_only = true;
       vol.p = e->pool.acquire(16);
       PairBuf pb;
       pb.hi = e->pool.acquire((size_t)vol.floats() * 2);
