@@ -84,6 +84,14 @@ int nrgbd_warp_to_volume(const float* imgs_packed, int c_cnt, int c_off, int C_t
                          int w, const float* K, const float* R, const float* t, const float* rays,
                          const float* d_planes, float cx, float cy, float* ws, float* out,
                          nrgbd_stream_t stream);
+/* f-5: gradient of nrgbd_warp_to_volume with respect to the source images (autograd of warp_img_feats_v3 / _mgpu:
+ * F.grid_sample bilinear / zeros / align_corners=False input gradient; R, t, K, d are constants: no gradient).
+ * grad_out [V][C][D][hw] (all C channels, no chunking); g_imgs [V][C][hw] is zeroed by the call, then scatter-added
+ * with fp32 atomics at the forward's corners and weights (order not deterministic, like ATen's grid_sampler backward).
+ * Same camera arguments and workspace (V*12 floats) as the forward. */
+int nrgbd_warp_to_volume_backward(const float* grad_out, int C, int V, int D, int h, int w, const float* K,
+                                  const float* R, const float* t, const float* rays, const float* d_planes, float cx,
+                                  float cy, float* ws, float* g_imgs, nrgbd_stream_t stream);
 /* K-Net input volume, channels-last [D][hw][CK]: [v*3+c warped src RGB | ref RGB | BV_cur - BV_predict]
  * replaces models/KVNET.py:147-166 (avg-pooled RGB is passed in packed [.][hw][4]). */
 int nrgbd_knet_input_volume(const float* src_rgb_packed, const float* ref_rgb_packed,
@@ -111,6 +119,17 @@ int nrgbd_resample_dpv(const float* vol, long long in_stride_d, long long in_str
                        float tan_hv, float z_half, float z_radius, float pad_value, int do_clamp,
                        float clamp_lo, float clamp_hi, float* out, long long out_stride_d,
                        long long out_stride_pix, nrgbd_stream_t stream);
+/* f-5: gradient of nrgbd_resample_dpv with respect to vol (autograd of _set_vol_border + grid_sample(bilinear,
+ * border) 3-D, + torch.clamp when do_clamp != 0; E, d_pts and the camera are constants). Same arguments and strides
+ * as the forward; grad_out is read at the out strides, g_vol is written at the in strides, which must be dense
+ * ((hw, 1) or (1, D)). The six faces get zero gradient; with do_clamp the gradient passes where lo <= x <= hi (vol
+ * is re-read for that, and may be NULL when do_clamp == 0). g_vol is zeroed by the call, then scatter-added with
+ * fp32 atomics (order not deterministic). */
+int nrgbd_resample_dpv_backward(const float* vol, long long in_stride_d, long long in_stride_pix, const float* E,
+                                const float* rays, const float* d_pts, int D, int H, int W, float tan_hh,
+                                float tan_hv, float z_half, float z_radius, float pad_value, int do_clamp,
+                                float clamp_lo, float clamp_hi, const float* grad_out, long long out_stride_d,
+                                long long out_stride_pix, float* g_vol, nrgbd_stream_t stream);
 
 /* ---- a4 tail, a9, a11: reductions over the D planes -------------------------------------------
  * out = log_softmax_d(sign * (a + b)) (b may be NULL):
@@ -128,6 +147,13 @@ int nrgbd_dpv_normalize(const float* a, long long in_sd, long long in_sp, const 
 int nrgbd_depth_regression(const float* bv, int n_pix, int D, long long in_sd, long long in_sp,
                            const float* d_planes, int bv_log, float* depth, float* conf,
                            nrgbd_stream_t stream);
+/* f-5: gradient of the depth of nrgbd_depth_regression with respect to bv, same layout and arguments:
+ * g_bv(d,pix) = (grad_depth[pix] * d_planes[d]) * exp(bv(d,pix))  (bv_log != 0; the rounding order of autograd
+ * through misc.py:541-546), or grad_depth[pix] * d_planes[d] (bv_log == 0; bv may then be NULL). Every element of
+ * g_bv is written; no atomics. conf has no gradient. */
+int nrgbd_depth_regression_backward(const float* grad_depth, const float* bv, int n_pix, int D, long long in_sd,
+                                    long long in_sp, const float* d_planes, int bv_log, float* g_bv,
+                                    nrgbd_stream_t stream);
 int nrgbd_exp(const float* x, long long n, float* y, nrgbd_stream_t stream);
 
 /* ---- f-1: backward of the plane sweep (autograd of warping/homography.py:293-331 as used by

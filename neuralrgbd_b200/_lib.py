@@ -26,15 +26,21 @@ SIGNATURES = {
                                              c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     'nrgbd_warp_to_volume': (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp,
                                      c_vp, c_vp, c_float, c_float, c_vp, c_vp, c_vp]),
+    'nrgbd_warp_to_volume_backward': (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                              c_float, c_float, c_vp, c_vp, c_vp]),
     'nrgbd_knet_input_volume': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp,
                                         c_vp, c_vp, c_vp, c_float, c_float, c_vp, c_vp, c_vp]),
     'nrgbd_knet_input_volume_pair': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp,
                                              c_vp, c_vp, c_vp, c_float, c_float, c_vp, c_vp, c_vp, c_vp, c_vp]),
     'nrgbd_resample_dpv': (c_int, [c_vp, c_ll, c_ll, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_float, c_float,
                                    c_float, c_float, c_float, c_int, c_float, c_float, c_vp, c_ll, c_ll, c_vp]),
+    'nrgbd_resample_dpv_backward': (c_int, [c_vp, c_ll, c_ll, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_float, c_float,
+                                            c_float, c_float, c_float, c_int, c_float, c_float, c_vp, c_ll, c_ll, c_vp,
+                                            c_vp]),
     'nrgbd_dpv_normalize': (c_int, [c_vp, c_ll, c_ll, c_vp, c_ll, c_ll, c_float, c_int, c_int, c_vp, c_ll, c_ll,
                                     c_vp, c_vp, c_vp, c_vp]),
     'nrgbd_depth_regression': (c_int, [c_vp, c_int, c_int, c_ll, c_ll, c_vp, c_int, c_vp, c_vp, c_vp]),
+    'nrgbd_depth_regression_backward': (c_int, [c_vp, c_vp, c_int, c_int, c_ll, c_ll, c_vp, c_int, c_vp, c_vp]),
     'nrgbd_exp': (c_int, [c_vp, c_ll, c_vp, c_vp]),
     'nrgbd_pack_conv_weight': (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     'nrgbd_conv_nhwc': (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_int, c_int, c_int,

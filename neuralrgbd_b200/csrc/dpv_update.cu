@@ -116,6 +116,23 @@ depth_regression_kernel(const float* __restrict__ bv, int n_pix, int D, long lon
   if (conf) conf[pix] = cf;
 }
 
+// Backward of depth_regression_kernel's depth for one slice: autograd through the reference's
+// depth + exp(BV[0, d]) * d (mutils/misc.py:541-546) gives g_bv(d, pix) = (g[pix] * d) * exp(bv), or g[pix] * d without
+// the exp. Thread per (plane, pixel) with pixels fastest for the [D][hw] layout, planes fastest for the pixel-major one.
+__global__ void __launch_bounds__(256)
+depth_regression_backward_kernel(const float* __restrict__ g, const float* __restrict__ bv, int n_pix, int D, long long sd,
+                                 long long sp, const float* __restrict__ dpl, int bv_log, int pixel_major,
+                                 float* __restrict__ g_bv) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)n_pix * D) return;
+  int pix, d;
+  if (pixel_major) { d = (int)(idx % D); pix = (int)(idx / D); }
+  else { pix = (int)(idx % n_pix); d = (int)(idx / n_pix); }
+  const long long o = (long long)d * sd + (long long)pix * sp;
+  const float gd = __fmul_rn(__ldg(g + pix), __ldg(dpl + d));
+  g_bv[o] = bv_log ? __fmul_rn(gd, expf(__ldg(bv + o))) : gd;
+}
+
 __global__ void exp_kernel(const float* __restrict__ x, long long n, float* __restrict__ y) {
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) y[i] = expf(x[i]);
@@ -153,6 +170,17 @@ int nrgbd_depth_regression(const float* bv, int n_pix, int D, long long in_sd, l
   NRGBD_REQUIRE(bv && d_planes && (depth || conf) && n_pix > 0 && D > 0, "bad arguments");
   depth_regression_kernel<<<ceil_div(n_pix, 256), 256, 0, st>>>(bv, n_pix, D, in_sd, in_sp, d_planes, bv_log, depth,
                                                                 conf);
+  NRGBD_COUNT(1);
+  NRGBD_LAUNCH_CHECK();
+  return NRGBD_OK;
+}
+
+int nrgbd_depth_regression_backward(const float* grad_depth, const float* bv, int n_pix, int D, long long in_sd,
+                                    long long in_sp, const float* d_planes, int bv_log, float* g_bv, cudaStream_t st) {
+  NRGBD_REQUIRE(grad_depth && d_planes && g_bv && (bv || !bv_log) && n_pix > 0 && D > 0, "bad arguments");
+  const long long n = (long long)n_pix * D;
+  depth_regression_backward_kernel<<<ceil_div(n, 256), 256, 0, st>>>(grad_depth, bv, n_pix, D, in_sd, in_sp, d_planes,
+                                                                     bv_log, in_sd == 1 ? 1 : 0, g_bv);
   NRGBD_COUNT(1);
   NRGBD_LAUNCH_CHECK();
   return NRGBD_OK;

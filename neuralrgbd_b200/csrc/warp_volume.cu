@@ -19,6 +19,20 @@ __device__ __forceinline__ float4 sample4(const float4* __restrict__ img, const 
   return r;
 }
 
+// Bilinear taps of source view v for the reference pixel with ray (r0, r1, r2) on the plane at depth dval: the
+// homography of warping/homography.py:434-446 in the pinned rounding order. Shared by the forward warp and its
+// backward, so the backward scatters to the forward's corners with the forward's weights, bit for bit.
+__device__ __forceinline__ Tap2D warp_tap(const float* __restrict__ t1, const float* __restrict__ KR, int v, float r0,
+                                          float r1, float r2, float dval, float cx, float cy, int w, int h) {
+  const float* kr = KR + v * 9;
+  const float t2x = dot3_chain(kr[0], kr[1], kr[2], r0, r1, r2);
+  const float t2y = dot3_chain(kr[3], kr[4], kr[5], r0, r1, r2);
+  const float t2z = dot3_chain(kr[6], kr[7], kr[8], r0, r1, r2);
+  float ix, iy;
+  plane_project(t1[v * 3], t1[v * 3 + 1], t1[v * 3 + 2], t2x, t2y, t2z, dval, cx, cy, (float)w, (float)h, ix, iy);
+  return make_tap2d(ix, iy, w, h);
+}
+
 // MODE 0: out[v][c_off + c][d][pix]  (reference layout: list of V tensors C x D x h x w)
 // MODE 1: out[d][pix][CK] with channels [v*3+c | ref rgb | bv_cur - bv_pred]  (K-Net input, NDHWC)
 template <int MODE>
@@ -33,19 +47,12 @@ warp_volume_kernel(const float4* __restrict__ imgs, int c_cnt, int c_off, int C_
   if (idx >= (long long)hw * D) return;
   const int pix = (int)(idx % hw);
   const int d = (int)(idx / hw);
-  const float Wf = (float)w, Hf = (float)h;
   const float r0 = rays[pix], r1 = rays[hw + pix], r2 = rays[2 * hw + pix];
   const float dval = __ldg(dpl + d);
   float* o1 = nullptr;
   if (MODE == 1) o1 = out + ((size_t)d * hw + pix) * CK;
   for (int v = 0; v < V; ++v) {
-    const float* kr = KR + v * 9;
-    const float t2x = dot3_chain(kr[0], kr[1], kr[2], r0, r1, r2);
-    const float t2y = dot3_chain(kr[3], kr[4], kr[5], r0, r1, r2);
-    const float t2z = dot3_chain(kr[6], kr[7], kr[8], r0, r1, r2);
-    float ix, iy;
-    plane_project(t1[v * 3], t1[v * 3 + 1], t1[v * 3 + 2], t2x, t2y, t2z, dval, cx, cy, Wf, Hf, ix, iy);
-    Tap2D tp = make_tap2d(ix, iy, w, h);
+    const Tap2D tp = warp_tap(t1, KR, v, r0, r1, r2, dval, cx, cy, w, h);
     float4 s = sample4(imgs + (size_t)v * hw, tp);
     const float sv[4] = {s.x, s.y, s.z, s.w};
     if (MODE == 0) {
@@ -127,6 +134,37 @@ knet_volume_rows_kernel(const float4* __restrict__ imgs, const float* __restrict
   }
 }
 
+// Backward of MODE 0 (F.grid_sample's bilinear / zeros / align_corners=False input gradient, summed over the D
+// planes): g_imgs[v][c][q] += grad_out[v][c][d][pix] * w_q for the in-range corners q of (d, pix). One thread per
+// (plane, pixel) as in the forward; the corners are scattered with fp32 atomics, so the summation order is not fixed.
+__global__ void __launch_bounds__(256)
+warp_volume_backward_kernel(const float* __restrict__ grad_out, int C, const float* __restrict__ t1,
+                            const float* __restrict__ KR, const float* __restrict__ rays, const float* __restrict__ dpl,
+                            int V, int D, int w, int h, float cx, float cy, float* __restrict__ g_imgs) {
+  const int hw = w * h;
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)hw * D) return;
+  const int pix = (int)(idx % hw);
+  const int d = (int)(idx / hw);
+  const float r0 = rays[pix], r1 = rays[hw + pix], r2 = rays[2 * hw + pix];
+  const float dval = __ldg(dpl + d);
+  for (int v = 0; v < V; ++v) {
+    const Tap2D tp = warp_tap(t1, KR, v, r0, r1, r2, dval, cx, cy, w, h);
+    const float wt[4] = {tp.w_nw, tp.w_ne, tp.w_sw, tp.w_se};
+    const int off[4] = {tp.o_nw, tp.o_ne, tp.o_sw, tp.o_se};
+    if (wt[0] == 0.f && wt[1] == 0.f && wt[2] == 0.f && wt[3] == 0.f) continue;
+    const float* go = grad_out + ((size_t)v * C * D + d) * hw + pix;
+    float* gi = g_imgs + (size_t)v * C * hw;
+    for (int c = 0; c < C; ++c) {
+      const float g = __ldg(go + (size_t)c * D * hw);
+      if (g == 0.f) continue;
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        if (wt[k] != 0.f) atomicAdd(gi + (size_t)c * hw + off[k], g * wt[k]);
+    }
+  }
+}
+
 __global__ void warp_setup_kernel(const float* __restrict__ K, const float* __restrict__ R,
                                   const float* __restrict__ t, int V, float* __restrict__ t1,
                                   float* __restrict__ KR) {
@@ -159,6 +197,24 @@ int nrgbd_warp_to_volume(const float* imgs_packed, int c_cnt, int c_off, int C_t
   warp_volume_kernel<0><<<ceil_div(n, 256), 256, 0, st>>>(reinterpret_cast<const float4*>(imgs_packed), c_cnt,
                                                           c_off, C_total, t1, KR, rays, d_planes, V, D, w, h, cx,
                                                           cy, out, nullptr, nullptr, nullptr, 0);
+  NRGBD_COUNT(2);
+  NRGBD_LAUNCH_CHECK();
+  return NRGBD_OK;
+}
+
+// Gradient of nrgbd_warp_to_volume with respect to the source images, all C channels at once.
+// grad_out: [V][C][D][hw]; g_imgs: [V][C][hw], zeroed here before the scatter; ws: V*12 floats.
+int nrgbd_warp_to_volume_backward(const float* grad_out, int C, int V, int D, int h, int w, const float* K,
+                                  const float* R, const float* t, const float* rays, const float* d_planes, float cx,
+                                  float cy, float* ws, float* g_imgs, cudaStream_t st) {
+  NRGBD_REQUIRE(grad_out && K && R && t && rays && d_planes && ws && g_imgs, "null pointer");
+  NRGBD_REQUIRE(C > 0 && V > 0 && D > 0 && h > 0 && w > 0, "empty problem");
+  float* t1 = ws; float* KR = ws + 3 * V;
+  warp_setup_kernel<<<ceil_div(V, 32), 32, 0, st>>>(K, R, t, V, t1, KR);
+  NRGBD_CUDA_CHECK(cudaMemsetAsync(g_imgs, 0, sizeof(float) * (size_t)V * C * h * w, st));
+  long long n = (long long)h * w * D;
+  warp_volume_backward_kernel<<<ceil_div(n, 256), 256, 0, st>>>(grad_out, C, t1, KR, rays, d_planes, V, D, w, h, cx, cy,
+                                                                g_imgs);
   NRGBD_COUNT(2);
   NRGBD_LAUNCH_CHECK();
   return NRGBD_OK;

@@ -179,27 +179,68 @@ def est_swp_volume_v4(feat_img_ref, feat_img_src, d_candi, R, t, cam_intrinsic, 
                               cx, cy, float(costV_sigma), metric)
 
 
-def _warp_views(feat_img_src, d_candi, R, t, K, rays, cx, cy):
+def _warp_forward(x, D, K, Rs, ts, rays, dpl, cx, cy):
+    """x [V,C,h,w] float32 contiguous -> [V,C,D,h,w], in 4-channel chunks."""
     L = _lib.lib()
+    V, C, H, W = x.shape
+    ws = torch.empty(L.nrgbd_sweep_workspace_floats(V), device=x.device, dtype=torch.float32)
+    out = torch.empty((V, C, D, H, W), device=x.device, dtype=torch.float32)
+    for c0 in range(0, C, 4):
+        cc = min(4, C - c0)
+        chunk = x[:, c0:c0 + cc].contiguous()
+        wide, narrow = pack_features(chunk)          # cc == 4 packs as wide [V,hw,4]: same memory layout
+        packed = narrow if narrow is not None else wide
+        check(L.nrgbd_warp_to_volume(ptr(packed), cc, c0, C, V, D, H, W, ptr(K), ptr(Rs), ptr(ts), ptr(rays),
+                                     ptr(dpl), _F(cx), _F(cy), ptr(ws), ptr(out), _stream()))
+    return out
+
+
+class _WarpToVolume(torch.autograd.Function):
+    """warp_img_feats_v3 / _mgpu with the image-feature gradients autograd gives the reference through
+    F.grid_sample (homography.py:183-280). Poses, intrinsics and plane depths get no gradient, as in the sweep.
+    Inputs after the camera terms are the views as the caller passed them (V tensors 1xCxhxw, or one NxCxhxw
+    tensor); each gets its own gradient."""
+
+    @staticmethod
+    def forward(ctx, K, Rs, ts, rays, dpl, cx, cy, *imgs):
+        x = torch.cat([i.detach().float() for i in imgs], dim=0).contiguous()
+        ctx.save_for_backward(K, Rs, ts, rays, dpl)
+        ctx.meta = (cx, cy, x.shape, [(i.shape[0], i.dtype) for i in imgs])
+        return _warp_forward(x, dpl.numel(), K, Rs, ts, rays, dpl, cx, cy)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        L = _lib.lib()
+        K, Rs, ts, rays, dpl = ctx.saved_tensors
+        cx, cy, (V, C, H, W), views = ctx.meta
+        dev = K.device
+        with torch.cuda.device(dev):
+            go = grad_out.detach().float().contiguous()
+            ws = torch.empty(L.nrgbd_sweep_workspace_floats(V), device=dev, dtype=torch.float32)
+            g = torch.empty((V, C, H, W), device=dev, dtype=torch.float32)
+            check(L.nrgbd_warp_to_volume_backward(ptr(go), C, V, dpl.numel(), H, W, ptr(K), ptr(Rs), ptr(ts), ptr(rays),
+                                                  ptr(dpl), _F(cx), _F(cy), ptr(ws), ptr(g), _stream()))
+        grads, v0 = [], 0
+        for n, dt in views:
+            grads.append(g[v0:v0 + n].to(dt))
+            v0 += n
+        return (None,) * 7 + tuple(grads)
+
+
+def _warp_views(feat_img_src, d_candi, R, t, K, rays, cx, cy):
     is_list = isinstance(R, (list, tuple)) and isinstance(t, (list, tuple))
     imgs = list(feat_img_src) if is_list else [feat_img_src]
     dev = _dev(imgs[0])
     with torch.cuda.device(dev):
-        x = torch.cat([i.float() for i in imgs], dim=0).contiguous()       # [V,C,h,w]
-        V, C, H, W = x.shape
         D = len(d_candi)
         dpl = _planes(d_candi, dev)
         Rs, ts = _stack_Rt(list(R) if is_list else [R], list(t) if is_list else [t], dev)
-        ws = torch.empty(L.nrgbd_sweep_workspace_floats(V), device=dev, dtype=torch.float32)
-        out = torch.empty((V, C, D, H, W), device=dev, dtype=torch.float32)
-        for c0 in range(0, C, 4):
-            cc = min(4, C - c0)
-            chunk = x[:, c0:c0 + cc].contiguous()
-            wide, narrow = pack_features(chunk)          # cc == 4 packs as wide [V,hw,4]: same memory layout
-            packed = narrow if narrow is not None else wide
-            check(L.nrgbd_warp_to_volume(ptr(packed), cc, c0, C, V, D, H, W, ptr(K), ptr(Rs), ptr(ts), ptr(rays),
-                                         ptr(dpl), _F(cx), _F(cy), ptr(ws), ptr(out), _stream()))
-    outs = [out[v] for v in range(V)]
+        if torch.is_grad_enabled() and any(i.requires_grad for i in imgs):
+            out = _WarpToVolume.apply(K, Rs, ts, rays, dpl, cx, cy, *imgs)
+        else:
+            x = torch.cat([i.float() for i in imgs], dim=0).contiguous()       # [V,C,h,w]
+            out = _warp_forward(x, D, K, Rs, ts, rays, dpl, cx, cy)
+    outs = [out[v] for v in range(out.shape[0])]
     return outs if is_list else outs[0]
 
 
@@ -207,7 +248,8 @@ def warp_img_feats_v3(feat_img_src, d_candi, R, t, cam_intrinsic):
     r'''
     Warp the feat_imgs_src to the reference view for all candidate depths (homography.py:234-280)
     feat_img_src - list of source image features (each NCHW, N=1) or one NCHW tensor
-    Returns a list of V tensors C x D x h x w (or one tensor).
+    Returns a list of V tensors C x D x h x w (or one tensor). Differentiable w.r.t. the source features when
+    they require grad (one gradient per list element); R, t and the intrinsics get none.
     '''
     first = feat_img_src[0] if isinstance(feat_img_src, (list, tuple)) else feat_img_src
     K, rays = _cam_tensors(cam_intrinsic, _dev(first))
@@ -256,6 +298,49 @@ def resample_params(cam_intrinsic, d_candi, d_candi_new=None):
     return d_pts, np.float32(math.tan(hhfov)), np.float32(math.tan(hvfov)), z_half, z_radius
 
 
+def _resample_forward(vol, E, rays, dp, D, H, W, tan_hh, tan_hv, z_half, z_radius, pad, clamp):
+    L = _lib.lib()
+    out = torch.empty((D, H, W), device=vol.device, dtype=torch.float32)
+    lo, hi = (clamp if clamp is not None else (0., 0.))
+    check(L.nrgbd_resample_dpv(ptr(vol), H * W, 1, ptr(E), ptr(rays), ptr(dp), D, H, W, _F(tan_hh), _F(tan_hv),
+                               _F(z_half), _F(z_radius), _F(pad), 1 if clamp is not None else 0,
+                               _F(lo), _F(hi), ptr(out), H * W, 1, _stream()))
+    return out
+
+
+class _ResampleDpv(torch.autograd.Function):
+    """resample_vol_cuda with the volume gradient autograd gives the reference through _set_vol_border +
+    grid_sample(bilinear, border) 3-D (homography.py:713-716), and through torch.clamp for the `clamp` extension.
+    rel_extM, the intrinsics and the plane depths get no gradient."""
+
+    @staticmethod
+    def forward(ctx, src_vol, E, rays, dp, params, pad, clamp):
+        N, D, H, W = src_vol.shape
+        vol = src_vol.detach().float().contiguous()
+        ctx.save_for_backward(vol, E, rays, dp)
+        ctx.meta = (params, pad, clamp, src_vol.dtype)
+        return _resample_forward(vol, E, rays, dp, D, H, W, *params, pad, clamp)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        L = _lib.lib()
+        vol, E, rays, dp = ctx.saved_tensors
+        (tan_hh, tan_hv, z_half, z_radius), pad, clamp, dtype = ctx.meta
+        N, D, H, W = vol.shape
+        lo, hi = (clamp if clamp is not None else (0., 0.))
+        with torch.cuda.device(vol.device):
+            go = grad_out.detach().float().contiguous()
+            g = torch.empty((D, H, W), device=vol.device, dtype=torch.float32)
+            check(L.nrgbd_resample_dpv_backward(ptr(vol), H * W, 1, ptr(E), ptr(rays), ptr(dp), D, H, W, _F(tan_hh),
+                                                _F(tan_hv), _F(z_half), _F(z_radius), _F(pad),
+                                                1 if clamp is not None else 0, _F(lo), _F(hi), ptr(go), H * W, 1,
+                                                ptr(g), _stream()))
+            g = g.unsqueeze(0)
+            if N > 1:          # the forward reads the first volume only
+                g = torch.cat([g, torch.zeros((N - 1, D, H, W), device=vol.device, dtype=torch.float32)])
+        return g.to(dtype), None, None, None, None, None, None
+
+
 def resample_vol_cuda(src_vol, rel_extM, cam_intrinsic=None, d_candi=None, d_candi_new=None,
                       padding_value=0., output_tensor=False, is_debug=False,
                       PointsDs_ref_cam_coord_in=None, clamp=None):
@@ -265,26 +350,25 @@ def resample_vol_cuda(src_vol, rel_extM, cam_intrinsic=None, d_candi=None, d_can
     d_candi : candidate depth values for the src view;
     d_candi_new : candidate depth values for the ref view.
     `clamp=(lo, hi)` (extension) fuses the clamp of test_utils/test_KVNet.py:58-59.
+    Differentiable w.r.t. src_vol when it requires grad (faces of the volume get zero gradient, as the reference
+    overwrites them before sampling); rel_extM, the intrinsics and the plane depths get none.
     '''
     assert d_candi is not None, 'd_candi should be some np.array object'
     if PointsDs_ref_cam_coord_in is not None or is_debug:
         raise _lib.NrgbdError('resample_vol_cuda: PointsDs_ref_cam_coord_in / is_debug are not supported '
                               '(the point cloud is never materialised)')
-    L = _lib.lib()
     dev = _dev(src_vol)
     with torch.cuda.device(dev):
         N, D, H, W = src_vol.shape
         K, rays = _cam_tensors(cam_intrinsic, dev)
         d_pts, tan_hh, tan_hv, z_half, z_radius = resample_params(cam_intrinsic, d_candi, d_candi_new)
         dp = planes_tensor(d_pts, dev)
-        E = rel_extM.to(device=dev, dtype=torch.float32).contiguous()
+        E = rel_extM.detach().to(device=dev, dtype=torch.float32).contiguous()
+        params = (tan_hh, tan_hv, z_half, z_radius)
+        if torch.is_grad_enabled() and src_vol.requires_grad:
+            return _ResampleDpv.apply(src_vol, E, rays, dp, params, float(padding_value), clamp)
         vol = src_vol.float().contiguous()
-        out = torch.empty((D, H, W), device=dev, dtype=torch.float32)
-        lo, hi = (clamp if clamp is not None else (0., 0.))
-        check(L.nrgbd_resample_dpv(ptr(vol), H * W, 1, ptr(E), ptr(rays), ptr(dp), D, H, W, _F(tan_hh), _F(tan_hv),
-                                   _F(z_half), _F(z_radius), _F(float(padding_value)), 1 if clamp is not None else 0,
-                                   _F(lo), _F(hi), ptr(out), H * W, 1, _stream()))
-    return out
+        return _resample_forward(vol, E, rays, dp, D, H, W, *params, float(padding_value), clamp)
 
 
 # ---------------------------------------------------------------------------------------------------------------
