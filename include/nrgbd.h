@@ -101,7 +101,8 @@ int nrgbd_knet_input_volume(const float* src_rgb_packed, const float* ref_rgb_pa
                             nrgbd_stream_t stream);
 
 /* the same volume, optionally (also / only: out may be NULL) as the split-fp16 operand pair (out_hi, out_lo: half
- * [D][hw][CK], CK = 16 or 32) of the f16-pair convolution that consumes it - see nrgbd_conv_nhwc_h2 */
+ * [D][hw][CK], CK = 16 or 32) of the f16-pair convolution that consumes it - see nrgbd_conv_nhwc_h2. out_lo == NULL with
+ * out_hi set: only hi = RN_f16(volume) is written (the operand of the single-product convolution). */
 int nrgbd_knet_input_volume_pair(const float* src_rgb_packed, const float* ref_rgb_packed,
                                  const float* bv_cur_hwd, const float* bv_pred_hwd, int V, int D, int h, int w,
                                  int CK, const float* K, const float* R, const float* t, const float* rays,
@@ -270,7 +271,8 @@ int nrgbd_bn_apply_stats(const float* x, const double* stats, double count, cons
 /* same pass, also (or only: y may be NULL) emitting the result as the split-fp16 operand pair (y_hi, y_lo: half tensors with
  * x's layout; both may be NULL) of the f16-pair convolution that consumes it - see nrgbd_conv_nhwc_h2. The residual is either
  * the fp32 tensor `res` or the operand pair (res_hi, res_lo) of a tensor that was only ever written as a pair (its value
- * hi + lo * 2^-11 carries 22 significand bits); at most one of the two forms. rezero_counter
+ * hi + lo * 2^-11 carries 22 significand bits); at most one of the two forms. y_hi set and y_lo == NULL: only
+ * hi = RN_f16(result) is written (the operand of the single-product convolution). rezero_counter
  * (optional, a zero-initialised device word): the last block to have read `stats` sets them back to zero, so the next
  * convolution accumulates into a clean buffer without a memset in between. */
 int nrgbd_bn_apply_stats_pair(const float* x, double* stats, double count, const float* gamma, const float* beta,
@@ -344,7 +346,13 @@ int nrgbd_conv_transpose2d_k4s2_nhwc_tc2(const float* x, int N, int Hin, int Win
  * by nrgbd_pack_conv_weight_h2 -> [taps][2 (hi | lo)][Cout_pad][Cin_pad] halves. Stride-1 filters stage ONE halo tile per
  * 32-channel chunk for all in-plane taps (the tap-per-box kernels re-read the tile kh*kw times from L2).
  * Same convolution semantics, outputs (fp32) and BatchNorm statistics as nrgbd_conv_nhwc. */
+/* Single product (conv_math = 'f16'): a pair whose lo is NULL is a plain fp16 tensor. Every entry below taking x_lo runs
+ * the single-product kernel when x_lo == NULL: out = sum RN_f16(x) * RN_f16(w) in fp32 (RN_f16: round to nearest even,
+ * saturating at +-65504), one wgmma per product, the packed weights' lo half never loaded; bias, LeakyReLU, statistics
+ * and the affine epilogue unchanged. A pair output with y_lo == NULL stores only hi = RN_f16(result) (pad channels as
+ * zeros). The residual of the affine epilogue keeps its pair form (res_hi and res_lo both set, or both NULL). */
 int nrgbd_conv_h2_plan(int Cin, int Cout, int* Cin_pad, int* Cout_pad, int* BN);   /* channel padding: Cin to 32; Cout into equal chunks of BN <= 128 */
+/* lo == NULL: only hi = RN_f16(x) is written, a plain fp32 -> fp16 conversion (saturating) */
 int nrgbd_split_f16_pair(const float* x, long long n, void* hi, void* lo, nrgbd_stream_t stream);
 int nrgbd_pack_conv_weight_h2(const float* w, int transposed, int Cout, int Cin, int taps, int Cin_pad, int Cout_pad, void* out,
                               nrgbd_stream_t stream);

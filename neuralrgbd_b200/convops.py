@@ -261,10 +261,12 @@ def h2_plan(Cin, Cout):
     return a.value, b.value, c.value          # Cin_pad, Cout_pad, BN
 
 
-def split_f16_pair(xc):
-    """fp32 tensor -> (hi, lo) float16 tensors of the same shape: x = hi + lo * 2^-11."""
+def split_f16_pair(xc, single=False):
+    """fp32 tensor -> (hi, lo) float16 tensors of the same shape: x = hi + lo * 2^-11. single: lo = None and hi = RN_f16(x),
+    the operand of the single-product convolution (conv_math='f16')."""
     L = _lib.lib()
-    hi = torch.empty(xc.shape, device=xc.device, dtype=torch.float16); lo = torch.empty_like(hi)
+    hi = torch.empty(xc.shape, device=xc.device, dtype=torch.float16)
+    lo = None if single else torch.empty_like(hi)
     check(L.nrgbd_split_f16_pair(ptr(xc), xc.numel(), ptr(hi), ptr(lo), _st()))
     return hi, lo
 
@@ -285,8 +287,9 @@ def pack_weight_h2(w, transposed=False):
     return out, Cin_pad, Cout_pad, BN
 
 
-def conv_h2(x, w, bias=None, stride=1, pad=0, dilation=1, leaky=False, want_stats=False):
-    """f16-pair tensor-core counterpart of conv() (same arguments / returns)."""
+def conv_h2(x, w, bias=None, stride=1, pad=0, dilation=1, leaky=False, want_stats=False, single=False):
+    """f16-pair tensor-core counterpart of conv() (same arguments / returns). single: the single-product kernel (x_lo = NULL),
+    sum RN_f16(x) * RN_f16(w) in fp32."""
     L = _lib.lib()
     is3d = x.dim() == 5
     N = x.shape[0]
@@ -295,7 +298,7 @@ def conv_h2(x, w, bias=None, stride=1, pad=0, dilation=1, leaky=False, want_stat
     Cout, Cin = w.shape[0], w.shape[1]
     wp, Cin_pad, Cout_pad, BN = pack_weight_h2(w)
     xc = to_cl_padded(x, Cin_pad)
-    xh, xl = split_f16_pair(xc)
+    xh, xl = split_f16_pair(xc, single)
     kd = w.shape[2] if is3d else 1
     kh, kw = w.shape[-2], w.shape[-1]
     Ho = (Hin + 2 * pad - dilation * (kh - 1) - 1) // stride + 1
@@ -310,9 +313,10 @@ def conv_h2(x, w, bias=None, stride=1, pad=0, dilation=1, leaky=False, want_stat
     return (out, stats) if want_stats else out
 
 
-def conv_h2_pair_out(x, w, bias=None, stride=1, pad=0, dilation=1, leaky=False):
+def conv_h2_pair_out(x, w, bias=None, stride=1, pad=0, dilation=1, leaky=False, single=False):
     """conv_h2 whose result is written only as the operand pair of the next convolution (nrgbd_conv_nhwc_h2_pair). Returns the
-    fp32 value of the pair, hi + lo * 2^-11, as NCHW / NCDHW, and the raw (hi, lo) half tensors (channels-last, Cs = pad32)."""
+    fp32 value of the pair, hi + lo * 2^-11, as NCHW / NCDHW, and the raw (hi, lo) half tensors (channels-last, Cs = pad32).
+    single: x_lo = y_lo = NULL - the single-product kernel, the output stored as hi only (lo returned as None)."""
     L = _lib.lib()
     is3d = x.dim() == 5
     N = x.shape[0]
@@ -320,7 +324,7 @@ def conv_h2_pair_out(x, w, bias=None, stride=1, pad=0, dilation=1, leaky=False):
     Hin, Win = x.shape[-2], x.shape[-1]
     Cout, Cin = w.shape[0], w.shape[1]
     wp, Cin_pad, Cout_pad, BN = pack_weight_h2(w)
-    xh, xl = split_f16_pair(to_cl_padded(x, Cin_pad))
+    xh, xl = split_f16_pair(to_cl_padded(x, Cin_pad), single)
     kd = w.shape[2] if is3d else 1
     kh, kw = w.shape[-2], w.shape[-1]
     Ho = (Hin + 2 * pad - dilation * (kh - 1) - 1) // stride + 1
@@ -329,10 +333,10 @@ def conv_h2_pair_out(x, w, bias=None, stride=1, pad=0, dilation=1, leaky=False):
     shape = (N,) + ((Din,) if is3d else ()) + (Ho, Wo, Cs)
     # poisoned: every element, pad channels included, must be written by the kernel
     yh = torch.full(shape, float('nan'), device=x.device, dtype=torch.float16)
-    yl = torch.full(shape, float('nan'), device=x.device, dtype=torch.float16)
+    yl = None if single else torch.full(shape, float('nan'), device=x.device, dtype=torch.float16)
     check(L.nrgbd_conv_nhwc_h2_pair(ptr(xh), ptr(xl), N, Din, Hin, Win, Cin_pad, Cin_pad, ptr(wp), ptr(bias), Cout, Cout_pad, BN,
                                     kd, kh, kw, stride, pad, dilation, ptr(yh), ptr(yl), Ho, Wo, Cs, 1 if leaky else 0, _st()))
-    val = yh.float() + yl.float() * (1.0 / 2048.0)
+    val = yh.float() if single else yh.float() + yl.float() * (1.0 / 2048.0)
     return from_cl(val.contiguous(), Cout), yh, yl
 
 
@@ -346,10 +350,13 @@ def bn_eval_coeffs(gamma, beta, running_mean, running_var, eps=1e-5):
     return scale, shift
 
 
-def conv_h2_affine(x, w, scale, shift, stride=1, pad=0, dilation=1, res=None, res_pair=False, relu=False, pair_out=False):
+def conv_h2_affine(x, w, scale, shift, stride=1, pad=0, dilation=1, res=None, res_pair=False, relu=False, pair_out=False,
+                   single=False):
     """Eval-mode convbn in one kernel (nrgbd_conv_nhwc_h2_affine): relu(conv(x, w) * scale + shift + res). res (NCHW / NCDHW,
     the output's shape) is passed as fp32 or, with res_pair, as its split-fp16 operand pair. pair_out: the result is written
-    only as the operand pair of the next convolution; returned as its fp32 value hi + lo * 2^-11 plus the raw (hi, lo)."""
+    only as the operand pair of the next convolution; returned as its fp32 value hi + lo * 2^-11 plus the raw (hi, lo).
+    single: the single-product kernel (x_lo = NULL); a pair output is stored as hi only (y_lo = NULL). The residual keeps
+    its pair form."""
     L = _lib.lib()
     is3d = x.dim() == 5
     N = x.shape[0]
@@ -357,7 +364,7 @@ def conv_h2_affine(x, w, scale, shift, stride=1, pad=0, dilation=1, res=None, re
     Hin, Win = x.shape[-2], x.shape[-1]
     Cout = w.shape[0]
     wp, Cin_pad, Cout_pad, BN = pack_weight_h2(w)
-    xh, xl = split_f16_pair(to_cl_padded(x, Cin_pad))
+    xh, xl = split_f16_pair(to_cl_padded(x, Cin_pad), single)
     kd = w.shape[2] if is3d else 1
     kh, kw = w.shape[-2], w.shape[-1]
     Ho = (Hin + 2 * pad - dilation * (kh - 1) - 1) // stride + 1
@@ -374,21 +381,22 @@ def conv_h2_affine(x, w, scale, shift, stride=1, pad=0, dilation=1, res=None, re
     y = yh = yl = None
     if pair_out:
         yh = torch.full(shape, float('nan'), device=x.device, dtype=torch.float16)     # every element must be written
-        yl = torch.full(shape, float('nan'), device=x.device, dtype=torch.float16)
+        yl = None if single else torch.full(shape, float('nan'), device=x.device, dtype=torch.float16)
     else:
         y = torch.zeros(shape, device=x.device, dtype=torch.float32)
     check(L.nrgbd_conv_nhwc_h2_affine(ptr(xh), ptr(xl), N, Din, Hin, Win, Cin_pad, Cin_pad, ptr(wp), Cout, Cout_pad, BN, kd, kh, kw,
                                       stride, pad, dilation, ptr(scale), ptr(shift), ptr(r), ptr(rh), ptr(rl), 1 if relu else 0,
                                       ptr(y), ptr(yh), ptr(yl), Ho, Wo, Cs, 0, _st()))
     if pair_out:
-        return from_cl((yh.float() + yl.float() * (1.0 / 2048.0)).contiguous(), Cout), yh, yl
+        val = yh.float() if single else yh.float() + yl.float() * (1.0 / 2048.0)
+        return from_cl(val.contiguous(), Cout), yh, yl
     return from_cl(y, Cout)
 
 
-def conv_cout1_h2(x, w, bias=0.0):
+def conv_cout1_h2(x, w, bias=0.0, single=False):
     """Single-output-channel k3 convolution (K-Net's last layer, models/basic.py:136-137) the way the engine runs it:
     a pointwise f16-pair conv to one channel per tap + nrgbd_tap_gather_sum. x [N, C, D, H, W] (or [N, C, H, W]),
-    w [1, C, 3, 3, 3] (or [1, C, 3, 3]) -> [N, 1, D, H, W] ([N, 1, H, W])."""
+    w [1, C, 3, 3, 3] (or [1, C, 3, 3]) -> [N, 1, D, H, W] ([N, 1, H, W]). single: the pointwise conv on hi only."""
     L = _lib.lib()
     is3d = x.dim() == 5
     N = x.shape[0]
@@ -399,7 +407,7 @@ def conv_cout1_h2(x, w, bias=0.0):
     taps = kd * 9
     wt = w[0].reshape(Cin, taps, 1, 1)                  # [Cin][Cout' = taps][1][1]: the transposed-kind source layout
     wp, Cin_pad, Cout_pad, BN = pack_weight_h2(wt, transposed=True)
-    xh, xl = split_f16_pair(to_cl_padded(x, Cin_pad))
+    xh, xl = split_f16_pair(to_cl_padded(x, Cin_pad), single)
     Cs = pad4(taps)
     q = torch.empty((N, D, H, W, Cs), device=x.device, dtype=torch.float32)
     check(L.nrgbd_conv_nhwc_h2(ptr(xh), ptr(xl), N, D, H, W, Cin_pad, Cin_pad, ptr(wp), None, taps, Cout_pad, BN, 1, 1, 1, 1, 0, 1,
@@ -409,13 +417,13 @@ def conv_cout1_h2(x, w, bias=0.0):
     return out
 
 
-def conv_transpose2d_h2(x, w, bias=None, leaky=False):
+def conv_transpose2d_h2(x, w, bias=None, leaky=False, single=False):
     L = _lib.lib()
     N, Cin, Hin, Win = x.shape
     Cout = w.shape[1]
     wp, Cin_pad, Cout_pad, BN = pack_weight_h2(w, transposed=True)
     xc = to_cl_padded(x, Cin_pad)
-    xh, xl = split_f16_pair(xc)
+    xh, xl = split_f16_pair(xc, single)
     Cs_out = pad4(Cout)
     y = torch.zeros((N, 2 * Hin, 2 * Win, Cs_out), device=x.device, dtype=torch.float32)
     check(L.nrgbd_conv_transpose2d_k4s2_nhwc_h2(ptr(xh), ptr(xl), N, Hin, Win, Cin_pad, Cin_pad, ptr(wp), ptr(bias), Cout,

@@ -378,7 +378,8 @@ bn_apply_stats_kernel(const float* __restrict__ x, const double* __restrict__ st
       if (y_hi) {                      // the consumer is an f16-pair convolution: emit its operand planes in the same pass
         uint2 h, l;
         nrgbd_split_pair4(o, h, l);
-        y_hi[i] = h; y_lo[i] = l;
+        y_hi[i] = h;
+        if (y_lo) y_lo[i] = l;         // no y_lo: hi only, the plain fp16 operand of a single-product convolution
       }
     }
   }
@@ -576,13 +577,14 @@ int nrgbd_bn_apply_stats(const float* x, const double* stats, double count, cons
 
 // Same pass, additionally (or only: y may be NULL) writing the result as the split-fp16 operand pair of the f16-pair
 // convolution that consumes it (nrgbd_conv_nhwc_h2): y_hi / y_lo are half tensors with x's layout (both may be NULL).
+// y_hi set and y_lo NULL: only hi = RN_f16(result) is written (the operand of the single-product convolution).
 // rezero_counter (optional): a zero-initialised device word; when given, the last block to have read `stats` sets them back
 // to zero (and the word back to 0), so the next convolution can accumulate into `stats` without a memset in between.
 int nrgbd_bn_apply_stats_pair(const float* x, double* stats, double count, const float* gamma, const float* beta, float eps,
                               float* run_mean, float* run_var, float momentum, const float* res, const void* res_hi, const void* res_lo,
                               int relu, long long n_pos, int Cs, int C, float* y, void* y_hi, void* y_lo, unsigned int* rezero_counter,
                               cudaStream_t st) {
-  NRGBD_REQUIRE(x && stats && gamma && beta && (y || (y_hi && y_lo)) && (y_hi == nullptr) == (y_lo == nullptr) && Cs % 4 == 0 && C <= Cs &&
+  NRGBD_REQUIRE(x && stats && gamma && beta && (y || y_hi) && !(y_lo && !y_hi) && Cs % 4 == 0 && C <= Cs &&
                     C <= 512 && n_pos > 0 && count > 0, "bad arguments");
   NRGBD_REQUIRE((res_hi == nullptr) == (res_lo == nullptr) && !(res && res_hi), "the residual is either an fp32 tensor or an operand pair");
   const uint2* rh = reinterpret_cast<const uint2*>(res_hi);

@@ -33,6 +33,12 @@
 //   warp 8      TMA producer: halo / tap box of the hi and the lo activation planes into the A ring, G taps of the hi and
 //               lo K-major weight tiles into the B ring; expect-tx mbarriers. It runs on into the next tile's stages, so
 //               that tile's first loads overlap this tile's last steps and epilogue.
+//
+// Single product (ONE, conv_math = 'f16', selected by x_lo == NULL): out = sum RN_f16(a) * RN_f16(b) in fp32. The
+// producer loads only the hi activation box and the hi weight slices (half the expect-tx bytes), the ring slots hold hi
+// only (the same shared memory holds twice the stages), and the consumers issue one wgmma per (tap, K slice) into the
+// main accumulators; there are no cross accumulators. The packed weights keep their [tap][hi | lo] layout: lo is never
+// loaded. Every epilogue is the same.
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -112,8 +118,8 @@ __device__ __forceinline__ void wg_mma(float* d, uint64_t a, uint64_t b) {
 }
 
 // BN: output channels per CTA (16..128). TF32: operand kind. G: in-plane taps per pipeline step (one weight box and one
-// barrier round trip per G taps). AFF: affine epilogue (see WgConv).
-template <int BN, bool TF32, int G, bool AFF>
+// barrier round trip per G taps). AFF: affine epilogue (see WgConv). ONE: single product, hi operands only (fp16 only).
+template <int BN, bool TF32, int G, bool AFF, bool ONE>
 __global__ void __launch_bounds__(WG_THREADS, BN <= 64 ? 2 : 1)
 conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo, const WgParams p) {
@@ -122,7 +128,9 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
   constexpr float SCALE = TF32 ? 1.f : 1.f / 2048.f;
   constexpr uint32_t B_HALF = (uint32_t)(G * BN * RB);
   constexpr int NJ = BN / 8;                          // 8-column accumulator blocks
+  static_assert(!(ONE && TF32), "the single-product form is built for fp16 operands only");
   // shared memory: [A ring: stages_a x (hi | lo)][B ring: stages_b x (hi G taps | lo G taps)][column sums 8 x 2 x BN floats]
+  // (ONE: the slots hold hi only)
   //                [CTA column sums 2 x BN doubles][barriers]
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t base = smem_u32(smem_raw);
@@ -175,15 +183,15 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
                 mbar_expect_tx(bar_afull + 8 * sa, p.a_tx_bytes);
                 const uint32_t dst = base + (uint32_t)sa * p.a_stage_bytes;
                 tma_load_5d(dst, &tm_a_hi, bar_afull + 8 * sa, cc * BKC, cx, cy, cz, n0);
-                tma_load_5d(dst + p.a_tile_bytes, &tm_a_lo, bar_afull + 8 * sa, cc * BKC, cx, cy, cz, n0);
+                if constexpr (!ONE) tma_load_5d(dst + p.a_tile_bytes, &tm_a_lo, bar_afull + 8 * sa, cc * BKC, cx, cy, cz, n0);
                 if (++sa == p.stages_a) { sa = 0; pha ^= 1u; }
               }
               mbar_wait(bar_bempty + 8 * sb, phb ^ 1u);
-              mbar_expect_tx(bar_bfull + 8 * sb, 2 * B_HALF);
+              mbar_expect_tx(bar_bfull + 8 * sb, (ONE ? 1 : 2) * B_HALF);
               const uint32_t dst = b_ring + (uint32_t)sb * p.b_stage_bytes;
               const int ws = p.wsel[kz * p.n_tap + tap];
               tma_load_3d(dst, &tm_b_hi, bar_bfull + 8 * sb, cc * BKC, cbase, ws);
-              tma_load_3d(dst + B_HALF, &tm_b_lo, bar_bfull + 8 * sb, cc * BKC, cbase, ws);
+              if constexpr (!ONE) tma_load_3d(dst + B_HALF, &tm_b_lo, bar_bfull + 8 * sb, cc * BKC, cbase, ws);
               if (++sb == p.stages_b) { sb = 0; phb ^= 1u; }
             }
           }
@@ -196,13 +204,13 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
   // ===== consumers: 64 GEMM rows per warpgroup; 16x8 tile: cw owns tile rows [8 cw, 8 cw + 8), 8x16 tile: columns
   // [8 cw, 8 cw + 8) of all 8 rows. Either way core-matrix group g is one tile row, one halo pitch down. =====
   const int cw = warp >> 2, w4 = warp & 3;
-  float acc_m[BN / 2], acc_c[BN / 2];
+  float acc_m[BN / 2], acc_c[ONE ? 1 : BN / 2];
   const uint32_t wg_off = (uint32_t)cw * p.wg_row16 * 16u;
   int sa = 0, sb = 0, sa_cur = 0, tap = 0;
   uint32_t pha = 0, phb = 0;
   for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
 #pragma unroll
-    for (int k = 0; k < BN / 2; ++k) { acc_m[k] = 0.f; acc_c[k] = 0.f; }
+    for (int k = 0; k < BN / 2; ++k) { acc_m[k] = 0.f; if constexpr (!ONE) acc_c[k] = 0.f; }
     int rel_a = -1, rel_b = -1;                       // slots of the previous step, released once it has retired
     for (int step = 0; step < n_steps; ++step) {
       const bool new_a = !p.halo || tap == 0;
@@ -223,8 +231,10 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
           const uint32_t ah = ao + 32u * ks, al = ah + p.a_tile_bytes;
           const uint32_t bh = b_hi + (uint32_t)(g * BN * RB) + 32u * ks, bl = bh + B_HALF;
           wg_mma<BN, TF32>(acc_m, wg_desc(ah, p.a_desc_hi), wg_desc(bh, p.b_desc_hi));
-          wg_mma<BN, TF32>(acc_c, wg_desc(ah, p.a_desc_hi), wg_desc(bl, p.b_desc_hi));
-          wg_mma<BN, TF32>(acc_c, wg_desc(al, p.a_desc_hi), wg_desc(bh, p.b_desc_hi));
+          if constexpr (!ONE) {
+            wg_mma<BN, TF32>(acc_c, wg_desc(ah, p.a_desc_hi), wg_desc(bl, p.b_desc_hi));
+            wg_mma<BN, TF32>(acc_c, wg_desc(al, p.a_desc_hi), wg_desc(bh, p.b_desc_hi));
+          }
         }
       }
       asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
@@ -266,7 +276,7 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
       pix[i] = (((long long)n0 * p.Dout + z0) * p.Hout + oy) * p.Wout + ox;
       if (!pair) dst_row[i] = p.y + pix[i] * (long long)p.Cs_out + p.c_off + cbase;
     }
-    if constexpr (AFF) {
+    if constexpr (AFF && !ONE) {
       // main + scale * cross for every column first: the cross accumulators die here, which leaves registers for the
       // residual loads of the store loop (no spills at BN = 64)
 #pragma unroll
@@ -288,7 +298,8 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
             if constexpr (AFF) {
               f = fmaf(acc_m[4 * j + 2 * i + e], part[c + e], part[BN + c + e]);      // residual and ReLU: in the store loop below
             } else {
-              f = fmaf(acc_c[4 * j + 2 * i + e], SCALE, acc_m[4 * j + 2 * i + e]);
+              if constexpr (ONE) f = acc_m[4 * j + 2 * i + e];
+              else f = fmaf(acc_c[4 * j + 2 * i + e], SCALE, acc_m[4 * j + 2 * i + e]);
               if (p.bias) f += __ldg(p.bias + cbase + c + e);
               if (p.leaky) f = f >= 0.f ? f : f * 0.01f;
             }
@@ -315,7 +326,7 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
           nrgbd_split_pair(v[i][0], h0, l0); nrgbd_split_pair(v[i][1], h1, l1);
           const long long o = pix[i] * (long long)p.Cs_out + cbase + c;
           *reinterpret_cast<__half2*>(p.y_hi + o) = __halves2half2(h0, h1);
-          *reinterpret_cast<__half2*>(p.y_lo + o) = __halves2half2(l0, l1);
+          if (p.y_lo) *reinterpret_cast<__half2*>(p.y_lo + o) = __halves2half2(l0, l1);   // no y_lo: the plain fp16 tensor hi
         } else if (vec2 && c + 1 < n_here) {
           *reinterpret_cast<float2*>(dst_row[i] + c) = make_float2(v[i][0], v[i][1]);
         } else {
@@ -437,17 +448,17 @@ inline uint32_t round_up(uint32_t v, uint32_t m) { return (v + m - 1) / m * m; }
 
 typedef void (*WgKernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const WgParams);
 
-template <bool TF32, int G, bool AFF = false>
+template <bool TF32, int G, bool AFF = false, bool ONE = false>
 WgKernel pick_kernel(int BN) {
   switch (BN) {
-    case 16: return conv_wg_kernel<16, TF32, G, AFF>;
-    case 32: return conv_wg_kernel<32, TF32, G, AFF>;
-    case 48: return conv_wg_kernel<48, TF32, G, AFF>;
-    case 64: return conv_wg_kernel<64, TF32, G, AFF>;
-    case 80: return conv_wg_kernel<80, TF32, G, AFF>;
-    case 96: return conv_wg_kernel<96, TF32, G, AFF>;
-    case 112: return conv_wg_kernel<112, TF32, G, AFF>;
-    case 128: return conv_wg_kernel<128, TF32, G, AFF>;
+    case 16: return conv_wg_kernel<16, TF32, G, AFF, ONE>;
+    case 32: return conv_wg_kernel<32, TF32, G, AFF, ONE>;
+    case 48: return conv_wg_kernel<48, TF32, G, AFF, ONE>;
+    case 64: return conv_wg_kernel<64, TF32, G, AFF, ONE>;
+    case 80: return conv_wg_kernel<80, TF32, G, AFF, ONE>;
+    case 96: return conv_wg_kernel<96, TF32, G, AFF, ONE>;
+    case 112: return conv_wg_kernel<112, TF32, G, AFF, ONE>;
+    case 128: return conv_wg_kernel<128, TF32, G, AFF, ONE>;
   }
   return nullptr;
 }
@@ -455,7 +466,8 @@ WgKernel pick_kernel(int BN) {
 // One launch: output channels [c_first, c_first + n_chunks * BN) in chunks of BN.
 int launch_chunks(const WgConv& c, WgParams p, int BN, int n_chunks, int c_first, cudaStream_t st) {
   const bool tf32 = c.tf32 != 0;
-  const int esize = tf32 ? 4 : 2, RB = BKC * esize;
+  const bool one = c.x_lo == nullptr;                 // single product: hi operands only (conv_wgmma checks fp16)
+  const int esize = tf32 ? 4 : 2, RB = BKC * esize, halves = one ? 1 : 2;
   p.c_first = c_first;
   // taps per pipeline step: a whole kernel row when the weight slices of the taps are consecutive (plain convolutions)
   int G = 1;
@@ -464,10 +476,11 @@ int launch_chunks(const WgConv& c, WgParams p, int BN, int n_chunks, int c_first
     for (int t = 1; t < p.n_kz * p.n_tap; ++t) consecutive = consecutive && c.wsel[t] == c.wsel[t - 1] + 1;
     if (consecutive) G = 3;
   }
-  // shared memory: two CTAs per SM when BN <= 64 and two A + two B stages fit half of the SM's 228 KB
+  // shared memory: two CTAs per SM when BN <= 64 and two A + two B stages fit half of the SM's 228 KB. Single-product
+  // stages are half the size, so the same plan gives them up to twice the depth (capped at 3 A and 8 B stages).
   const size_t extra = (size_t)8 * 2 * BN * 4 + (size_t)2 * BN * 8 + 256;
   auto plan = [&](size_t cap, int g, int& sa, int& sb) {
-    const size_t b_stage = (size_t)2 * g * BN * RB;
+    const size_t b_stage = (size_t)halves * g * BN * RB;
     sa = 2;
     if (cap < extra + 2 * (size_t)p.a_stage_bytes + 2 * b_stage) return false;
     sb = (int)((cap - extra - 2 * (size_t)p.a_stage_bytes) / b_stage);
@@ -482,24 +495,27 @@ int launch_chunks(const WgConv& c, WgParams p, int BN, int n_chunks, int c_first
   if (!ok) { cap = 232448; ok = plan(cap, G, sa, sb); }
   if (!ok) { nrgbd_set_error("conv_wgmma: tile does not fit the shared-memory pipeline"); return NRGBD_ERR_UNSUPPORTED; }
   p.stages_a = sa; p.stages_b = sb;
-  p.b_stage_bytes = (uint32_t)(2 * G * BN * RB);
+  p.b_stage_bytes = (uint32_t)(halves * G * BN * RB);
   const size_t smem = (size_t)sa * p.a_stage_bytes + (size_t)sb * p.b_stage_bytes + extra;
   CUtensorMap tb_hi, tb_lo;
   int rc = encode_w_map(&tb_hi, c.w_hi, esize, c.w_tap_stride, c.n_wslices, c.Cout_pad, c.Cin_pad, BN, G);
-  if (rc == NRGBD_OK) rc = encode_w_map(&tb_lo, c.w_lo, esize, c.w_tap_stride, c.n_wslices, c.Cout_pad, c.Cin_pad, BN, G);
+  if (rc == NRGBD_OK && !one) rc = encode_w_map(&tb_lo, c.w_lo, esize, c.w_tap_stride, c.n_wslices, c.Cout_pad, c.Cin_pad, BN, G);
   if (rc != NRGBD_OK) return rc;
   CUtensorMap ta_hi, ta_lo;
   rc = encode_act_map(&ta_hi, c.x_hi, esize, c.N, c.Din, c.Hin, c.Win, c.Cin_pad, c.Cs_in, p.box_w, p.box_h, p.in_stride);
-  if (rc == NRGBD_OK) rc = encode_act_map(&ta_lo, c.x_lo, esize, c.N, c.Din, c.Hin, c.Win, c.Cin_pad, c.Cs_in, p.box_w, p.box_h, p.in_stride);
+  if (rc == NRGBD_OK && !one) rc = encode_act_map(&ta_lo, c.x_lo, esize, c.N, c.Din, c.Hin, c.Win, c.Cin_pad, c.Cs_in, p.box_w, p.box_h, p.in_stride);
   if (rc != NRGBD_OK) return rc;
+  if (one) { tb_lo = tb_hi; ta_lo = ta_hi; }          // never read by the single-product kernel
   const bool aff = p.aff_scale != nullptr;
   if (aff && tf32) { nrgbd_set_error("conv_wgmma: the affine epilogue is built for split-fp16 operands only"); return NRGBD_ERR_UNSUPPORTED; }
-  WgKernel fn = aff ? (G == 3 ? pick_kernel<false, 3, true>(BN) : pick_kernel<false, 1, true>(BN))
-                    : tf32 ? (G == 3 ? pick_kernel<true, 3>(BN) : pick_kernel<true, 1>(BN))
-                           : (G == 3 ? pick_kernel<false, 3>(BN) : pick_kernel<false, 1>(BN));
+  WgKernel fn = one ? (aff ? (G == 3 ? pick_kernel<false, 3, true, true>(BN) : pick_kernel<false, 1, true, true>(BN))
+                           : (G == 3 ? pick_kernel<false, 3, false, true>(BN) : pick_kernel<false, 1, false, true>(BN)))
+             : aff ? (G == 3 ? pick_kernel<false, 3, true>(BN) : pick_kernel<false, 1, true>(BN))
+                   : tf32 ? (G == 3 ? pick_kernel<true, 3>(BN) : pick_kernel<true, 1>(BN))
+                          : (G == 3 ? pick_kernel<false, 3>(BN) : pick_kernel<false, 1>(BN));
   if (!fn) { nrgbd_set_error("conv_wgmma: unsupported chunk width %d", BN); return NRGBD_ERR_UNSUPPORTED; }
-  static size_t configured[2][2][2][8] = {};
-  size_t& conf = configured[aff][tf32][G == 3][BN / 16 - 1];
+  static size_t configured[2][2][2][2][8] = {};
+  size_t& conf = configured[one][aff][tf32][G == 3][BN / 16 - 1];
   if (smem > conf) {
     cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { nrgbd_set_error("conv_wgmma: cannot opt in to %zu bytes of shared memory: %s", smem, cudaGetErrorString(e)); return NRGBD_ERR_CUDA; }
@@ -521,6 +537,8 @@ int launch_chunks(const WgConv& c, WgParams p, int BN, int n_chunks, int c_first
 int conv_wgmma(const WgConv& c, cudaStream_t st) {
   NRGBD_REQUIRE(c.n_tap >= 1 && c.n_tap <= WG_MAX_TAP2D && c.n_kz >= 1 && c.n_kz <= 3 && c.Cin_pad % BKC == 0 && c.Cout_pad % 16 == 0,
                 "unsupported convolution shape");
+  NRGBD_REQUIRE(c.x_hi && (c.x_lo || !c.tf32), "the single-product form (x_lo == NULL) is built for fp16 operands only");
+  const int halves = c.x_lo ? 2 : 1;
   const int esize = c.tf32 ? 4 : 2, RB = BKC * esize;
   WgParams p{};
   p.y = c.y; p.bias = c.bias; p.stats = c.stats;
@@ -562,9 +580,9 @@ int conv_wgmma(const WgConv& c, cudaStream_t st) {
   p.b_desc_hi = (uint32_t)((8 * RB) >> 4) | (swz_mode << 30);
   p.wg_row16 = (uint32_t)((8 * (p.wide ? 1 : pitch) * RB) >> 4);   // 8 pixels right / 8 (halo) rows down
   p.box_w = pitch; p.box_h = halo_rows;
-  p.a_tx_bytes = 2u * (uint32_t)(halo_rows * pitch * RB);
+  p.a_tx_bytes = (uint32_t)halves * (uint32_t)(halo_rows * pitch * RB);
   p.a_tile_bytes = round_up((uint32_t)(halo_rows * pitch * RB), 1024);
-  p.a_stage_bytes = 2 * p.a_tile_bytes;
+  p.a_stage_bytes = (uint32_t)halves * p.a_tile_bytes;
   // Cout in chunks of 128 channels, the last one narrower (320 = 128 + 128 + 64): one launch per chunk width
   const int n_chunks = (c.Cout_pad + 127) / 128;
   const int BN = c.Cout_pad < 128 ? c.Cout_pad : 128;
@@ -579,7 +597,7 @@ namespace {
 // ---- operand preparation -------------------------------------------------------------------------------------------
 __device__ __forceinline__ void split_pair(float a, __half& hi, __half& lo) { nrgbd_split_pair(a, hi, lo); }
 
-// fp32 [n] -> hi / lo halves [n]
+// fp32 [n] -> hi / lo halves [n] (lo == NULL: hi only, the plain fp16 conversion)
 __global__ void __launch_bounds__(256)
 split_f16_pair_kernel(const float4* __restrict__ x, long long n4, uint2* __restrict__ hi, uint2* __restrict__ lo) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
@@ -591,7 +609,8 @@ split_f16_pair_kernel(const float4* __restrict__ x, long long n4, uint2* __restr
     ho.y = (uint32_t)__half_as_ushort(h[2]) | ((uint32_t)__half_as_ushort(h[3]) << 16);
     lo2.x = (uint32_t)__half_as_ushort(l[0]) | ((uint32_t)__half_as_ushort(l[1]) << 16);
     lo2.y = (uint32_t)__half_as_ushort(l[2]) | ((uint32_t)__half_as_ushort(l[3]) << 16);
-    hi[i] = ho; lo[i] = lo2;
+    hi[i] = ho;
+    if (lo) lo[i] = lo2;
   }
 }
 
@@ -631,8 +650,9 @@ int nrgbd_conv_h2_plan(int Cin, int Cout, int* Cin_pad, int* Cout_pad, int* BN) 
   return 1;
 }
 
+// lo == NULL: only hi = RN_f16(x) (saturating) is written - a plain fp32 -> fp16 conversion
 int nrgbd_split_f16_pair(const float* x, long long n, void* hi, void* lo, cudaStream_t st) {
-  NRGBD_REQUIRE(x && hi && lo && n > 0 && n % 4 == 0, "bad arguments");
+  NRGBD_REQUIRE(x && hi && n > 0 && n % 4 == 0, "bad arguments");
   long long blocks = (n / 4 + 255) / 256;
   if (blocks > nrgbd_sm_count() * 16ll) blocks = nrgbd_sm_count() * 16ll;
   split_f16_pair_kernel<<<(unsigned)blocks, 256, 0, st>>>(reinterpret_cast<const float4*>(x), n / 4, reinterpret_cast<uint2*>(hi),
@@ -672,7 +692,7 @@ int nrgbd_conv_nhwc_h2(const void* x_hi, const void* x_lo, int N, int Din, int H
 int nrgbd_conv_nhwc_h2_pair(const void* x_hi, const void* x_lo, int N, int Din, int Hin, int Win, int Cin_pad, int Cs_in, const void* w,
                             const float* bias, int Cout, int Cout_pad, int BN, int kd, int kh, int kw, int stride, int pad, int dilation,
                             void* y_hi, void* y_lo, int Hout, int Wout, int Cs_out, int leaky, cudaStream_t st) {
-  NRGBD_REQUIRE(y_hi && y_lo, "null pointer");
+  NRGBD_REQUIRE(y_hi, "null pointer");
   return conv_nhwc_h2_impl(x_hi, x_lo, N, Din, Hin, Win, Cin_pad, Cs_in, w, bias, Cout, Cout_pad, BN, kd, kh, kw, stride, pad, dilation, nullptr, y_hi,
                            y_lo, Hout, Wout, Cs_out, 0, leaky, nullptr, st);
 }
@@ -681,7 +701,7 @@ static int conv_nhwc_h2_impl(const void* x_hi, const void* x_lo, int N, int Din,
                              const float* bias, int Cout, int Cout_pad, int BN, int kd, int kh, int kw, int stride, int pad, int dilation, float* y,
                              void* y_hi, void* y_lo, int Hout, int Wout, int Cs_out, int c_off, int leaky, double* stats, cudaStream_t st,
                              const WgConv* aff) {
-  NRGBD_REQUIRE(x_hi && x_lo && w, "null pointer");
+  NRGBD_REQUIRE(x_hi && w, "null pointer");
   NRGBD_REQUIRE(Cin_pad % 32 == 0 && Cin_pad >= 32 && Cin_pad <= Cs_in && Cs_in % 8 == 0 && Cout_pad % 16 == 0 && Cout <= Cout_pad && Cout > Cout_pad - 16 &&
                     BN == (Cout_pad < 128 ? Cout_pad : 128), "channel counts not supported by the f16-pair tensor-core path");
   NRGBD_REQUIRE(kd >= 1 && kd <= 3 && kh * kw <= WG_MAX_TAP2D && stride >= 1 && stride <= 8, "unsupported filter");
@@ -689,7 +709,7 @@ static int conv_nhwc_h2_impl(const void* x_hi, const void* x_lo, int N, int Din,
                     Wout == (Win + 2 * pad - dilation * (kw - 1) - 1) / stride + 1, "output extent mismatch");
   if (y_hi) {
     // the output as the operand pair of the next convolution: every Cs_out channel stored, pad channels as zeros
-    NRGBD_REQUIRE(Cs_out % 32 == 0 && Cs_out >= Cout_pad && c_off == 0 && stats == nullptr && (((uintptr_t)y_hi | (uintptr_t)y_lo) & 15) == 0 && y_lo,
+    NRGBD_REQUIRE(Cs_out % 32 == 0 && Cs_out >= Cout_pad && c_off == 0 && stats == nullptr && (((uintptr_t)y_hi | (uintptr_t)y_lo) & 15) == 0,
                   "pair output needs Cs_out % 32 == 0, c_off == 0 and no statistics");
   }
   WgConv c{};
@@ -722,7 +742,7 @@ int nrgbd_conv_nhwc_h2_affine(const void* x_hi, const void* x_lo, int N, int Din
                               const float* scale, const float* shift, const float* res, const void* res_hi, const void* res_lo, int relu,
                               float* y, void* y_hi, void* y_lo, int Hout, int Wout, int Cs_out, int c_off, cudaStream_t st) {
   NRGBD_REQUIRE(scale && shift, "null scale / shift");
-  NRGBD_REQUIRE((y != nullptr) != (y_hi != nullptr) && (y_hi == nullptr) == (y_lo == nullptr), "the output is either fp32 (y) or a pair (y_hi, y_lo)");
+  NRGBD_REQUIRE((y != nullptr) != (y_hi != nullptr) && !(y_lo && !y_hi), "the output is either fp32 (y) or a pair (y_hi, y_lo or NULL)");
   NRGBD_REQUIRE((res_hi == nullptr) == (res_lo == nullptr) && !(res && res_hi), "the residual is either an fp32 tensor or an operand pair");
   WgConv aff{};
   aff.aff_scale = scale; aff.aff_shift = shift; aff.res = res; aff.res_hi = res_hi; aff.res_lo = res_lo; aff.relu = relu ? 1 : 0;
@@ -734,7 +754,7 @@ int nrgbd_conv_nhwc_h2_affine(const void* x_hi, const void* x_lo, int N, int Din
 int nrgbd_conv_transpose2d_k4s2_nhwc_h2(const void* x_hi, const void* x_lo, int N, int Hin, int Win, int Cin_pad, int Cs_in, const void* w,
                                         const float* bias, int Cout, int Cout_pad, int BN, float* y, int Cs_out, int c_off, int leaky,
                                         cudaStream_t st) {
-  NRGBD_REQUIRE(x_hi && x_lo && w && y, "null pointer");
+  NRGBD_REQUIRE(x_hi && w && y, "null pointer");
   NRGBD_REQUIRE(Cin_pad % 32 == 0 && Cin_pad >= 32 && Cin_pad <= Cs_in && Cs_in % 8 == 0 && Cout_pad % 16 == 0 && Cout <= Cout_pad && Cout > Cout_pad - 16 &&
                     BN == (Cout_pad < 128 ? Cout_pad : 128), "channel counts not supported by the f16-pair tensor-core path");
   const int kys[2][2] = {{1, 3}, {0, 2}};

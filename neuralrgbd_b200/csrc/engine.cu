@@ -56,7 +56,7 @@ struct ParamRef { float* p; long long n; bool owned; };
 struct Packed { float* w; int Cin, Cin_pad, Cout, Cout_pad, taps; };
 struct PackedTc { float* hi; float* lo; int Cin_pad, Cout_pad, taps; };
 struct PackedH2 { void* w; int Cin_pad, Cout_pad, BN, taps; };       // f16-pair tiles [taps][2][Cout_pad][Cin_pad] halves
-struct PairBuf { float* hi; float* lo; };                          // split-fp16 planes of an activation (pool blocks)
+struct PairBuf { float* hi; float* lo; };                          // split-fp16 planes of an activation (pool blocks); lo null: fp16 only
 
 struct Camera {
   bool set = false;
@@ -84,8 +84,12 @@ struct nrgbd_kvnet {
   std::unordered_map<std::string, Packed> packed;
   std::unordered_map<std::string, PackedTc> packed_tc;
   std::unordered_map<std::string, PackedH2> packed_h2;
-  std::unordered_map<const float*, PairBuf> pairs;   // activations that currently have a split-fp16 copy (conv_math 2)
-  int conv_math = 0;                // 0: exact fp32 FFMA implicit GEMM; 1: wgmma 3xTF32; 2: wgmma split-fp16 pairs (conv_f16.cu)
+  // activations that currently have a split-fp16 copy (conv_math 2 and 3). In conv_math 3 only the tensors read as residuals
+  // keep a lo half; the rest are plain fp16 (lo null), since a convolution reads hi only.
+  std::unordered_map<const float*, PairBuf> pairs;
+  // 0: exact fp32 FFMA implicit GEMM; 1: wgmma 3xTF32; 2: wgmma split-fp16 pairs (conv_f16.cu); 3: single fp16 products on the
+  // same paths as 2 (convolutions launched with x_lo = NULL)
+  int conv_math = 0;
   int refine = 0;                   // refinement of KVNET(...): 0 the DPV R-Net, 1 the guided filter ('DGF'), 2 none (if_refined=False)
   int refine_up = 0;                // DPV R-Net with if_upsample_d: widths D0 = 2D, D1 = 4D (Refine.py:44-48)
   bool packed_dirty = true;
@@ -178,9 +182,17 @@ void release(Eng* e, Act& a) {
   a.p = nullptr;
 }
 
+// conv_math 2 and 3 take the f16-pair paths; 3 differs only in what the pairs hold and how convolutions are launched
+inline bool pair_mode(const Eng* e) { return e->conv_math == 2 || e->conv_math == 3; }
+// Whether a pair written now needs its lo half: always in conv_math 2; in conv_math 3 only when a residual add reads it
+// (a residual keeps its 22-bit value; convolutions read hi only)
+inline bool keep_lo(const Eng* e, bool res_read) { return e->conv_math == 2 || res_read; }
+// x_lo of a convolution launch: NULL runs the single-product kernel (conv_math 3) even when the pair has a lo for a residual
+inline const void* conv_lo(const Eng* e, const PairBuf* pb) { return e->conv_math == 3 ? nullptr : pb->lo; }
+
 // Split-fp16 operand planes of an activation (x = hi + lo * 2^-11), created on first use by a convolution and kept
 // until the activation is released: several convolutions may consume the same tensor (BasicBlock input: conv1 +
-// downsample). Activations are never written again after their first conv consumer has run.
+// downsample). Activations are never written again after their first conv consumer has run. conv_math 3: hi only.
 const PairBuf* pair_of(Eng* e, const Act& x) {
   auto it = e->pairs.find(x.p);
   if (it != e->pairs.end()) return &it->second;
@@ -188,8 +200,8 @@ const PairBuf* pair_of(Eng* e, const Act& x) {
   PairBuf pb;
   const size_t bytes = (size_t)x.floats() * 2;
   pb.hi = e->pool.acquire(bytes);
-  pb.lo = e->pool.acquire(bytes);
-  if (!pb.hi || !pb.lo) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; return nullptr; }
+  pb.lo = keep_lo(e, false) ? e->pool.acquire(bytes) : nullptr;
+  if (!pb.hi || (!pb.lo && keep_lo(e, false))) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; return nullptr; }
   ENG_CALL(e, nrgbd_split_f16_pair(x.p, x.floats(), pb.hi, pb.lo, (nrgbd_stream_t)e->st));
   e->pairs[x.p] = pb;
   return &e->pairs[x.p];
@@ -296,7 +308,7 @@ const PackedH2* packw_h2_taps(Eng* e, const std::string& name, int Cin, int taps
 // zeros there) and the packed weight's rows [C, Cin_pad) are zero, so the padding adds exact zeros to every sum. This
 // is also the one condition under which an activation may exist only as its operand pair (the K-Net input volume).
 bool use_h2(Eng* e, const Act& x) {
-  return e->conv_math == 2 && pad32(x.C) <= x.Cs && x.Cs % 8 == 0;
+  return pair_mode(e) && pad32(x.C) <= x.Cs && x.Cs % 8 == 0;
 }
 
 bool use_tc(Eng* e, const Act& x, int Cout) {
@@ -336,21 +348,21 @@ Act conv(Eng* e, const Act& x, const std::string& wname, int Cout, int kd, int k
     PairBuf pb;
     y.p = e->pool.acquire(16);                                    // key of the pair buffers
     pb.hi = e->pool.acquire((size_t)y.floats() * 2);
-    pb.lo = e->pool.acquire((size_t)y.floats() * 2);
-    if (!y.p || !pb.hi || !pb.lo) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; return y; }
+    pb.lo = keep_lo(e, false) ? e->pool.acquire((size_t)y.floats() * 2) : nullptr;   // R-Net: no residuals
+    if (!y.p || !pb.hi || (!pb.lo && keep_lo(e, false))) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; return y; }
     e->pairs[y.p] = pb;
     const double flops = 2.0 * (double)x.N * x.D * Ho * Wo * Cout * x.C * kd * k * k;
     char tag[56];
     snprintf(tag, sizeof(tag), "conv%dd k%d s%d d%d %d->%d %dx%dx%dx%d", kd > 1 ? 3 : 2, k, stride, dil, x.C, Cout, x.N, x.D, Ho, Wo);
     ProfScope ps(e, 0, flops, tag);
-    ENG_CALL(e, nrgbd_conv_nhwc_h2_pair(pin->hi, pin->lo, x.N, x.D, x.H, x.W, ph->Cin_pad, x.Cs, ph->w, b, Cout, ph->Cout_pad, ph->BN, kd, k, k,
+    ENG_CALL(e, nrgbd_conv_nhwc_h2_pair(pin->hi, conv_lo(e, pin), x.N, x.D, x.H, x.W, ph->Cin_pad, x.Cs, ph->w, b, Cout, ph->Cout_pad, ph->BN, kd, k, k,
                                         stride, pad, dil, pb.hi, pb.lo, Ho, Wo, y.Cs, leaky ? 1 : 0, (nrgbd_stream_t)e->st));
     return y;
   }
   if (dst) y = *dst; else y = acquire(e, x.N, x.D, Ho, Wo, Cout, out_Cs);
   float* b = bias_name ? param(e, bias_name) : nullptr;
   if (e->rc) return y;
-  if (want_stats && e->conv_math != 2) cudaMemsetAsync(stats_buf, 0, sizeof(double) * 2 * Cout, e->st);   // f16-pair mode: kept zero by the BN pass
+  if (want_stats && !pair_mode(e)) cudaMemsetAsync(stats_buf, 0, sizeof(double) * 2 * Cout, e->st);   // f16-pair mode: kept zero by the BN pass
   const double flops = 2.0 * (double)x.N * x.D * Ho * Wo * Cout * x.C * kd * k * k;
   char tag[56];
   snprintf(tag, sizeof(tag), "conv%dd k%d s%d d%d %d->%d %dx%dx%dx%d", kd > 1 ? 3 : 2, k, stride, dil, x.C, Cout, x.N, x.D, Ho, Wo);
@@ -359,7 +371,7 @@ Act conv(Eng* e, const Act& x, const std::string& wname, int Cout, int kd, int k
     const PairBuf* pb = pair_of(e, x);
     if (e->rc) return y;
     ProfScope ps(e, 0, flops, tag);
-    ENG_CALL(e, nrgbd_conv_nhwc_h2(pb->hi, pb->lo, x.N, x.D, x.H, x.W, ph->Cin_pad, x.Cs, ph->w, b, Cout, ph->Cout_pad, ph->BN, kd, k, k, stride,
+    ENG_CALL(e, nrgbd_conv_nhwc_h2(pb->hi, conv_lo(e, pb), x.N, x.D, x.H, x.W, ph->Cin_pad, x.Cs, ph->w, b, Cout, ph->Cout_pad, ph->BN, kd, k, k, stride,
                                    pad, dil, y.p, Ho, Wo, y.Cs, c_off, leaky ? 1 : 0, want_stats ? stats_buf : nullptr, (nrgbd_stream_t)e->st));
     return y;
   }
@@ -440,9 +452,9 @@ const float* eval_coef(Eng* e, const std::string& pre) {
 // Eval-mode Conv (no bias) + BatchNorm(running statistics) [+ residual] [+ ReLU] of a tracked layer. f16-pair mode: ONE
 // convolution with the affine epilogue, written as the operand pair of the next convolution when only convolutions read it
 // (out_use 2), else as fp32. Other modes: the convolution without statistics, then nrgbd_bn_apply. No statistic is read or
-// written, no running buffer updated.
+// written, no running buffer updated. res_read: a later residual add reads the pair (see convbn).
 Act convbn_eval(Eng* e, const Act& x, const std::string& wname, int Cout, int kd, int k, int stride, int pad, int dil, bool relu,
-                const Act* res, int out_use, const float* scale) {
+                const Act* res, int out_use, const float* scale, bool res_read = false) {
   const float* shift = scale + 512;
   if (use_h2(e, x)) {
     const int Ho = (x.H + 2 * pad - dil * (k - 1) - 1) / stride + 1, Wo = (x.W + 2 * pad - dil * (k - 1) - 1) / stride + 1;
@@ -455,8 +467,8 @@ Act convbn_eval(Eng* e, const Act& x, const std::string& wname, int Cout, int kd
       y.N = x.N; y.D = x.D; y.H = Ho; y.W = Wo; y.C = Cout; y.Cs = pad32(Cout); y.pair_only = true;
       y.p = e->pool.acquire(16);                                    // key of the pair buffers
       pb.hi = e->pool.acquire((size_t)y.floats() * 2);
-      pb.lo = e->pool.acquire((size_t)y.floats() * 2);
-      if (!y.p || !pb.hi || !pb.lo) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; return y; }
+      pb.lo = keep_lo(e, res_read) ? e->pool.acquire((size_t)y.floats() * 2) : nullptr;
+      if (!y.p || !pb.hi || (!pb.lo && keep_lo(e, res_read))) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; return y; }
       e->pairs[y.p] = pb;
     } else {
       y = acquire(e, x.N, x.D, Ho, Wo, Cout);
@@ -468,7 +480,7 @@ Act convbn_eval(Eng* e, const Act& x, const std::string& wname, int Cout, int kd
       if (res->Cs != y.Cs || res->pos() != y.pos()) { nrgbd_set_error("engine: residual layout differs from the output's"); e->rc = NRGBD_ERR_BAD_ARG; return y; }
       if (res->pair_only) {
         auto it = e->pairs.find(res->p);
-        if (it == e->pairs.end()) { nrgbd_set_error("engine: residual has neither an fp32 copy nor an operand pair"); e->rc = NRGBD_ERR_BAD_ARG; return y; }
+        if (it == e->pairs.end() || !it->second.lo) { nrgbd_set_error("engine: residual has neither an fp32 copy nor a full operand pair"); e->rc = NRGBD_ERR_BAD_ARG; return y; }
         res_hi = it->second.hi; res_lo = it->second.lo;
       } else {
         res_f = res->p;
@@ -477,7 +489,7 @@ Act convbn_eval(Eng* e, const Act& x, const std::string& wname, int Cout, int kd
     char tag[56];
     snprintf(tag, sizeof(tag), "conv%dd k%d s%d d%d %d->%d %dx%dx%dx%d", kd > 1 ? 3 : 2, k, stride, dil, x.C, Cout, x.N, x.D, Ho, Wo);
     ProfScope ps(e, 0, 2.0 * (double)x.N * x.D * Ho * Wo * Cout * x.C * kd * k * k, tag);
-    ENG_CALL(e, nrgbd_conv_nhwc_h2_affine(pin->hi, pin->lo, x.N, x.D, x.H, x.W, ph->Cin_pad, x.Cs, ph->w, Cout, ph->Cout_pad, ph->BN, kd, k, k,
+    ENG_CALL(e, nrgbd_conv_nhwc_h2_affine(pin->hi, conv_lo(e, pin), x.N, x.D, x.H, x.W, ph->Cin_pad, x.Cs, ph->w, Cout, ph->Cout_pad, ph->BN, kd, k, k,
                                           stride, pad, dil, scale, shift, res_f, res_hi, res_lo, relu ? 1 : 0, out_use == 2 ? nullptr : y.p,
                                           pb.hi, pb.lo, Ho, Wo, y.Cs, 0, (nrgbd_stream_t)e->st));
     return y;
@@ -494,30 +506,33 @@ Act convbn_eval(Eng* e, const Act& x, const std::string& wname, int Cout, int kd
 // out_use (f16-pair mode only): 0 = the result is read as fp32 only; 1 = also by a convolution (the BatchNorm pass emits the
 // split-fp16 operand planes together with the fp32 tensor); 2 = ONLY by a convolution (no fp32 copy is written: y.p keeps
 // the raw conv output and must not be read as an activation). A residual `res` that itself exists only as a pair (out_use 2
-// of an earlier layer) is read from that pair.
+// of an earlier layer) is read from that pair. res_read (out_use 2): a later residual add reads the result, so its pair keeps
+// the lo half in conv_math 3 too (elsewhere conv_math 3 writes hi only).
 Act convbn(Eng* e, const Act& x, const std::string& pre, int Cout, int kd, int k, int stride, int pad, int dil,
-           bool relu, const Act* res, int out_use = 0) {
+           bool relu, const Act* res, int out_use = 0, bool res_read = false) {
   int p = (kd == 1 && dil > 1) ? dil : pad;          // psm_submodule.convbn :13
-  if (const float* sc = eval_coef(e, pre + ".1")) return convbn_eval(e, x, pre + ".0.weight", Cout, kd, k, stride, p, dil, relu, res, out_use, sc);
+  if (const float* sc = eval_coef(e, pre + ".1"))
+    return convbn_eval(e, x, pre + ".0.weight", Cout, kd, k, stride, p, dil, relu, res, out_use, sc, res_read);
   Act y = conv(e, x, pre + ".0.weight", Cout, kd, k, stride, p, dil, nullptr, false, true);
   float* g = param(e, pre + ".1.weight");
   float* b = param(e, pre + ".1.bias");
   float* rm = e->bn_update_running ? param_opt(e, pre + ".1.running_mean") : nullptr;
   float* rv = e->bn_update_running ? param_opt(e, pre + ".1.running_var") : nullptr;
   if (e->rc) return y;
-  if (e->conv_math == 2) {
+  if (pair_mode(e)) {
     const bool pair = out_use && use_h2(e, y);
+    const bool lo = keep_lo(e, res_read && out_use == 2);   // out_use 1: a residual add reads the fp32 copy
     PairBuf pb; pb.hi = pb.lo = nullptr;
     if (pair) {
       pb.hi = e->pool.acquire((size_t)y.floats() * 2);
-      pb.lo = e->pool.acquire((size_t)y.floats() * 2);
-      if (!pb.hi || !pb.lo) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; return y; }
+      pb.lo = lo ? e->pool.acquire((size_t)y.floats() * 2) : nullptr;
+      if (!pb.hi || (!pb.lo && lo)) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; return y; }
     }
     const float* res_f = res ? res->p : nullptr;
     const void *res_hi = nullptr, *res_lo = nullptr;
     if (res && res->pair_only) {
       auto it = e->pairs.find(res->p);
-      if (it == e->pairs.end()) { nrgbd_set_error("engine: residual has neither an fp32 copy nor an operand pair"); e->rc = NRGBD_ERR_BAD_ARG; return y; }
+      if (it == e->pairs.end() || !it->second.lo) { nrgbd_set_error("engine: residual has neither an fp32 copy nor a full operand pair"); e->rc = NRGBD_ERR_BAD_ARG; return y; }
       res_f = nullptr; res_hi = it->second.hi; res_lo = it->second.lo;
     }
     ENG_CALL(e, nrgbd_bn_apply_stats_pair(y.p, e->stats, (double)y.pos(), g, b, 1e-5f, rm && rv ? rm : nullptr, rm && rv ? rv : nullptr,
@@ -561,7 +576,7 @@ Act basic_block(Eng* e, Act& x, const std::string& pre, int planes, int stride, 
     float* rm = e->bn_update_running ? param_opt(e, pre + ".downsample.1.running_mean") : nullptr;
     float* rv = e->bn_update_running ? param_opt(e, pre + ".downsample.1.running_var") : nullptr;
     if (!e->rc) {
-      if (e->conv_math == 2)
+      if (pair_mode(e))
         ENG_CALL(e, nrgbd_bn_apply_stats_pair(sc.p, e->stats, (double)sc.pos(), g, b, 1e-5f, rm && rv ? rm : nullptr, rm && rv ? rv : nullptr,
                                               0.1f, nullptr, nullptr, nullptr, 0, sc.pos(), sc.Cs, sc.C, sc.p, nullptr, nullptr, e->bn_counter,
                                               (nrgbd_stream_t)e->st));
@@ -588,7 +603,8 @@ Act basic_block(Eng* e, Act& x, const std::string& pre, int planes, int stride, 
                                        0.1f, res->p, 0, o.pos(), o.Cs, o.C, o.p, (nrgbd_stream_t)e->st));
     }
   } else {
-    o = convbn(e, t, pre + ".conv2", planes, 1, 3, 1, 1, dil, false, res, fp32_out ? 1 : 2);
+    // a block output that exists only as a pair is the residual of the next block (layer1-3 inner blocks, layer3 -> layer4.0)
+    o = convbn(e, t, pre + ".conv2", planes, 1, 3, 1, 1, dil, false, res, fp32_out ? 1 : 2, true);
   }
   release(e, t);
   if (down) release(e, sc);
@@ -641,7 +657,7 @@ void feature_cnn(Eng* e, const Act& x0, Act& l1_out, Act& feat_out) {
   } else {
     Act a = convbn(e, x0, P + ".firstconv.0", 32, 1, 3, 2, 1, 1, true, nullptr, 2);
     Act b = convbn(e, a, P + ".firstconv.2", 32, 1, 3, 1, 1, 1, true, nullptr, 2); release(e, a);
-    c = convbn(e, b, P + ".firstconv.4", 32, 1, 3, 1, 1, 1, true, nullptr, 2); release(e, b);     // layer1.0 reads it as conv input and as residual: pair only
+    c = convbn(e, b, P + ".firstconv.4", 32, 1, 3, 1, 1, 1, true, nullptr, 2, true); release(e, b);     // layer1.0 reads it as conv input and as residual: pair only
   }
   Act l1 = make_layer(e, c, true, P + ".layer1", 32, 3, 1, 1, false);
   Act raw = make_layer(e, l1, false, P + ".layer2", 64, 16, 2, 1, true);
@@ -703,7 +719,7 @@ void conv_transpose(Eng* e, const Act& x, const std::string& wname, const char* 
     const PairBuf* pb = pair_of(e, x);
     if (e->rc) return;
     ProfScope ps(e, 0, flops, tag);
-    ENG_CALL(e, nrgbd_conv_transpose2d_k4s2_nhwc_h2(pb->hi, pb->lo, x.N, x.H, x.W, ph->Cin_pad, x.Cs, ph->w, tb, Cout, ph->Cout_pad, ph->BN,
+    ENG_CALL(e, nrgbd_conv_transpose2d_k4s2_nhwc_h2(pb->hi, conv_lo(e, pb), x.N, x.H, x.W, ph->Cin_pad, x.Cs, ph->w, tb, Cout, ph->Cout_pad, ph->BN,
                                                     dst.p, dst.Cs, 0, 1, st));
     return;
   }
@@ -788,20 +804,20 @@ void dgf_refine(Eng* e, const float* bv_hwd, const Act& frame_ref, float* out) {
 // models/basic.py:113-139 on a channels-last volume [D][h][w][CK] -> gain [D][hw] (DHW, Cs = 1)
 Act kv_net(Eng* e, const Act& vol) {
   const int f = e->KF;
-  auto cb = [&](const Act& x, const std::string& name, bool relu, const Act* res, int out_use) {
-    return convbn(e, x, name, f, 3, 3, 1, 1, 1, relu, res, out_use);
+  auto cb = [&](const Act& x, const std::string& name, bool relu, const Act* res, int out_use, bool res_read) {
+    return convbn(e, x, name, f, 3, 3, 1, 1, 1, relu, res, out_use, res_read);
   };
-  Act a = cb(vol, "kv_net.dres0.0", true, nullptr, 2);
+  Act a = cb(vol, "kv_net.dres0.0", true, nullptr, 2, false);
   // in f16-pair mode no K-Net activation has an fp32 copy: convolutions read the operand pairs, and so do the residual adds
-  Act c = cb(a, "kv_net.dres0.2", true, nullptr, 2); release(e, a);      // also the residual of dres1
+  Act c = cb(a, "kv_net.dres0.2", true, nullptr, 2, true); release(e, a);      // also the residual of dres1
   for (int i = 1; i <= 4; ++i) {
     std::string p = "kv_net.dres" + std::to_string(i);
-    Act r = cb(c, p + ".0", true, nullptr, 2);
-    Act o = cb(r, p + ".2", false, &c, 2);
+    Act r = cb(c, p + ".0", true, nullptr, 2, false);
+    Act o = cb(r, p + ".2", false, &c, 2, i < 4);                              // the residual of dres(i + 1)
     release(e, r); release(e, c);
     c = o;
   }
-  Act o = cb(c, "kv_net.classify.0", true, nullptr, 2); release(e, c);
+  Act o = cb(c, "kv_net.classify.0", true, nullptr, 2, false); release(e, c);
   Act gain;
   if (use_h2(e, o)) {
     // Conv3d(f -> 1, k3) (models/basic.py:136-137) as a pointwise conv to 27 per-tap channels on the tensor cores + the shifted
@@ -818,7 +834,7 @@ Act kv_net(Eng* e, const Act& vol) {
       char tag[56];
       snprintf(tag, sizeof(tag), "conv3d k3 s1 d1 %d->1 %dx%dx%dx%d", o.C, o.N, o.D, o.H, o.W);
       ProfScope ps(e, 0, 2.0 * (double)o.pos() * o.C * 27, tag);
-      ENG_CALL(e, nrgbd_conv_nhwc_h2(pb->hi, pb->lo, o.N, o.D, o.H, o.W, ph->Cin_pad, o.Cs, ph->w, nullptr, 27, ph->Cout_pad, ph->BN, 1, 1, 1, 1,
+      ENG_CALL(e, nrgbd_conv_nhwc_h2(pb->hi, conv_lo(e, pb), o.N, o.D, o.H, o.W, ph->Cin_pad, o.Cs, ph->w, nullptr, 27, ph->Cout_pad, ph->BN, 1, 1, 1, 1,
                                      0, 1, q.p, o.H, o.W, q.Cs, 0, 0, nullptr, (nrgbd_stream_t)e->st));
       ENG_CALL(e, nrgbd_tap_gather_sum(q.p, o.N, o.D, o.H, o.W, q.Cs, 3, 3, 0.f, gain.p, (nrgbd_stream_t)e->st));
     }
@@ -983,8 +999,8 @@ int nrgbd_kvnet_set_option(nrgbd_kvnet* e, const char* key, int value) {
     e->refine_up = value ? 1 : 0;
     return NRGBD_OK;
   }
-  if (k == "conv_math") {            // 0: exact fp32 (CUDA cores); 1: wgmma 3xTF32; 2: wgmma split-fp16 pairs
-    if (value < 0 || value > 2) { nrgbd_set_error("conv_math must be 0 (fp32), 1 (tf32x3) or 2 (f16x3)"); return NRGBD_ERR_BAD_ARG; }
+  if (k == "conv_math") {            // 0: exact fp32 (CUDA cores); 1: wgmma 3xTF32; 2: wgmma split-fp16 pairs; 3: single fp16 products
+    if (value < 0 || value > 3) { nrgbd_set_error("conv_math must be 0 (fp32), 1 (tf32x3), 2 (f16x3) or 3 (f16)"); return NRGBD_ERR_BAD_ARG; }
     drop_graphs(e); e->conv_math = value;
     // f16-pair mode keeps the statistics buffers zero between uses (the BatchNorm pass re-zeroes what it consumed)
     cudaMemset(e->stats, 0, sizeof(double) * 2 * 512); cudaMemset(e->stats_b, 0, sizeof(double) * 2 * 512); cudaMemset(e->bn_counter, 0, sizeof(unsigned int));
@@ -1229,8 +1245,8 @@ static int forward_core(nrgbd_kvnet* e, bool steady, bool need_cur_refined, bool
       vol.p = e->pool.acquire(16);
       PairBuf pb;
       pb.hi = e->pool.acquire((size_t)vol.floats() * 2);
-      pb.lo = e->pool.acquire((size_t)vol.floats() * 2);
-      if (!vol.p || !pb.hi || !pb.lo) { if (!e->rc) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; } }
+      pb.lo = keep_lo(e, false) ? e->pool.acquire((size_t)vol.floats() * 2) : nullptr;
+      if (!vol.p || !pb.hi || (!pb.lo && keep_lo(e, false))) { if (!e->rc) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; } }
       else {
         ENG_CALL(e, nrgbd_knet_input_volume_pair(rgbq.p, rgbq.p + (size_t)V * hw * 4, e->bv_cur_hwd, e->prior_hwd, V, D, h, w, vol.Cs,
                                                  c1.K, Rs, ts, c1.rays, e->d_planes, c1.cx, c1.cy, e->ws_sweep, nullptr, pb.hi, pb.lo, st));

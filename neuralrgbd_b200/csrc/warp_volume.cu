@@ -129,7 +129,8 @@ knet_volume_rows_kernel(const float4* __restrict__ imgs, const float* __restrict
     for (int g = 0; g < CK4; ++g) {
       uint2 hq, lq;
       nrgbd_split_pair4(row + 4 * g, hq, lq);
-      out_hi[vox * CK4 + g] = hq; out_lo[vox * CK4 + g] = lq;
+      out_hi[vox * CK4 + g] = hq;
+      if (out_lo) out_lo[vox * CK4 + g] = lq;
     }
   }
 }
@@ -235,14 +236,15 @@ int nrgbd_knet_input_volume(const float* src_rgb_packed, const float* ref_rgb_pa
 }
 
 // Same volume, optionally (also / only) as the split-fp16 operand pair (out_hi, out_lo: half [D][hw][CK]) of the f16-pair
-// convolution that consumes it; out may be NULL when the pair is requested.
+// convolution that consumes it; out may be NULL when the pair is requested. out_hi set and out_lo NULL: hi only (the
+// operand of the single-product convolution).
 int nrgbd_knet_input_volume_pair(const float* src_rgb_packed, const float* ref_rgb_packed, const float* bv_cur_hwd,
                                  const float* bv_pred_hwd, int V, int D, int h, int w, int CK, const float* K,
                                  const float* R, const float* t, const float* rays, const float* d_planes, float cx,
                                  float cy, float* ws, float* out, void* out_hi, void* out_lo, cudaStream_t st) {
   NRGBD_REQUIRE(src_rgb_packed && ref_rgb_packed && bv_cur_hwd && bv_pred_hwd && K && R && t && rays &&
-                    d_planes && ws && (out || (out_hi && out_lo)), "null pointer");
-  NRGBD_REQUIRE(V > 0 && D > 0 && h > 0 && w > 0 && CK >= 3 * V + 4 && (out_hi == nullptr) == (out_lo == nullptr), "bad shape");
+                    d_planes && ws && (out || out_hi), "null pointer");
+  NRGBD_REQUIRE(V > 0 && D > 0 && h > 0 && w > 0 && CK >= 3 * V + 4 && !(out_lo && !out_hi), "bad shape");
   float* t1 = ws; float* KR = ws + 3 * V;
   warp_setup_kernel<<<ceil_div(V, 32), 32, 0, st>>>(K, R, t, V, t1, KR);
   long long n = (long long)h * w * D;

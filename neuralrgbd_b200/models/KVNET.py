@@ -99,7 +99,9 @@ class KVNET(nn.Module):
         self.cam_intrinsics = cam_intrinsics          # captured at construction: used by D-Net (KVNET.py:64-67)
         self.feat_dist = 'L2'                         # basic.py:146 default, never overridden by KVNET
         # convolution arithmetic: 'f16x3' (default; wgmma on split-fp16 operand pairs, 22-bit products, fp32 accumulate -
-        # the fastest AND the closest to the reference of the tensor paths), 'tf32x3' (wgmma 3xTF32), 'fp32' (exact CUDA-core FFMA)
+        # the fastest AND the closest to the reference of the tensor paths), 'tf32x3' (wgmma 3xTF32), 'fp32' (exact CUDA-core FFMA),
+        # 'f16' (opt-in throughput mode: one fp16 product per MAC, fp32 accumulate - the operand precision of a TF32 GPU run,
+        # not the 1e-4 envelope of the other modes; INTEGRATION.md)
         self.conv_math = 'f16x3'
 
         D = len(d_candi)
@@ -249,9 +251,9 @@ class KVNET(nn.Module):
             ent = self._engine(H, W, V, dev)
             self._sync_params(ent, dev)
             if ent['conv_math'] != self.conv_math:
-                modes = {'fp32': 0, 'tf32x3': 1, 'f16x3': 2}
+                modes = {'fp32': 0, 'tf32x3': 1, 'f16x3': 2, 'f16': 3}
                 if self.conv_math not in modes:
-                    raise ValueError("conv_math must be 'fp32', 'tf32x3' or 'f16x3'")
+                    raise ValueError("conv_math must be 'fp32', 'tf32x3', 'f16x3' or 'f16'")
                 check(L.nrgbd_kvnet_set_option(ent['h'], b'conv_math', modes[self.conv_math]))
                 ent['conv_math'] = self.conv_math
             # .eval(): the 13 BatchNorm layers with running statistics (K-Net's BatchNorm3d, the feature CNN's downsample
