@@ -155,6 +155,27 @@ int nrgbd_depth_regression(const float* bv, int n_pix, int D, long long in_sd, l
 int nrgbd_depth_regression_backward(const float* grad_depth, const float* bv, int n_pix, int D, long long in_sd,
                                     long long in_sp, const float* d_planes, int bv_log, float* g_bv,
                                     nrgbd_stream_t stream);
+/* Depth variance of one slice (mutils/misc.py:550-572 depth_var), same bv layout as nrgbd_depth_regression; mean and var
+ * are [n_pix]:
+ *   var[pix] = (sum_d ((p(d,pix) * d_planes[d] - mean[pix])^2) / var_div) / D,  p = bv_log ? exp(bv) : bv,
+ * summed sequentially over d, every operation rounded on its own. var_div is 2 * d_sigma^2 rounded to float. */
+int nrgbd_depth_var(const float* bv, int n_pix, int D, long long in_sd, long long in_sp, const float* d_planes,
+                    int bv_log, const float* mean, float var_div, float* var, nrgbd_stream_t stream);
+/* Gradient of nrgbd_depth_var with respect to bv (g_bv, same layout as bv: every plane written) and mean (g_mean
+ * [n_pix]), in the rounding order of autograd through misc.py:566-572. Either output may be NULL; no atomics. */
+int nrgbd_depth_var_backward(const float* grad_var, const float* bv, int n_pix, int D, long long in_sd, long long in_sp,
+                             const float* d_planes, int bv_log, const float* mean, float var_div, float* g_bv,
+                             float* g_mean, nrgbd_stream_t stream);
+/* value[n*n_pix + pix] = max_d (is_min: min_d) of p(n,d,pix), p = bv_log ? exp(bv) : bv, element (n,d,pix) of bv at
+ * n*in_sn + d*in_sd + pix*in_sp (misc.py:599-604 dpv_statistics 'max' / 'min'). index (may be NULL) receives the plane as
+ * ATen's max.dim / min.dim on the CPU gives it: ties keep the first plane, the first NaN wins. */
+int nrgbd_dpv_extreme(const float* bv, int n_pix, int n_slices, int D, long long in_sn, long long in_sd, long long in_sp,
+                      int bv_log, int is_min, float* value, int* index, nrgbd_stream_t stream);
+/* Gradient of nrgbd_dpv_extreme's value: g_bv = grad_value * exp(bv) (bv_log; grad_value alone otherwise, bv may then be
+ * NULL) at the plane index names, 0 at every other plane. Every element of g_bv is written; same layout as bv. */
+int nrgbd_dpv_extreme_backward(const float* grad_value, const float* bv, const int* index, int n_pix, int n_slices, int D,
+                               long long in_sn, long long in_sd, long long in_sp, int bv_log, float* g_bv,
+                               nrgbd_stream_t stream);
 int nrgbd_exp(const float* x, long long n, float* y, nrgbd_stream_t stream);
 
 /* ---- f-1: backward of the plane sweep (autograd of warping/homography.py:293-331 as used by

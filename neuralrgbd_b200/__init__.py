@@ -15,7 +15,7 @@ _PATCHES = (
     ('warping.homography', 'neuralrgbd_b200.warping.homography',
      ('est_swp_volume_v4', 'warp_img_feats_v3', 'warp_img_feats_mgpu', 'resample_vol_cuda', 'get_rel_extrinsicM',
       'back_warp_th_Rt', 'back_warp_th_Rt_msrc')),
-    ('mutils.misc', 'neuralrgbd_b200.mutils.misc', ('depth_val_regression', 'valid_dpv')),
+    ('mutils.misc', 'neuralrgbd_b200.mutils.misc', ('depth_val_regression', 'depth_var', 'dpv_statistics', 'valid_dpv')),
     ('models.KVNET', 'neuralrgbd_b200.models.KVNET', ('KVNET',)),
     ('ICP.opt_pose_numerical', 'neuralrgbd_b200.ICP.opt_pose_numerical', ('local_BA_direct', 'local_BA_direct_parallel')),
 )

@@ -41,6 +41,10 @@ SIGNATURES = {
                                     c_vp, c_vp, c_vp, c_vp]),
     'nrgbd_depth_regression': (c_int, [c_vp, c_int, c_int, c_ll, c_ll, c_vp, c_int, c_vp, c_vp, c_vp]),
     'nrgbd_depth_regression_backward': (c_int, [c_vp, c_vp, c_int, c_int, c_ll, c_ll, c_vp, c_int, c_vp, c_vp]),
+    'nrgbd_depth_var': (c_int, [c_vp, c_int, c_int, c_ll, c_ll, c_vp, c_int, c_vp, c_float, c_vp, c_vp]),
+    'nrgbd_depth_var_backward': (c_int, [c_vp, c_vp, c_int, c_int, c_ll, c_ll, c_vp, c_int, c_vp, c_float, c_vp, c_vp, c_vp]),
+    'nrgbd_dpv_extreme': (c_int, [c_vp, c_int, c_int, c_int, c_ll, c_ll, c_ll, c_int, c_int, c_vp, c_vp, c_vp]),
+    'nrgbd_dpv_extreme_backward': (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_ll, c_ll, c_ll, c_int, c_vp, c_vp]),
     'nrgbd_exp': (c_int, [c_vp, c_ll, c_vp, c_vp]),
     'nrgbd_pack_conv_weight': (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     'nrgbd_conv_nhwc': (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_int, c_int, c_int,
