@@ -445,7 +445,7 @@ int nrgbd_kvnet_set_param(nrgbd_kvnet* e, const char* name, const float* data, l
 int nrgbd_kvnet_set_camera(nrgbd_kvnet* e, int slot, const float* K_host, const float* rays_host, float cx,
                            float cy, double hfov_deg, double vfov_deg);
 int nrgbd_kvnet_set_planes(nrgbd_kvnet* e, const float* d_host, int D);   /* float32(d_candi) */
-int nrgbd_kvnet_set_option(nrgbd_kvnet* e, const char* key, int value);   /* "bn_update_running", "profile", "conv_math" (0 fp32 FFMA, 1 wgmma 3xTF32, 2 wgmma split-fp16 pairs), "use_graph" (CUDA-graph replay, default 1), "bn_eval" (1: the module is in .eval(): BatchNorm layers with running statistics normalise with them and update nothing, the others keep batch statistics; default 0), "refine" (refined outputs: 0 the DPV R-Net, default; 1 the guided filter of refineNet_name='DGF', [H][W] depth maps; 2 none, if_refined=False), "refine_upsample_d" (1: the DPV R-Net of if_upsample_d=True, refined log-DPVs of 4D planes; default 0) */
+int nrgbd_kvnet_set_option(nrgbd_kvnet* e, const char* key, int value);   /* "bn_update_running", "profile", "conv_math" (0 fp32 FFMA, 1 wgmma 3xTF32, 2 wgmma split-fp16 pairs, 3 wgmma single fp16 products), "use_graph" (CUDA-graph replay, default 1), "bn_eval" (1: the module is in .eval(): BatchNorm layers with running statistics normalise with them and update nothing, the others keep batch statistics; default 0), "refine" (refined outputs: 0 the DPV R-Net, default; 1 the guided filter of refineNet_name='DGF', [H][W] depth maps; 2 none, if_refined=False), "refine_upsample_d" (1: the DPV R-Net of if_upsample_d=True, refined log-DPVs of 4D planes; default 0) */
 /* with option "profile"=1 the engine brackets its conv (category 0, work = flops) and plane-sweep
  * (category 1, work = algorithmic bytes) launches with CUDA events; this returns and clears the sums. */
 int nrgbd_kvnet_profile_read(nrgbd_kvnet* e, int category, double* ms, double* work, long long* launches);

@@ -53,10 +53,12 @@ struct Pool {           // stream-ordered reuse of cudaMalloc'd blocks (single s
 };
 
 struct ParamRef { float* p; long long n; bool owned; };
-struct Packed { float* w; int Cin, Cin_pad, Cout, Cout_pad, taps; };
-struct PackedTc { float* hi; float* lo; int Cin_pad, Cout_pad, taps; };
-struct PackedH2 { void* w; int Cin_pad, Cout_pad, BN, taps; };       // f16-pair tiles [taps][2][Cout_pad][Cin_pad] halves
-struct PairBuf { float* hi; float* lo; };                          // split-fp16 planes of an activation (pool blocks); lo null: fp16 only
+// One packing of a conv weight: fp32 (PK_F32), TF32 hi planes in w and lo planes in lo (PK_TC), or f16-pair tiles
+// [taps][2][Cout_pad][Cin_pad] halves in w with the kernel's N tile BN (PK_H2, PK_H2_TAPS). w null: not packed yet.
+struct Packed { float* w = nullptr; float* lo = nullptr; int Cin_pad = 0, Cout_pad = 0, BN = 0; };
+enum Packing { PK_F32, PK_TC, PK_H2, PK_H2_TAPS, PK_COUNT };
+typedef std::array<Packed, PK_COUNT> PackedSet;                    // every packing of one parameter
+struct PairBuf { float* hi = nullptr; float* lo = nullptr; };      // split-fp16 planes of an activation (pool blocks); lo null: fp16 only
 
 struct Camera {
   bool set = false;
@@ -81,9 +83,7 @@ struct nrgbd_kvnet {
   float* eval_coef = nullptr;       // [NRGBD_BN_EVAL_MAX][scale 512 | shift 512] of those layers, recomputed by every forward
   std::unordered_map<std::string, int> eval_slot;   // BatchNorm prefix -> row of eval_coef (empty in train mode)
   std::unordered_map<std::string, ParamRef> params;
-  std::unordered_map<std::string, Packed> packed;
-  std::unordered_map<std::string, PackedTc> packed_tc;
-  std::unordered_map<std::string, PackedH2> packed_h2;
+  std::unordered_map<std::string, PackedSet> packed;   // by parameter name: set_param drops all packings of a re-set weight
   // activations that currently have a split-fp16 copy (conv_math 2 and 3). In conv_math 3 only the tensors read as residuals
   // keep a lo half; the rest are plain fp16 (lo null), since a convolution reads hi only.
   std::unordered_map<const float*, PairBuf> pairs;
@@ -92,7 +92,6 @@ struct nrgbd_kvnet {
   int conv_math = 0;
   int refine = 0;                   // refinement of KVNET(...): 0 the DPV R-Net, 1 the guided filter ('DGF'), 2 none (if_refined=False)
   int refine_up = 0;                // DPV R-Net with if_upsample_d: widths D0 = 2D, D1 = 4D (Refine.py:44-48)
-  bool packed_dirty = true;
   Camera cam[2];
   float* d_planes = nullptr;
   std::vector<float> d_host;
@@ -100,9 +99,6 @@ struct nrgbd_kvnet {
   double* stats = nullptr;          // [2][512] per-channel sums of the conv in flight
   double* stats_b = nullptr;        // second set: a conv that consumes one BatchNorm (fused) while producing the next
   unsigned int* bn_counter = nullptr;   // f16-pair mode: the BatchNorm pass re-zeroes the statistics it consumed (no memset nodes)
-  int fuse_bn = 1;                  // tf32x3: 1 folds a BN+ReLU whose only reader is a convolution into that convolution's operand split
-  float* scale = nullptr;           // [512]
-  float* shift = nullptr;           // [512]
   float* ws_sweep = nullptr;        // V*12
   cudaStream_t st = nullptr;
   int rc = 0;                       // first error of the current forward
@@ -190,21 +186,52 @@ inline bool keep_lo(const Eng* e, bool res_read) { return e->conv_math == 2 || r
 // x_lo of a convolution launch: NULL runs the single-product kernel (conv_math 3) even when the pair has a lo for a residual
 inline const void* conv_lo(const Eng* e, const PairBuf* pb) { return e->conv_math == 3 ? nullptr : pb->lo; }
 
+// Pool blocks of a split-fp16 pair of `floats` elements: hi, then lo when `lo` is set (see keep_lo)
+bool acquire_pair(Eng* e, long long floats, bool lo, PairBuf& pb) {
+  if (e->rc) return false;
+  pb.hi = e->pool.acquire((size_t)floats * 2);
+  pb.lo = lo ? e->pool.acquire((size_t)floats * 2) : nullptr;
+  if (pb.hi && (pb.lo || !lo)) return true;
+  nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM;
+  return false;
+}
+
+// An activation written only as the operand pair of the convolutions that read it (f16-pair mode): y.p is a 16-byte pool
+// block that keys the pair in e->pairs, not an fp32 tensor. res_read: a residual add reads it too, so its lo half is kept.
+Act pair_act(Eng* e, int N, int D, int H, int W, int C, bool res_read, PairBuf& pb) {
+  Act y; y.N = N; y.D = D; y.H = H; y.W = W; y.C = C; y.Cs = pad32(C); y.pair_only = true;
+  if (e->rc) return y;
+  y.p = e->pool.acquire(16);
+  if (!acquire_pair(e, y.floats(), keep_lo(e, res_read), pb)) return y;
+  if (!y.p) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; return y; }
+  e->pairs[y.p] = pb;
+  return y;
+}
+
 // Split-fp16 operand planes of an activation (x = hi + lo * 2^-11), created on first use by a convolution and kept
 // until the activation is released: several convolutions may consume the same tensor (BasicBlock input: conv1 +
 // downsample). Activations are never written again after their first conv consumer has run. conv_math 3: hi only.
 const PairBuf* pair_of(Eng* e, const Act& x) {
   auto it = e->pairs.find(x.p);
   if (it != e->pairs.end()) return &it->second;
-  if (e->rc) return nullptr;
   PairBuf pb;
-  const size_t bytes = (size_t)x.floats() * 2;
-  pb.hi = e->pool.acquire(bytes);
-  pb.lo = keep_lo(e, false) ? e->pool.acquire(bytes) : nullptr;
-  if (!pb.hi || (!pb.lo && keep_lo(e, false))) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; return nullptr; }
+  if (!acquire_pair(e, x.floats(), keep_lo(e, false), pb)) return nullptr;
   ENG_CALL(e, nrgbd_split_f16_pair(x.p, x.floats(), pb.hi, pb.lo, (nrgbd_stream_t)e->st));
-  e->pairs[x.p] = pb;
-  return &e->pairs[x.p];
+  return &(e->pairs[x.p] = pb);
+}
+
+// Residual operand of a BatchNorm epilogue: the fp32 tensor, or the (hi, lo) pair of a residual that exists only as a pair
+struct Residual { const float* f = nullptr; const void* hi = nullptr; const void* lo = nullptr; };
+Residual residual_of(Eng* e, const Act* res) {
+  Residual r;
+  if (!res) return r;
+  if (!res->pair_only) { r.f = res->p; return r; }
+  auto it = e->pairs.find(res->p);
+  if (it == e->pairs.end() || !it->second.lo) {
+    nrgbd_set_error("engine: residual has neither an fp32 copy nor a full operand pair"); e->rc = NRGBD_ERR_BAD_ARG; return r;
+  }
+  r.hi = it->second.hi; r.lo = it->second.lo;
+  return r;
 }
 
 float* param(Eng* e, const std::string& name) {
@@ -220,87 +247,50 @@ float* param_opt(Eng* e, const std::string& name) {
   return it == e->params.end() ? nullptr : it->second.p;
 }
 
-const Packed* packw(Eng* e, const std::string& name, int Cout, int Cin, int taps, bool transposed) {
+// Training-mode BatchNorm `pre`: its affine parameters, and the running buffers the pass updates (both, or neither: option
+// bn_update_running off, or a layer without running statistics)
+struct BnParams { float* gamma; float* beta; float* rm; float* rv; };
+BnParams bn_params(Eng* e, const std::string& pre) {
+  BnParams p;
+  p.gamma = param(e, pre + ".weight"); p.beta = param(e, pre + ".bias");
+  float* rm = e->bn_update_running ? param_opt(e, pre + ".running_mean") : nullptr;
+  float* rv = e->bn_update_running ? param_opt(e, pre + ".running_var") : nullptr;
+  p.rm = rm && rv ? rm : nullptr; p.rv = rm && rv ? rv : nullptr;
+  return p;
+}
+
+void free_packed(PackedSet& s) { for (auto& pk : s) { cudaFree(pk.w); cudaFree(pk.lo); } }
+
+// Conv weight `name` [Cout][Cin][taps] (transposed: [Cin][Cout][taps]) in the packing `kind`, made on first use.
+// PK_H2_TAPS is the weight of a single-output-channel conv [1][Cin][taps] packed as the POINTWISE conv [taps][Cin] (one
+// output channel per tap) for the tap-gather form of K-Net's last layer (nrgbd_tap_gather_sum): the transposed-kind f16-pair
+// packing, requested with Cout = taps and 1 tap.
+const Packed* packw(Eng* e, const std::string& name, Packing kind, int Cout, int Cin, int taps, bool transposed) {
   auto it = e->packed.find(name);
-  if (it != e->packed.end()) return &it->second;
+  if (it != e->packed.end() && it->second[kind].w) return &it->second[kind];
   float* src = param(e, name);
-  if (!src) return nullptr;
-  auto pr = e->params[name];
-  if (pr.n != (long long)Cout * Cin * taps) {
-    if (e->rc == 0) { nrgbd_set_error("engine: parameter '%s' has %lld elements, expected %lld", name.c_str(), pr.n, (long long)Cout * Cin * taps); e->rc = NRGBD_ERR_BAD_ARG; }
+  if (!src || e->rc) return nullptr;
+  const long long n = e->params[name].n;
+  if (n != (long long)Cout * Cin * taps) {
+    nrgbd_set_error("engine: parameter '%s' has %lld elements, expected %lld", name.c_str(), n, (long long)Cout * Cin * taps);
+    e->rc = NRGBD_ERR_BAD_ARG;
     return nullptr;
   }
-  Packed pk; pk.Cin = Cin; pk.Cout = Cout; pk.taps = taps; pk.Cin_pad = pad4(Cin); pk.Cout_pad = pad4(Cout);
-  size_t bytes = (size_t)taps * pk.Cin_pad * pk.Cout_pad * sizeof(float);
-  void* q = nullptr;
-  if (cudaMalloc(&q, bytes) != cudaSuccess) { e->rc = NRGBD_ERR_NOMEM; nrgbd_set_error("engine: cudaMalloc failed for packed weight"); return nullptr; }
-  pk.w = (float*)q;
-  ENG_CALL(e, nrgbd_pack_conv_weight(src, transposed ? 1 : 0, Cout, Cin, taps, pk.Cin_pad, pk.Cout_pad, pk.w, (nrgbd_stream_t)e->st));
-  e->packed[name] = pk;
-  return &e->packed[name];
-}
-
-const PackedTc* packw_tc(Eng* e, const std::string& name, int Cout, int Cin, int taps, bool transposed) {
-  auto it = e->packed_tc.find(name);
-  if (it != e->packed_tc.end()) return &it->second;
-  float* src = param(e, name);
-  if (!src) return nullptr;
-  auto pr = e->params[name];
-  if (pr.n != (long long)Cout * Cin * taps) {
-    if (e->rc == 0) { nrgbd_set_error("engine: parameter '%s' has %lld elements, expected %lld", name.c_str(), pr.n, (long long)Cout * Cin * taps); e->rc = NRGBD_ERR_BAD_ARG; }
-    return nullptr;
+  const bool h2 = kind == PK_H2 || kind == PK_H2_TAPS;
+  Packed pk;
+  if (h2) nrgbd_conv_h2_plan(Cin, Cout, &pk.Cin_pad, &pk.Cout_pad, &pk.BN);
+  else if (kind == PK_TC) { pk.Cin_pad = pad32(Cin); pk.Cout_pad = pad16(Cout); }
+  else { pk.Cin_pad = pad4(Cin); pk.Cout_pad = pad4(Cout); }
+  const size_t bytes = (size_t)taps * pk.Cin_pad * pk.Cout_pad * (h2 ? 2 * 2 : sizeof(float));    // f16 pairs: two halves
+  if (cudaMalloc((void**)&pk.w, bytes) != cudaSuccess || (kind == PK_TC && cudaMalloc((void**)&pk.lo, bytes) != cudaSuccess)) {
+    cudaFree(pk.w); e->rc = NRGBD_ERR_NOMEM; nrgbd_set_error("engine: cudaMalloc failed for packed weight"); return nullptr;
   }
-  PackedTc pk; pk.taps = taps; pk.Cin_pad = pad32(Cin); pk.Cout_pad = pad16(Cout);
-  size_t bytes = (size_t)taps * pk.Cin_pad * pk.Cout_pad * sizeof(float);
-  void* q = nullptr; void* r = nullptr;
-  if (cudaMalloc(&q, bytes) != cudaSuccess || cudaMalloc(&r, bytes) != cudaSuccess) { e->rc = NRGBD_ERR_NOMEM; nrgbd_set_error("engine: cudaMalloc failed for packed weight"); return nullptr; }
-  pk.hi = (float*)q; pk.lo = (float*)r;
-  ENG_CALL(e, nrgbd_pack_conv_weight_tc(src, transposed ? 1 : 0, Cout, Cin, taps, pk.Cin_pad, pk.Cout_pad, pk.hi, pk.lo, (nrgbd_stream_t)e->st));
-  e->packed_tc[name] = pk;
-  return &e->packed_tc[name];
-}
-
-const PackedH2* packw_h2(Eng* e, const std::string& name, int Cout, int Cin, int taps, bool transposed) {
-  auto it = e->packed_h2.find(name);
-  if (it != e->packed_h2.end()) return &it->second;
-  float* src = param(e, name);
-  if (!src) return nullptr;
-  auto pr = e->params[name];
-  if (pr.n != (long long)Cout * Cin * taps) {
-    if (e->rc == 0) { nrgbd_set_error("engine: parameter '%s' has %lld elements, expected %lld", name.c_str(), pr.n, (long long)Cout * Cin * taps); e->rc = NRGBD_ERR_BAD_ARG; }
-    return nullptr;
-  }
-  PackedH2 pk; pk.taps = taps;
-  nrgbd_conv_h2_plan(Cin, Cout, &pk.Cin_pad, &pk.Cout_pad, &pk.BN);
-  void* q = nullptr;
-  if (cudaMalloc(&q, (size_t)taps * 2 * pk.Cin_pad * pk.Cout_pad * 2) != cudaSuccess) { e->rc = NRGBD_ERR_NOMEM; nrgbd_set_error("engine: cudaMalloc failed for packed weight"); return nullptr; }
-  pk.w = q;
-  ENG_CALL(e, nrgbd_pack_conv_weight_h2(src, transposed ? 1 : 0, Cout, Cin, taps, pk.Cin_pad, pk.Cout_pad, pk.w, (nrgbd_stream_t)e->st));
-  e->packed_h2[name] = pk;
-  return &e->packed_h2[name];
-}
-
-// Weight of a single-output-channel conv [1][Cin][taps] packed as the POINTWISE conv [taps][Cin] (one output channel per tap) for
-// the tap-gather form of K-Net's last layer (nrgbd_tap_gather_sum): that is the transposed-kind packing with Cout = taps.
-const PackedH2* packw_h2_taps(Eng* e, const std::string& name, int Cin, int taps) {
-  const std::string key = name + "#taps";
-  auto it = e->packed_h2.find(key);
-  if (it != e->packed_h2.end()) return &it->second;
-  float* src = param(e, name);
-  if (!src) return nullptr;
-  auto pr = e->params[name];
-  if (pr.n != (long long)Cin * taps) {
-    if (e->rc == 0) { nrgbd_set_error("engine: parameter '%s' has %lld elements, expected %lld", name.c_str(), pr.n, (long long)Cin * taps); e->rc = NRGBD_ERR_BAD_ARG; }
-    return nullptr;
-  }
-  PackedH2 pk; pk.taps = 1;
-  nrgbd_conv_h2_plan(Cin, taps, &pk.Cin_pad, &pk.Cout_pad, &pk.BN);
-  void* q = nullptr;
-  if (cudaMalloc(&q, (size_t)2 * pk.Cin_pad * pk.Cout_pad * 2) != cudaSuccess) { e->rc = NRGBD_ERR_NOMEM; nrgbd_set_error("engine: cudaMalloc failed for packed weight"); return nullptr; }
-  pk.w = q;
-  ENG_CALL(e, nrgbd_pack_conv_weight_h2(src, 1, taps, Cin, 1, pk.Cin_pad, pk.Cout_pad, pk.w, (nrgbd_stream_t)e->st));
-  e->packed_h2[key] = pk;
-  return &e->packed_h2[key];
+  const int tr = transposed ? 1 : 0;
+  nrgbd_stream_t st = (nrgbd_stream_t)e->st;
+  if (h2) ENG_CALL(e, nrgbd_pack_conv_weight_h2(src, tr, Cout, Cin, taps, pk.Cin_pad, pk.Cout_pad, pk.w, st));
+  else if (kind == PK_TC) ENG_CALL(e, nrgbd_pack_conv_weight_tc(src, tr, Cout, Cin, taps, pk.Cin_pad, pk.Cout_pad, pk.w, pk.lo, st));
+  else ENG_CALL(e, nrgbd_pack_conv_weight(src, tr, Cout, Cin, taps, pk.Cin_pad, pk.Cout_pad, pk.w, st));
+  return &(e->packed[name][kind] = pk);
 }
 
 // f16-pair tensor path: any conv whose activation carries its channels padded to the packed weight's Cin_pad = pad32(C).
@@ -325,84 +315,91 @@ void split_act(Eng* e, const Act& x, Act& hi, Act& lo) {
   ENG_CALL(e, nrgbd_split_tf32(x.p, x.floats(), hi.p, lo.p, (nrgbd_stream_t)e->st));
 }
 
-// conv (2-D when x.D == 1 and kd == 1) into a fresh activation or into `dst` at channel c_off
-// pair_out (f16-pair mode, no BatchNorm after the conv): the result is written only as the operand pair of the convolution that
-// consumes it (y.p is a 16-byte key of the pair, y.pair_only) - no fp32 tensor, no split pass
+// Output extent, algorithmic FLOPs and profile tag of a convolution; bench.py's roofline and --layer-table read the tags.
+// transposed: a ConvTranspose2d, whose every output reads 1 / stride^2 of the taps.
+struct ConvGeom { int Ho, Wo; double flops; char tag[56]; };
+ConvGeom conv_geom(const Act& x, int Cout, int kd, int k, int stride, int pad, int dil, bool transposed = false) {
+  ConvGeom g;
+  const int span = dil * (k - 1) + 1;
+  g.Ho = transposed ? (x.H - 1) * stride - 2 * pad + span : (x.H + 2 * pad - span) / stride + 1;
+  g.Wo = transposed ? (x.W - 1) * stride - 2 * pad + span : (x.W + 2 * pad - span) / stride + 1;
+  g.flops = 2.0 * x.N * x.D * g.Ho * g.Wo * Cout * x.C * kd * k * k / (transposed ? stride * stride : 1);
+  if (transposed) snprintf(g.tag, sizeof(g.tag), "convT k%d s%d %d->%d %dx%dx%d", k, stride, x.C, Cout, x.N, g.Ho, g.Wo);
+  else snprintf(g.tag, sizeof(g.tag), "conv%dd k%d s%d d%d %d->%d %dx%dx%dx%d", kd > 1 ? 3 : 2, k, stride, dil, x.C, Cout, x.N, x.D, g.Ho, g.Wo);
+  return g;
+}
+
+// Where conv() writes. Default: a fresh activation with acquire()'s channel stride, per-channel sums into e->stats.
+struct ConvOut {
+  Act* dst = nullptr;                       // write into this activation instead
+  int Cs = -1;                              // channel stride of the fresh activation
+  double* stats = nullptr;                  // per-channel sums into this buffer instead
+  const nrgbd_bn_input* in_bn = nullptr;    // 3xTF32: x is the RAW output of a conv, normalised while its operands are split
+  // f16-pair mode, no BatchNorm after the conv: the result is written only as the operand pair of the convolution that
+  // consumes it (y.p is a 16-byte key of the pair, y.pair_only) - no fp32 tensor, no split pass
+  bool pair_only = false;
+};
+
+// conv (2-D when x.D == 1 and kd == 1)
 Act conv(Eng* e, const Act& x, const std::string& wname, int Cout, int kd, int k, int stride, int pad, int dil,
-         const char* bias_name, bool leaky, bool want_stats, Act* dst = nullptr, int c_off = 0, int out_Cs = -1,
-         double* stats_buf = nullptr, const nrgbd_bn_input* in_bn = nullptr, bool pair_out = false) {
-  if (!stats_buf) stats_buf = e->stats;
+         const char* bias_name, bool leaky, bool want_stats, const ConvOut& out = ConvOut()) {
+  double* stats = want_stats ? (out.stats ? out.stats : e->stats) : nullptr;
+  nrgbd_stream_t st = (nrgbd_stream_t)e->st;
   if (x.pair_only && !use_h2(e, x)) {          // x.p is no fp32 tensor: only the f16-pair path can read x
     if (!e->rc) { nrgbd_set_error("engine: '%s' reads an activation that exists only as an operand pair", wname.c_str()); e->rc = NRGBD_ERR_BAD_ARG; }
     return Act();
   }
-  int Ho = (x.H + 2 * pad - dil * (k - 1) - 1) / stride + 1;
-  int Wo = (x.W + 2 * pad - dil * (k - 1) - 1) / stride + 1;
-  Act y;
-  if (pair_out && use_h2(e, x) && Cout >= 16 && !dst && !want_stats && c_off == 0 && out_Cs < 0 && stride == 1) {
-    y.N = x.N; y.D = x.D; y.H = Ho; y.W = Wo; y.C = Cout; y.Cs = pad32(Cout); y.pair_only = true;
-    float* b = bias_name ? param(e, bias_name) : nullptr;
-    const PackedH2* ph = packw_h2(e, wname, Cout, x.C, kd * k * k, false);
+  const ConvGeom g = conv_geom(x, Cout, kd, k, stride, pad, dil);
+  const int taps = kd * k * k;
+  float* b = bias_name ? param(e, bias_name) : nullptr;
+  if (out.pair_only && use_h2(e, x) && Cout >= 16 && !out.dst && !want_stats && out.Cs < 0 && stride == 1) {
+    const Packed* ph = packw(e, wname, PK_H2, Cout, x.C, taps, false);
     const PairBuf* pin = pair_of(e, x);
-    if (e->rc) return y;
     PairBuf pb;
-    y.p = e->pool.acquire(16);                                    // key of the pair buffers
-    pb.hi = e->pool.acquire((size_t)y.floats() * 2);
-    pb.lo = keep_lo(e, false) ? e->pool.acquire((size_t)y.floats() * 2) : nullptr;   // R-Net: no residuals
-    if (!y.p || !pb.hi || (!pb.lo && keep_lo(e, false))) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; return y; }
-    e->pairs[y.p] = pb;
-    const double flops = 2.0 * (double)x.N * x.D * Ho * Wo * Cout * x.C * kd * k * k;
-    char tag[56];
-    snprintf(tag, sizeof(tag), "conv%dd k%d s%d d%d %d->%d %dx%dx%dx%d", kd > 1 ? 3 : 2, k, stride, dil, x.C, Cout, x.N, x.D, Ho, Wo);
-    ProfScope ps(e, 0, flops, tag);
+    Act y = pair_act(e, x.N, x.D, g.Ho, g.Wo, Cout, false, pb);      // R-Net: no residuals
+    if (e->rc) return y;
+    ProfScope ps(e, 0, g.flops, g.tag);
     ENG_CALL(e, nrgbd_conv_nhwc_h2_pair(pin->hi, conv_lo(e, pin), x.N, x.D, x.H, x.W, ph->Cin_pad, x.Cs, ph->w, b, Cout, ph->Cout_pad, ph->BN, kd, k, k,
-                                        stride, pad, dil, pb.hi, pb.lo, Ho, Wo, y.Cs, leaky ? 1 : 0, (nrgbd_stream_t)e->st));
+                                        stride, pad, dil, pb.hi, pb.lo, g.Ho, g.Wo, y.Cs, leaky ? 1 : 0, st));
     return y;
   }
-  if (dst) y = *dst; else y = acquire(e, x.N, x.D, Ho, Wo, Cout, out_Cs);
-  float* b = bias_name ? param(e, bias_name) : nullptr;
+  Act y = out.dst ? *out.dst : acquire(e, x.N, x.D, g.Ho, g.Wo, Cout, out.Cs);
   if (e->rc) return y;
-  if (want_stats && !pair_mode(e)) cudaMemsetAsync(stats_buf, 0, sizeof(double) * 2 * Cout, e->st);   // f16-pair mode: kept zero by the BN pass
-  const double flops = 2.0 * (double)x.N * x.D * Ho * Wo * Cout * x.C * kd * k * k;
-  char tag[56];
-  snprintf(tag, sizeof(tag), "conv%dd k%d s%d d%d %d->%d %dx%dx%dx%d", kd > 1 ? 3 : 2, k, stride, dil, x.C, Cout, x.N, x.D, Ho, Wo);
+  if (stats && !pair_mode(e)) cudaMemsetAsync(stats, 0, sizeof(double) * 2 * Cout, e->st);   // f16-pair mode: kept zero by the BN pass
   if (use_h2(e, x)) {
-    const PackedH2* ph = packw_h2(e, wname, Cout, x.C, kd * k * k, false);
+    const Packed* ph = packw(e, wname, PK_H2, Cout, x.C, taps, false);
     const PairBuf* pb = pair_of(e, x);
     if (e->rc) return y;
-    ProfScope ps(e, 0, flops, tag);
+    ProfScope ps(e, 0, g.flops, g.tag);
     ENG_CALL(e, nrgbd_conv_nhwc_h2(pb->hi, conv_lo(e, pb), x.N, x.D, x.H, x.W, ph->Cin_pad, x.Cs, ph->w, b, Cout, ph->Cout_pad, ph->BN, kd, k, k, stride,
-                                   pad, dil, y.p, Ho, Wo, y.Cs, c_off, leaky ? 1 : 0, want_stats ? stats_buf : nullptr, (nrgbd_stream_t)e->st));
+                                   pad, dil, y.p, g.Ho, g.Wo, y.Cs, 0, leaky ? 1 : 0, stats, st));
     return y;
   }
   if (use_tc(e, x, Cout)) {
-    const PackedTc* pt = packw_tc(e, wname, Cout, x.C, kd * k * k, false);
-    if (!e->rc && in_bn) {
+    const Packed* pt = packw(e, wname, PK_TC, Cout, x.C, taps, false);
+    if (!e->rc && out.in_bn) {
       // x is the RAW output of the producing conv: BatchNorm + ReLU are applied in the pass that splits the operands
       // (4 B read + 8 B written per element, against 4 + 4 for a separate BatchNorm pass and 4 + 8 for the split after it)
-      ProfScope ps(e, 0, flops, tag);
-      ENG_CALL(e, nrgbd_conv_nhwc_tc2_bn_in(x.p, x.N, x.D, x.H, x.W, pt->Cin_pad, x.Cs, pt->hi, pt->lo, b, Cout, pt->Cout_pad, kd, k, k,
-                                            stride, pad, dil, y.p, Ho, Wo, y.Cs, c_off, leaky ? 1 : 0, want_stats ? stats_buf : nullptr,
-                                            in_bn, (nrgbd_stream_t)e->st));
+      ProfScope ps(e, 0, g.flops, g.tag);
+      ENG_CALL(e, nrgbd_conv_nhwc_tc2_bn_in(x.p, x.N, x.D, x.H, x.W, pt->Cin_pad, x.Cs, pt->w, pt->lo, b, Cout, pt->Cout_pad, kd, k, k,
+                                            stride, pad, dil, y.p, g.Ho, g.Wo, y.Cs, 0, leaky ? 1 : 0, stats, out.in_bn, st));
       return y;
     }
     Act xh, xl;
     split_act(e, x, xh, xl);
     if (!e->rc) {
-      ProfScope ps(e, 0, flops, tag);
-      ENG_CALL(e, nrgbd_conv_nhwc_tc(xh.p, xl.p, x.N, x.D, x.H, x.W, pt->Cin_pad, x.Cs, pt->hi, pt->lo, b, Cout, pt->Cout_pad, kd, k, k,
-                                     stride, pad, dil, y.p, Ho, Wo, y.Cs, c_off, leaky ? 1 : 0, want_stats ? stats_buf : nullptr,
-                                     (nrgbd_stream_t)e->st));
+      ProfScope ps(e, 0, g.flops, g.tag);
+      ENG_CALL(e, nrgbd_conv_nhwc_tc(xh.p, xl.p, x.N, x.D, x.H, x.W, pt->Cin_pad, x.Cs, pt->w, pt->lo, b, Cout, pt->Cout_pad, kd, k, k,
+                                     stride, pad, dil, y.p, g.Ho, g.Wo, y.Cs, 0, leaky ? 1 : 0, stats, st));
     }
     release(e, xh); release(e, xl);
     return y;
   }
-  const Packed* pk = packw(e, wname, Cout, x.C, kd * k * k, false);
+  const Packed* pk = packw(e, wname, PK_F32, Cout, x.C, taps, false);
   if (e->rc) return y;
-  ProfScope ps(e, 0, flops, tag);
+  ProfScope ps(e, 0, g.flops, g.tag);
   ENG_CALL(e, nrgbd_conv_nhwc(x.p, x.N, x.D, x.H, x.W, pk->Cin_pad, x.Cs, pk->w, b, Cout, pk->Cout_pad, kd, k, k, stride,
-                              pad, dil, y.p, Ho, Wo, y.Cs, c_off, leaky ? 1 : 0, want_stats ? stats_buf : nullptr,
-                              (nrgbd_stream_t)e->st));
+                              pad, dil, y.p, g.Ho, g.Wo, y.Cs, 0, leaky ? 1 : 0, stats, st));
   return y;
 }
 
@@ -457,41 +454,20 @@ Act convbn_eval(Eng* e, const Act& x, const std::string& wname, int Cout, int kd
                 const Act* res, int out_use, const float* scale, bool res_read = false) {
   const float* shift = scale + 512;
   if (use_h2(e, x)) {
-    const int Ho = (x.H + 2 * pad - dil * (k - 1) - 1) / stride + 1, Wo = (x.W + 2 * pad - dil * (k - 1) - 1) / stride + 1;
-    const PackedH2* ph = packw_h2(e, wname, Cout, x.C, kd * k * k, false);
+    const ConvGeom g = conv_geom(x, Cout, kd, k, stride, pad, dil);
+    const Packed* ph = packw(e, wname, PK_H2, Cout, x.C, kd * k * k, false);
     const PairBuf* pin = pair_of(e, x);
-    Act y;
+    if (e->rc) return Act();
+    PairBuf pb;
+    Act y = out_use == 2 ? pair_act(e, x.N, x.D, g.Ho, g.Wo, Cout, res_read, pb) : acquire(e, x.N, x.D, g.Ho, g.Wo, Cout);
     if (e->rc) return y;
-    PairBuf pb; pb.hi = pb.lo = nullptr;
-    if (out_use == 2) {
-      y.N = x.N; y.D = x.D; y.H = Ho; y.W = Wo; y.C = Cout; y.Cs = pad32(Cout); y.pair_only = true;
-      y.p = e->pool.acquire(16);                                    // key of the pair buffers
-      pb.hi = e->pool.acquire((size_t)y.floats() * 2);
-      pb.lo = keep_lo(e, res_read) ? e->pool.acquire((size_t)y.floats() * 2) : nullptr;
-      if (!y.p || !pb.hi || (!pb.lo && keep_lo(e, res_read))) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; return y; }
-      e->pairs[y.p] = pb;
-    } else {
-      y = acquire(e, x.N, x.D, Ho, Wo, Cout);
-      if (e->rc) return y;
-    }
-    const float* res_f = nullptr;
-    const void *res_hi = nullptr, *res_lo = nullptr;
-    if (res) {
-      if (res->Cs != y.Cs || res->pos() != y.pos()) { nrgbd_set_error("engine: residual layout differs from the output's"); e->rc = NRGBD_ERR_BAD_ARG; return y; }
-      if (res->pair_only) {
-        auto it = e->pairs.find(res->p);
-        if (it == e->pairs.end() || !it->second.lo) { nrgbd_set_error("engine: residual has neither an fp32 copy nor a full operand pair"); e->rc = NRGBD_ERR_BAD_ARG; return y; }
-        res_hi = it->second.hi; res_lo = it->second.lo;
-      } else {
-        res_f = res->p;
-      }
-    }
-    char tag[56];
-    snprintf(tag, sizeof(tag), "conv%dd k%d s%d d%d %d->%d %dx%dx%dx%d", kd > 1 ? 3 : 2, k, stride, dil, x.C, Cout, x.N, x.D, Ho, Wo);
-    ProfScope ps(e, 0, 2.0 * (double)x.N * x.D * Ho * Wo * Cout * x.C * kd * k * k, tag);
+    if (res && (res->Cs != y.Cs || res->pos() != y.pos())) { nrgbd_set_error("engine: residual layout differs from the output's"); e->rc = NRGBD_ERR_BAD_ARG; return y; }
+    const Residual r = residual_of(e, res);
+    if (e->rc) return y;
+    ProfScope ps(e, 0, g.flops, g.tag);
     ENG_CALL(e, nrgbd_conv_nhwc_h2_affine(pin->hi, conv_lo(e, pin), x.N, x.D, x.H, x.W, ph->Cin_pad, x.Cs, ph->w, Cout, ph->Cout_pad, ph->BN, kd, k, k,
-                                          stride, pad, dil, scale, shift, res_f, res_hi, res_lo, relu ? 1 : 0, out_use == 2 ? nullptr : y.p,
-                                          pb.hi, pb.lo, Ho, Wo, y.Cs, 0, (nrgbd_stream_t)e->st));
+                                          stride, pad, dil, scale, shift, r.f, r.hi, r.lo, relu ? 1 : 0, out_use == 2 ? nullptr : y.p,
+                                          pb.hi, pb.lo, g.Ho, g.Wo, y.Cs, 0, (nrgbd_stream_t)e->st));
     return y;
   }
   if (res && res->pair_only) { nrgbd_set_error("engine: residual exists only as an operand pair"); e->rc = NRGBD_ERR_BAD_ARG; return Act(); }
@@ -499,6 +475,24 @@ Act convbn_eval(Eng* e, const Act& x, const std::string& wname, int Cout, int kd
   if (!e->rc)
     ENG_CALL(e, nrgbd_bn_apply(y.p, scale, shift, res ? res->p : nullptr, relu ? 1 : 0, y.pos(), y.Cs, y.C, y.p, (nrgbd_stream_t)e->st));
   return y;
+}
+
+// Training-mode BatchNorm `pre` [+ residual] [+ ReLU] in place on the RAW conv output y, from that conv's sums `stats`
+void bn_train(Eng* e, Act& y, const std::string& pre, const double* stats, const float* res, bool relu) {
+  const BnParams bn = bn_params(e, pre);
+  ENG_CALL(e, nrgbd_bn_apply_stats(y.p, stats, (double)y.pos(), bn.gamma, bn.beta, 1e-5f, bn.rm, bn.rv, 0.1f, res, relu ? 1 : 0,
+                                   y.pos(), y.Cs, y.C, y.p, (nrgbd_stream_t)e->st));
+}
+
+// 3xTF32 descriptor of training-mode BatchNorm `pre` + ReLU on t, the RAW output of the conv whose sums are in `stats`:
+// applied by the convolution that reads t while it splits its operands (nrgbd_conv_nhwc_tc2_bn_in)
+nrgbd_bn_input bn_input(Eng* e, const std::string& pre, const double* stats, const Act& t) {
+  const BnParams p = bn_params(e, pre);
+  nrgbd_bn_input bn;
+  bn.stats = stats; bn.count = (double)t.pos();
+  bn.gamma = p.gamma; bn.beta = p.beta; bn.running_mean = p.rm; bn.running_var = p.rv;
+  bn.eps = 1e-5f; bn.momentum = 0.1f; bn.relu = 1; bn.C = t.C;
+  return bn;
 }
 
 // Conv (no bias) + BatchNorm(batch statistics) [+ ReLU] [+ residual]; BN applied in place.
@@ -514,36 +508,20 @@ Act convbn(Eng* e, const Act& x, const std::string& pre, int Cout, int kd, int k
   if (const float* sc = eval_coef(e, pre + ".1"))
     return convbn_eval(e, x, pre + ".0.weight", Cout, kd, k, stride, p, dil, relu, res, out_use, sc, res_read);
   Act y = conv(e, x, pre + ".0.weight", Cout, kd, k, stride, p, dil, nullptr, false, true);
-  float* g = param(e, pre + ".1.weight");
-  float* b = param(e, pre + ".1.bias");
-  float* rm = e->bn_update_running ? param_opt(e, pre + ".1.running_mean") : nullptr;
-  float* rv = e->bn_update_running ? param_opt(e, pre + ".1.running_var") : nullptr;
+  if (!pair_mode(e)) { bn_train(e, y, pre + ".1", e->stats, res ? res->p : nullptr, relu); return y; }
+  const BnParams bn = bn_params(e, pre + ".1");
   if (e->rc) return y;
-  if (pair_mode(e)) {
-    const bool pair = out_use && use_h2(e, y);
-    const bool lo = keep_lo(e, res_read && out_use == 2);   // out_use 1: a residual add reads the fp32 copy
-    PairBuf pb; pb.hi = pb.lo = nullptr;
-    if (pair) {
-      pb.hi = e->pool.acquire((size_t)y.floats() * 2);
-      pb.lo = lo ? e->pool.acquire((size_t)y.floats() * 2) : nullptr;
-      if (!pb.hi || (!pb.lo && lo)) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; return y; }
-    }
-    const float* res_f = res ? res->p : nullptr;
-    const void *res_hi = nullptr, *res_lo = nullptr;
-    if (res && res->pair_only) {
-      auto it = e->pairs.find(res->p);
-      if (it == e->pairs.end() || !it->second.lo) { nrgbd_set_error("engine: residual has neither an fp32 copy nor a full operand pair"); e->rc = NRGBD_ERR_BAD_ARG; return y; }
-      res_f = nullptr; res_hi = it->second.hi; res_lo = it->second.lo;
-    }
-    ENG_CALL(e, nrgbd_bn_apply_stats_pair(y.p, e->stats, (double)y.pos(), g, b, 1e-5f, rm && rv ? rm : nullptr, rm && rv ? rv : nullptr,
-                                          0.1f, res_f, res_hi, res_lo, relu ? 1 : 0, y.pos(), y.Cs, y.C, (pair && out_use == 2) ? nullptr : y.p,
-                                          pb.hi, pb.lo, e->bn_counter, (nrgbd_stream_t)e->st));
-    y.pair_only = pair && out_use == 2;
-    if (pair) e->pairs[y.p] = pb;
-    return y;
-  }
-  ENG_CALL(e, nrgbd_bn_apply_stats(y.p, e->stats, (double)y.pos(), g, b, 1e-5f, rm && rv ? rm : nullptr, rm && rv ? rv : nullptr,
-                                   0.1f, res ? res->p : nullptr, relu ? 1 : 0, y.pos(), y.Cs, y.C, y.p, (nrgbd_stream_t)e->st));
+  const bool pair = out_use && use_h2(e, y);
+  PairBuf pb;
+  // out_use 1: a residual add reads the fp32 copy
+  if (pair && !acquire_pair(e, y.floats(), keep_lo(e, res_read && out_use == 2), pb)) return y;
+  const Residual r = residual_of(e, res);
+  if (e->rc) return y;
+  ENG_CALL(e, nrgbd_bn_apply_stats_pair(y.p, e->stats, (double)y.pos(), bn.gamma, bn.beta, 1e-5f, bn.rm, bn.rv, 0.1f, r.f, r.hi, r.lo,
+                                        relu ? 1 : 0, y.pos(), y.Cs, y.C, (pair && out_use == 2) ? nullptr : y.p, pb.hi, pb.lo,
+                                        e->bn_counter, (nrgbd_stream_t)e->st));
+  y.pair_only = pair && out_use == 2;
+  if (pair) e->pairs[y.p] = pb;
   return y;
 }
 
@@ -560,48 +538,25 @@ Act basic_block(Eng* e, Act& x, const std::string& pre, int planes, int stride, 
   // Fused form (3xTF32 path): conv1 leaves its RAW output and per-channel sums; BN1 + ReLU are applied by conv2 while it
   // splits its operands (nrgbd_conv_nhwc_tc2_bn_in) - one read + one write of the activation less per block.
   Act probe = x; probe.C = planes; probe.Cs = pad32(planes);
-  const bool fused = e->fuse_bn && takes_tc2(e, x, planes) && takes_tc2(e, probe, planes);
+  const bool fused = takes_tc2(e, x, planes) && takes_tc2(e, probe, planes);
   Act t;
-  if (fused) t = conv(e, x, pre + ".conv1.0.0.weight", planes, 1, 3, stride, p1, dil, nullptr, false, true, nullptr, 0, -1, e->stats_b);
-  else t = convbn(e, x, pre + ".conv1.0", planes, 1, 3, stride, 1, dil, true, nullptr, 2);
+  if (fused) {
+    ConvOut raw; raw.stats = e->stats_b;
+    t = conv(e, x, pre + ".conv1.0.0.weight", planes, 1, 3, stride, p1, dil, nullptr, false, true, raw);
+  } else {
+    t = convbn(e, x, pre + ".conv1.0", planes, 1, 3, stride, 1, dil, true, nullptr, 2);
+  }
   Act sc; const Act* res = &x;
-  const float* down_eval = down ? eval_coef(e, pre + ".downsample.1") : nullptr;
-  if (down_eval) {
-    sc = convbn_eval(e, x, pre + ".downsample.0.weight", planes, 1, 1, stride, 0, 1, false, nullptr, 0, down_eval);
-    res = &sc;
-  } else if (down) {
-    // downsample = Sequential(Conv2d 1x1 stride, BatchNorm2d) :125-131 -> names downsample.0 / downsample.1
-    sc = conv(e, x, pre + ".downsample.0.weight", planes, 1, 1, stride, 0, 1, nullptr, false, true);
-    float* g = param(e, pre + ".downsample.1.weight"); float* b = param(e, pre + ".downsample.1.bias");
-    float* rm = e->bn_update_running ? param_opt(e, pre + ".downsample.1.running_mean") : nullptr;
-    float* rv = e->bn_update_running ? param_opt(e, pre + ".downsample.1.running_var") : nullptr;
-    if (!e->rc) {
-      if (pair_mode(e))
-        ENG_CALL(e, nrgbd_bn_apply_stats_pair(sc.p, e->stats, (double)sc.pos(), g, b, 1e-5f, rm && rv ? rm : nullptr, rm && rv ? rv : nullptr,
-                                              0.1f, nullptr, nullptr, nullptr, 0, sc.pos(), sc.Cs, sc.C, sc.p, nullptr, nullptr, e->bn_counter,
-                                              (nrgbd_stream_t)e->st));
-      else
-      ENG_CALL(e, nrgbd_bn_apply_stats(sc.p, e->stats, (double)sc.pos(), g, b, 1e-5f, rm && rv ? rm : nullptr, rm && rv ? rv : nullptr,
-                                       0.1f, nullptr, 0, sc.pos(), sc.Cs, sc.C, sc.p, (nrgbd_stream_t)e->st));
-    }
+  if (down) {      // downsample = Sequential(Conv2d 1x1 stride, BatchNorm2d) :125-131
+    sc = convbn(e, x, pre + ".downsample", planes, 1, 1, stride, 0, 1, false, nullptr);
     res = &sc;
   }
   Act o;
   if (fused) {
-    nrgbd_bn_input bn;
-    bn.stats = e->stats_b; bn.count = (double)t.pos();
-    bn.gamma = param(e, pre + ".conv1.0.1.weight"); bn.beta = param(e, pre + ".conv1.0.1.bias");
-    bn.running_mean = e->bn_update_running ? param_opt(e, pre + ".conv1.0.1.running_mean") : nullptr;
-    bn.running_var = e->bn_update_running ? param_opt(e, pre + ".conv1.0.1.running_var") : nullptr;
-    bn.eps = 1e-5f; bn.momentum = 0.1f; bn.relu = 1; bn.C = planes;
-    o = conv(e, t, pre + ".conv2.0.weight", planes, 1, 3, 1, p1, dil, nullptr, false, true, nullptr, 0, -1, e->stats, &bn);
-    float* g = param(e, pre + ".conv2.1.weight"); float* b = param(e, pre + ".conv2.1.bias");
-    float* rm = e->bn_update_running ? param_opt(e, pre + ".conv2.1.running_mean") : nullptr;
-    float* rv = e->bn_update_running ? param_opt(e, pre + ".conv2.1.running_var") : nullptr;
-    if (!e->rc) {
-      ENG_CALL(e, nrgbd_bn_apply_stats(o.p, e->stats, (double)o.pos(), g, b, 1e-5f, rm && rv ? rm : nullptr, rm && rv ? rv : nullptr,
-                                       0.1f, res->p, 0, o.pos(), o.Cs, o.C, o.p, (nrgbd_stream_t)e->st));
-    }
+    const nrgbd_bn_input bn = bn_input(e, pre + ".conv1.0.1", e->stats_b, t);
+    ConvOut bn_in; bn_in.in_bn = &bn;
+    o = conv(e, t, pre + ".conv2.0.weight", planes, 1, 3, 1, p1, dil, nullptr, false, true, bn_in);
+    bn_train(e, o, pre + ".conv2.1", e->stats, res->p, false);
   } else {
     // a block output that exists only as a pair is the residual of the next block (layer1-3 inner blocks, layer3 -> layer4.0)
     o = convbn(e, t, pre + ".conv2", planes, 1, 3, 1, 1, dil, false, res, fp32_out ? 1 : 2, true);
@@ -630,30 +585,18 @@ void feature_cnn(Eng* e, const Act& x0, Act& l1_out, Act& feat_out) {
   // operand split of the conv that consumes them (the raw 5x240x320x32 tensors are read once instead of read+written+read).
   Act c;
   Act probe32 = x0; probe32.C = 32; probe32.Cs = pad32(32); probe32.H = (x0.H + 2 - 3) / 2 + 1; probe32.W = (x0.W + 2 - 3) / 2 + 1;
-  if (e->fuse_bn && takes_tc2(e, probe32, 32)) {
-    auto bn_of = [&](const std::string& pre, double* stats, const Act& t) {
-      nrgbd_bn_input bn;
-      bn.stats = stats; bn.count = (double)t.pos();
-      bn.gamma = param(e, pre + ".1.weight"); bn.beta = param(e, pre + ".1.bias");
-      bn.running_mean = e->bn_update_running ? param_opt(e, pre + ".1.running_mean") : nullptr;
-      bn.running_var = e->bn_update_running ? param_opt(e, pre + ".1.running_var") : nullptr;
-      bn.eps = 1e-5f; bn.momentum = 0.1f; bn.relu = 1; bn.C = 32;
-      return bn;
-    };
-    Act a = conv(e, x0, P + ".firstconv.0.0.weight", 32, 1, 3, 2, 1, 1, nullptr, false, true, nullptr, 0, pad32(32), e->stats_b);
-    nrgbd_bn_input bn_a = bn_of(P + ".firstconv.0", e->stats_b, a);
-    Act b = conv(e, a, P + ".firstconv.2.0.weight", 32, 1, 3, 1, 1, 1, nullptr, false, true, nullptr, 0, -1, e->stats, &bn_a);
+  if (takes_tc2(e, probe32, 32)) {
+    ConvOut oa; oa.Cs = pad32(32); oa.stats = e->stats_b;
+    Act a = conv(e, x0, P + ".firstconv.0.0.weight", 32, 1, 3, 2, 1, 1, nullptr, false, true, oa);
+    const nrgbd_bn_input bn_a = bn_input(e, P + ".firstconv.0.1", e->stats_b, a);
+    ConvOut ob; ob.in_bn = &bn_a;
+    Act b = conv(e, a, P + ".firstconv.2.0.weight", 32, 1, 3, 1, 1, 1, nullptr, false, true, ob);
     release(e, a);
-    nrgbd_bn_input bn_b = bn_of(P + ".firstconv.2", e->stats, b);
-    c = conv(e, b, P + ".firstconv.4.0.weight", 32, 1, 3, 1, 1, 1, nullptr, false, true, nullptr, 0, -1, e->stats_b, &bn_b);
+    const nrgbd_bn_input bn_b = bn_input(e, P + ".firstconv.2.1", e->stats, b);
+    ConvOut oc; oc.stats = e->stats_b; oc.in_bn = &bn_b;
+    c = conv(e, b, P + ".firstconv.4.0.weight", 32, 1, 3, 1, 1, 1, nullptr, false, true, oc);
     release(e, b);
-    float* g = param(e, P + ".firstconv.4.1.weight"); float* bb = param(e, P + ".firstconv.4.1.bias");
-    float* rm = e->bn_update_running ? param_opt(e, P + ".firstconv.4.1.running_mean") : nullptr;
-    float* rv = e->bn_update_running ? param_opt(e, P + ".firstconv.4.1.running_var") : nullptr;
-    if (!e->rc) {
-      ENG_CALL(e, nrgbd_bn_apply_stats(c.p, e->stats_b, (double)c.pos(), g, bb, 1e-5f, rm && rv ? rm : nullptr, rm && rv ? rv : nullptr,
-                                       0.1f, nullptr, 1, c.pos(), c.Cs, c.C, c.p, (nrgbd_stream_t)e->st));
-    }
+    bn_train(e, c, P + ".firstconv.4.1", e->stats_b, nullptr, true);
   } else {
     Act a = convbn(e, x0, P + ".firstconv.0", 32, 1, 3, 2, 1, 1, true, nullptr, 2);
     Act b = convbn(e, a, P + ".firstconv.2", 32, 1, 3, 1, 1, 1, true, nullptr, 2); release(e, a);
@@ -701,7 +644,8 @@ void feature_cnn(Eng* e, const Act& x0, Act& l1_out, Act& feat_out) {
   release(e, raw); release(e, skip);
   Act lc = convbn(e, cat, P + ".lastconv.0", 128, 1, 3, 1, 1, 1, true, nullptr, 2);
   release(e, cat);
-  feat_out = conv(e, lc, P + ".lastconv.2.weight", e->F, 1, 1, 1, 0, 1, nullptr, false, false, nullptr, 0, pad4(e->F));   // dense: the sweep's wide layout
+  ConvOut dense; dense.Cs = pad4(e->F);                              // the sweep's wide layout
+  feat_out = conv(e, lc, P + ".lastconv.2.weight", e->F, 1, 1, 1, 0, 1, nullptr, false, false, dense);
   release(e, lc);
   l1_out = l1;
 }
@@ -711,39 +655,37 @@ void conv_transpose(Eng* e, const Act& x, const std::string& wname, const char* 
   float* tb = param(e, bias_name);
   if (e->rc) return;
   nrgbd_stream_t st = (nrgbd_stream_t)e->st;
-  const double flops = 2.0 * 4.0 * (double)x.H * x.W * Cout * x.C * 4;
-  char tag[56];
-  snprintf(tag, sizeof(tag), "convT k4 s2 %d->%d %dx%dx%d", x.C, Cout, x.N, 2 * x.H, 2 * x.W);
+  const ConvGeom g = conv_geom(x, Cout, 1, 4, 2, 1, 1, true);
   if (use_h2(e, x)) {
-    const PackedH2* ph = packw_h2(e, wname, Cout, x.C, 16, true);
+    const Packed* ph = packw(e, wname, PK_H2, Cout, x.C, 16, true);
     const PairBuf* pb = pair_of(e, x);
     if (e->rc) return;
-    ProfScope ps(e, 0, flops, tag);
+    ProfScope ps(e, 0, g.flops, g.tag);
     ENG_CALL(e, nrgbd_conv_transpose2d_k4s2_nhwc_h2(pb->hi, conv_lo(e, pb), x.N, x.H, x.W, ph->Cin_pad, x.Cs, ph->w, tb, Cout, ph->Cout_pad, ph->BN,
                                                     dst.p, dst.Cs, 0, 1, st));
     return;
   }
   if (use_tc(e, x, Cout)) {
-    const PackedTc* pt = packw_tc(e, wname, Cout, x.C, 16, true);
+    const Packed* pt = packw(e, wname, PK_TC, Cout, x.C, 16, true);
     if (!e->rc && nrgbd_conv_tc2_supported(pt->Cin_pad, pt->Cout_pad)) {
-      ProfScope ps(e, 0, flops, tag);
-      ENG_CALL(e, nrgbd_conv_transpose2d_k4s2_nhwc_tc2(x.p, x.N, x.H, x.W, pt->Cin_pad, x.Cs, pt->hi, pt->lo, tb, Cout, pt->Cout_pad,
+      ProfScope ps(e, 0, g.flops, g.tag);
+      ENG_CALL(e, nrgbd_conv_transpose2d_k4s2_nhwc_tc2(x.p, x.N, x.H, x.W, pt->Cin_pad, x.Cs, pt->w, pt->lo, tb, Cout, pt->Cout_pad,
                                                        dst.p, dst.Cs, 0, 1, st));
       return;
     }
     Act xh, xl;
     split_act(e, x, xh, xl);
     if (!e->rc) {
-      ProfScope ps(e, 0, flops, tag);
-      ENG_CALL(e, nrgbd_conv_transpose2d_k4s2_nhwc_tc(xh.p, xl.p, x.N, x.H, x.W, pt->Cin_pad, x.Cs, pt->hi, pt->lo, tb, Cout, pt->Cout_pad,
+      ProfScope ps(e, 0, g.flops, g.tag);
+      ENG_CALL(e, nrgbd_conv_transpose2d_k4s2_nhwc_tc(xh.p, xl.p, x.N, x.H, x.W, pt->Cin_pad, x.Cs, pt->w, pt->lo, tb, Cout, pt->Cout_pad,
                                                       dst.p, dst.Cs, 0, 1, st));
     }
     release(e, xh); release(e, xl);
     return;
   }
-  const Packed* pk = packw(e, wname, Cout, x.C, 16, true);
+  const Packed* pk = packw(e, wname, PK_F32, Cout, x.C, 16, true);
   if (e->rc) return;
-  ProfScope ps(e, 0, flops, tag);
+  ProfScope ps(e, 0, g.flops, g.tag);
   ENG_CALL(e, nrgbd_conv_transpose2d_k4s2_nhwc(x.p, x.N, x.H, x.W, pk->Cin_pad, x.Cs, pk->w, tb, Cout, pk->Cout_pad, dst.p, dst.Cs, 0, 1, st));
 }
 
@@ -759,21 +701,23 @@ void r_net(Eng* e, const float* bv_hwd, const float* feat_ref, int feat_Cs, cons
     ENG_CALL(e, nrgbd_copy_channels(bv_hwd, hw, D, 0, D, 1, in0.p, in0.Cs, 0, st));           // torch.exp(BV)
     ENG_CALL(e, nrgbd_copy_channels(feat_ref, hw, feat_Cs, 0, F, 0, in0.p, in0.Cs, D, st));
   }
-  Act a = conv(e, in0, "r_net.conv0.0.weight", D + F, 1, 3, 1, 1, 1, "r_net.conv0.0.bias", true, false, nullptr, 0, -1, nullptr, nullptr, true); release(e, in0);
-  Act b = conv(e, a, "r_net.conv0_1.0.weight", D + F, 1, 3, 1, 1, 1, "r_net.conv0_1.0.bias", true, false, nullptr, 0, -1, nullptr, nullptr, true); release(e, a);
+  ConvOut pair; pair.pair_only = true;          // conv0 ... conv2_1: each one's only reader is the next convolution
+  Act a = conv(e, in0, "r_net.conv0.0.weight", D + F, 1, 3, 1, 1, 1, "r_net.conv0.0.bias", true, false, pair); release(e, in0);
+  Act b = conv(e, a, "r_net.conv0_1.0.weight", D + F, 1, 3, 1, 1, 1, "r_net.conv0_1.0.bias", true, false, pair); release(e, a);
   Act t0 = acquire(e, 1, 1, 2 * h, 2 * w, D0 + F / 2);
   conv_transpose(e, b, "r_net.trans_conv0.0.weight", "r_net.trans_conv0.0.bias", D0, t0);
   if (!e->rc) ENG_CALL(e, nrgbd_copy_channels(l1_ref, 4 * hw, l1_Cs, 0, F / 2, 0, t0.p, t0.Cs, D0, st));
   release(e, b);
-  Act c = conv(e, t0, "r_net.conv1.0.weight", D0 + F / 2, 1, 3, 1, 1, 1, "r_net.conv1.0.bias", true, false, nullptr, 0, -1, nullptr, nullptr, true); release(e, t0);
-  Act d = conv(e, c, "r_net.conv1_1.0.weight", D0 + F / 2, 1, 3, 1, 1, 1, "r_net.conv1_1.0.bias", true, false, nullptr, 0, -1, nullptr, nullptr, true); release(e, c);
+  Act c = conv(e, t0, "r_net.conv1.0.weight", D0 + F / 2, 1, 3, 1, 1, 1, "r_net.conv1.0.bias", true, false, pair); release(e, t0);
+  Act d = conv(e, c, "r_net.conv1_1.0.weight", D0 + F / 2, 1, 3, 1, 1, 1, "r_net.conv1_1.0.bias", true, false, pair); release(e, c);
   Act t1 = acquire(e, 1, 1, H, W, D1 + 3);
   conv_transpose(e, d, "r_net.trans_conv1.0.weight", "r_net.trans_conv1.0.bias", D1, t1);
   if (!e->rc) ENG_CALL(e, nrgbd_copy_channels(frame_ref.p, (long long)H * W, frame_ref.Cs, 0, 3, 0, t1.p, t1.Cs, D1, st));
   release(e, d);
-  Act f = conv(e, t1, "r_net.conv2.0.weight", D1 + 3, 1, 3, 1, 1, 1, "r_net.conv2.0.bias", true, false, nullptr, 0, -1, nullptr, nullptr, true); release(e, t1);
-  Act g = conv(e, f, "r_net.conv2_1.0.weight", D1, 1, 3, 1, 1, 1, "r_net.conv2_1.0.bias", true, false, nullptr, 0, -1, nullptr, nullptr, true); release(e, f);
-  conv(e, g, "r_net.conv2_2.weight", D1, 1, 3, 1, 1, 1, "r_net.conv2_2.bias", false, false, &out, 0, D1); release(e, g);
+  Act f = conv(e, t1, "r_net.conv2.0.weight", D1 + 3, 1, 3, 1, 1, 1, "r_net.conv2.0.bias", true, false, pair); release(e, t1);
+  Act g = conv(e, f, "r_net.conv2_1.0.weight", D1, 1, 3, 1, 1, 1, "r_net.conv2_1.0.bias", true, false, pair); release(e, f);
+  ConvOut into_out; into_out.dst = &out;
+  conv(e, g, "r_net.conv2_2.weight", D1, 1, 3, 1, 1, 1, "r_net.conv2_2.bias", false, false, into_out); release(e, g);
   // F.log_softmax(conv2_2_out, dim=1): channels are contiguous per pixel (Cs == D1); above 256 planes dpv_normalize takes
   // its thread-per-pixel path
   if (!e->rc)
@@ -822,7 +766,7 @@ Act kv_net(Eng* e, const Act& vol) {
   if (use_h2(e, o)) {
     // Conv3d(f -> 1, k3) (models/basic.py:136-137) as a pointwise conv to 27 per-tap channels on the tensor cores + the shifted
     // sum of the taps: as a direct implicit GEMM its N is 1 (27 x 12 sixteen-column MMAs per 128 positions, issue-bound)
-    const PackedH2* ph = packw_h2_taps(e, "kv_net.classify.2.weight", o.C, 27);
+    const Packed* ph = packw(e, "kv_net.classify.2.weight", PK_H2_TAPS, 27, o.C, 1, true);
     const PairBuf* pb = pair_of(e, o);
     Act q; q.N = o.N; q.D = o.D; q.H = o.H; q.W = o.W; q.C = 27; q.Cs = 28; q.p = nullptr;
     gain = acquire(e, o.N, o.D, o.H, o.W, 1, 1);
@@ -840,7 +784,8 @@ Act kv_net(Eng* e, const Act& vol) {
     }
     if (q.p) e->pool.release(q.p);
   } else {
-    gain = conv(e, o, "kv_net.classify.2.weight", 1, 3, 3, 1, 1, 1, nullptr, false, false, nullptr, 0, 1);
+    ConvOut dense; dense.Cs = 1;
+    gain = conv(e, o, "kv_net.classify.2.weight", 1, 3, 3, 1, 1, 1, nullptr, false, false, dense);
   }
   release(e, o);
   return gain;
@@ -885,8 +830,6 @@ int nrgbd_kvnet_create(int H, int W, int D, int V, int feature_dim, int kv_featu
   bool ok = cudaMalloc((void**)&e->stats, sizeof(double) * 2 * 512) == cudaSuccess &&
             cudaMalloc((void**)&e->stats_b, sizeof(double) * 2 * 512) == cudaSuccess &&
             cudaMalloc((void**)&e->bn_counter, sizeof(unsigned int)) == cudaSuccess &&
-            cudaMalloc((void**)&e->scale, sizeof(float) * 512) == cudaSuccess &&
-            cudaMalloc((void**)&e->shift, sizeof(float) * 512) == cudaSuccess &&
             cudaMalloc((void**)&e->eval_coef, sizeof(float) * 1024 * NRGBD_BN_EVAL_MAX) == cudaSuccess &&
             cudaMalloc((void**)&e->ws_sweep, sizeof(float) * 12 * V) == cudaSuccess &&
             cudaMalloc((void**)&e->bv_cur_hwd, sizeof(float) * hw * D) == cudaSuccess &&
@@ -903,11 +846,9 @@ int nrgbd_kvnet_create(int H, int W, int D, int V, int feature_dim, int kv_featu
 int nrgbd_kvnet_destroy(nrgbd_kvnet* e) {
   if (!e) return NRGBD_OK;
   for (auto& kv : e->params) if (kv.second.owned) cudaFree(kv.second.p);
-  for (auto& kv : e->packed) cudaFree(kv.second.w);
-  for (auto& kv : e->packed_tc) { cudaFree(kv.second.hi); cudaFree(kv.second.lo); }
-  for (auto& kv : e->packed_h2) cudaFree(kv.second.w);
+  for (auto& kv : e->packed) free_packed(kv.second);
   for (int i = 0; i < 2; ++i) { cudaFree(e->cam[i].K); cudaFree(e->cam[i].rays); }
-  cudaFree(e->d_planes); cudaFree(e->stats); cudaFree(e->stats_b); cudaFree(e->bn_counter); cudaFree(e->scale); cudaFree(e->shift); cudaFree(e->eval_coef); cudaFree(e->ws_sweep);
+  cudaFree(e->d_planes); cudaFree(e->stats); cudaFree(e->stats_b); cudaFree(e->bn_counter); cudaFree(e->eval_coef); cudaFree(e->ws_sweep);
   cudaFree(e->bv_cur_hwd); cudaFree(e->dpv_hwd); cudaFree(e->prior_hwd); cudaFree(e->depth); cudaFree(e->conf);
   cudaFree(e->x0_buf); cudaFree(e->rt_buf); cudaFree(e->ref_cur_hwd); cudaFree(e->ref_kv_hwd);
   drop_graphs(e);
@@ -920,7 +861,7 @@ int nrgbd_kvnet_destroy(nrgbd_kvnet* e) {
 
 // Register a parameter under its reference state_dict name. is_device != 0: `data` is a device
 // pointer the engine borrows (must outlive the engine or be re-set); else a host array that is copied.
-// Setting a conv weight again invalidates its packed copy.
+// Setting a conv weight again drops every packed copy of it.
 int nrgbd_kvnet_set_param(nrgbd_kvnet* e, const char* name, const float* data, long long n, int is_device) {
   NRGBD_REQUIRE(e && name && data && n > 0, "bad arguments");
   drop_graphs(e);
@@ -934,11 +875,7 @@ int nrgbd_kvnet_set_param(nrgbd_kvnet* e, const char* name, const float* data, l
     e->params.erase(it);
   }
   auto pk = e->packed.find(key);
-  if (pk != e->packed.end()) { cudaFree(pk->second.w); e->packed.erase(pk); }
-  auto pt = e->packed_tc.find(key);
-  if (pt != e->packed_tc.end()) { cudaFree(pt->second.hi); cudaFree(pt->second.lo); e->packed_tc.erase(pt); }
-  auto p2 = e->packed_h2.find(key);
-  if (p2 != e->packed_h2.end()) { cudaFree(p2->second.w); e->packed_h2.erase(p2); }
+  if (pk != e->packed.end()) { free_packed(pk->second); e->packed.erase(pk); }
   ParamRef r; r.n = n; r.owned = !is_device;
   if (is_device) {
     r.p = const_cast<float*>(data);
@@ -986,7 +923,6 @@ int nrgbd_kvnet_set_option(nrgbd_kvnet* e, const char* key, int value) {
   if (k == "bn_update_running") { drop_graphs(e); e->bn_update_running = value; return NRGBD_OK; }
   if (k == "profile") { e->profile = value; return NRGBD_OK; }
   if (k == "bn_eval") { drop_graphs(e); e->bn_eval = value ? 1 : 0; return NRGBD_OK; }
-  if (k == "fuse_bn") { if (e->fuse_bn != value) drop_graphs(e); e->fuse_bn = value; return NRGBD_OK; }
   if (k == "use_graph") { drop_graphs(e); e->use_graph = value; return NRGBD_OK; }
   if (k == "refine") {               // 0: DPV R-Net (default); 1: guided filter (DGF); 2: none
     if (value < 0 || value > 2) { nrgbd_set_error("refine must be 0 (DPV), 1 (DGF) or 2 (none)"); return NRGBD_ERR_BAD_ARG; }
@@ -1241,17 +1177,10 @@ static int forward_core(nrgbd_kvnet* e, bool steady, bool need_cur_refined, bool
       // vol.p is only the key of the pair buffers (a 16-byte block). dres0.0 decides its path by the same use_h2(vol),
       // so it reads the pair: CK = 10 (t_win_r = 1) runs at Cin_pad = 32 like CK = 16 and 28. The row kernel stores
       // 32 channels, the zeros [CK, 32) included.
-      vol.pair_only = true;
-      vol.p = e->pool.acquire(16);
       PairBuf pb;
-      pb.hi = e->pool.acquire((size_t)vol.floats() * 2);
-      pb.lo = keep_lo(e, false) ? e->pool.acquire((size_t)vol.floats() * 2) : nullptr;
-      if (!vol.p || !pb.hi || (!pb.lo && keep_lo(e, false))) { if (!e->rc) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; } }
-      else {
-        ENG_CALL(e, nrgbd_knet_input_volume_pair(rgbq.p, rgbq.p + (size_t)V * hw * 4, e->bv_cur_hwd, e->prior_hwd, V, D, h, w, vol.Cs,
-                                                 c1.K, Rs, ts, c1.rays, e->d_planes, c1.cx, c1.cy, e->ws_sweep, nullptr, pb.hi, pb.lo, st));
-        e->pairs[vol.p] = pb;
-      }
+      vol = pair_act(e, 1, D, h, w, CK, false, pb);
+      ENG_CALL(e, nrgbd_knet_input_volume_pair(rgbq.p, rgbq.p + (size_t)V * hw * 4, e->bv_cur_hwd, e->prior_hwd, V, D, h, w, vol.Cs,
+                                               c1.K, Rs, ts, c1.rays, e->d_planes, c1.cx, c1.cy, e->ws_sweep, nullptr, pb.hi, pb.lo, st));
     } else {
       vol = acquire(e, 1, D, h, w, CK);
       ENG_CALL(e, nrgbd_knet_input_volume(rgbq.p, rgbq.p + (size_t)V * hw * 4, e->bv_cur_hwd, e->prior_hwd, V, D, h, w, vol.Cs,

@@ -199,6 +199,35 @@ def test_kvnet_vs_oracle_first_window(conv_math):
     assert maxabs(np.exp(got[0].cpu().numpy()), np.exp(orc[0])) <= 1e-4
 
 
+@pytest.mark.parametrize('conv_math', ['fp32', 'tf32x3', 'f16x3', 'f16'])
+def test_kvnet_load_state_dict_after_forward(conv_math):
+    """New weights loaded into a module whose engine has run reach every packed copy of them: the next K-Net step
+    matches a fresh module built with those weights (the f16 modes keep K-Net's last layer in a second, per-tap packing)."""
+    c = cases.kvnet_case('kvnet_256_d16')
+    cam = cam_torch(cases.cam_for(O.make_cam_intrinsics, c['W'] // 4, c['H'] // 4))
+    rng = np.random.RandomState(11)
+    sd_b = {k: (v * (1 + 0.1 * rng.standard_normal(v.shape))).astype(v.dtype) if v.dtype.kind == 'f' else v
+            for k, v in ((k, np.asarray(v)) for k, v in c['sd'].items())}
+    ref_f, src_f, poses = cases.window(c, 2)
+
+    def dpv(m, prior):
+        with torch.no_grad():
+            return m(T(ref_f), T(src_f), T(poses), torch.zeros(1), cam_intrinsics=[cam], BV_predict=prior)[3]
+    model = build_model(c, cam)
+    model.conv_math = conv_math
+    prior = dpv(model, None).clone()                 # first window with state dict A
+    before = dpv(model, prior).cpu().numpy()         # K-Net step with A
+    model.load_state_dict({k: torch.from_numpy(v) for k, v in sd_b.items()})
+    got = dpv(model, prior).cpu().numpy()
+    fresh = build_model(dict(c, sd=sd_b), cam)
+    fresh.conv_math = conv_math
+    want = dpv(fresh, prior).cpu().numpy()
+    # two identical modules agree to the rounding of the BatchNorm sums' double-precision atomics, far below the K-Net gate
+    # (5e-4); the change of weights moves the DPV by far more
+    assert maxabs(np.exp(got), np.exp(want)) <= 1e-5
+    assert maxabs(np.exp(before), np.exp(want)) > 1e-3
+
+
 def test_engine_rejects_bad_shapes():
     from neuralrgbd_b200 import _lib
     import ctypes
