@@ -428,6 +428,28 @@ int nrgbd_guided_filter_refine(const float* dmap, int h, int w, const float* img
                                int H, int W, const float* w0, const float* b0, const float* w1, const float* b1,
                                int r, float eps, float* ws, float* out, nrgbd_stream_t stream);
 
+/* ---- models/GF BoxFilter(r) and GuidedFilter(r, eps) on N x C x H x W fp32 planes, forward and backward (the autograd
+ * mirrors neuralrgbd_b200.models.GF). Box sums use the reference's cumulative-sum form: prefixes accumulated in double
+ * and rounded to fp32 at every position, then box_filter.py's differences; every other forward step is one fp32
+ * operation in the reference's order. The backwards follow autograd's order through guided_filter.py / box_filter.py
+ * (the diff's slice / cat adjoint, then a reverse prefix sum). No atomics: identical results from run to run.
+ * BoxFilter: x, out, grad_out, grad_x are N x C x H x W; H, W >= 2r + 1; ws holds
+ * nrgbd_box_filter_workspace_floats(N, C, H, W) floats. */
+long long nrgbd_box_filter_workspace_floats(int N, int C, int H, int W);
+int nrgbd_box_filter(const float* x, int N, int C, int H, int W, int r, float* ws, float* out, nrgbd_stream_t stream);
+int nrgbd_box_filter_backward(const float* grad_out, int N, int C, int H, int W, int r, float* ws, float* grad_x,
+                              nrgbd_stream_t stream);
+/* GuidedFilter: x is N x Cx x H x W (Cx = 1 broadcasts over y's channels, or Cx = Cy), y, out and grad_out are
+ * N x Cy x H x W; H, W > 2r + 1. ws: nrgbd_gf_workspace_floats(N, Cx, Cy, H, W, backward) floats. The backward recomputes
+ * the forward's box sums from x and y; grad_x (N x Cx x H x W, summed over y's channels when Cx = 1) and grad_y
+ * (N x Cy x H x W) may each be NULL. */
+long long nrgbd_gf_workspace_floats(int N, int Cx, int Cy, int H, int W, int backward);
+int nrgbd_guided_filter(const float* x, const float* y, int N, int Cx, int Cy, int H, int W, int r, float eps, float* ws,
+                        float* out, nrgbd_stream_t stream);
+int nrgbd_guided_filter_backward(const float* grad_out, const float* x, const float* y, int N, int Cx, int Cy, int H,
+                                 int W, int r, float eps, float* ws, float* grad_x, float* grad_y,
+                                 nrgbd_stream_t stream);
+
 /* ---- a4, a6: whole-frame engine -------------------------------------------------------------
  * replaces models/KVNET.py:35-185 (KVNET.__init__/forward with if_refined=True, refineNet_name='DPV')
  * + models/basic.py:223-323 (D_NET_BASIC.forward) + the DPV propagation of

@@ -17,10 +17,13 @@ _PATCHES = (
       'back_warp_th_Rt', 'back_warp_th_Rt_msrc')),
     ('mutils.misc', 'neuralrgbd_b200.mutils.misc', ('depth_val_regression', 'depth_var', 'dpv_statistics', 'valid_dpv')),
     ('models.KVNET', 'neuralrgbd_b200.models.KVNET', ('KVNET',)),
+    ('models.GF.guided_filter', 'neuralrgbd_b200.models.GF.guided_filter', ('GuidedFilter',)),
+    ('models.GF.box_filter', 'neuralrgbd_b200.models.GF.box_filter', ('BoxFilter',)),
     ('ICP.opt_pose_numerical', 'neuralrgbd_b200.ICP.opt_pose_numerical', ('local_BA_direct', 'local_BA_direct_parallel')),
 )
-# packages a checkout may lack (the LBA pose optimiser): without one, only its patch is skipped
-_OPTIONAL = ('ICP',)
+# directories a checkout may lack (the LBA pose optimiser, the guided filter): without one, only the patches of the
+# modules inside it are skipped
+_OPTIONAL = ('ICP', 'models/GF')
 
 
 def install_as_reference_modules(reference_code_dir=None):
@@ -29,7 +32,8 @@ def install_as_reference_modules(reference_code_dir=None):
     reference_code_dir: the `code/` directory of an NVlabs/neuralrgbd checkout (e.g. $NRGBD_REFERENCE_CODE). It is put on
     sys.path and the reference's OWN modules are imported; then the mirrored functions / classes are set as
     attributes on them (`warping.homography.est_swp_volume_v4`, `warp_img_feats_v3`, `warp_img_feats_mgpu`,
-    `resample_vol_cuda`, `mutils.misc.depth_val_regression`, `models.KVNET.KVNET`, ...). Everything else the reference
+    `resample_vol_cuda`, `mutils.misc.depth_val_regression`, `models.KVNET.KVNET`, `models.GF.guided_filter.GuidedFilter`,
+    ...). A reference `RefineNet_DGF` built afterwards carries the mirror GuidedFilter. Everything else the reference
     modules define (`warping.View`, `mutils.misc.get_entries_list_dict`, `m_makedir`, `save_ScenePathInfo`, the
     data loaders' imports) keeps working, because the packages are not replaced.  The unmodified
     `test_utils/test_KVNet.py:test` looks both `warp_homo.resample_vol_cuda` and `model_KV(...)` up at call time,
@@ -39,7 +43,8 @@ def install_as_reference_modules(reference_code_dir=None):
     registered under the reference's names - enough for code that only needs the mirrored symbols.
 
     `ICP.opt_pose_numerical.local_BA_direct(_parallel)` (the LBA pose optimiser) is patched too when the checkout has an
-    `ICP` package; a checkout without one skips only that patch.
+    `ICP` package, and `models.GF.guided_filter.GuidedFilter` / `models.GF.box_filter.BoxFilter` when it has `models/GF`;
+    a checkout without one skips only those patches.
 
     Returns a namespace with the patched (or registered) modules (`opt_pose_numerical` is None when that patch was
     skipped) and `patched`: {module: [symbols]}.
@@ -53,8 +58,9 @@ def install_as_reference_modules(reference_code_dir=None):
     mods, patched = {}, {}
     for ref_name, mirror_name, symbols in _PATCHES:
         pkg_name = ref_name.split('.')[0]
-        if (pkg_name in _OPTIONAL and reference_code_dir is not None
-                and not os.path.isdir(os.path.join(reference_code_dir, pkg_name))):
+        if reference_code_dir is not None and any(
+                (ref_name.replace('.', '/') + '/').startswith(d + '/')
+                and not os.path.isdir(os.path.join(reference_code_dir, *d.split('/'))) for d in _OPTIONAL):
             continue
         mirror = importlib.import_module(mirror_name)
         ref_mod = sys.modules.get(ref_name)

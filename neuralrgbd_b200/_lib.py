@@ -100,6 +100,13 @@ SIGNATURES = {
     'nrgbd_guided_filter_workspace_floats': (c_ll, [c_int, c_int]),
     'nrgbd_guided_filter_refine': (c_int, [c_vp, c_int, c_int, c_vp, c_ll, c_ll, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_int,
                                            c_float, c_vp, c_vp, c_vp]),
+    'nrgbd_box_filter_workspace_floats': (c_ll, [c_int, c_int, c_int, c_int]),
+    'nrgbd_box_filter': (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
+    'nrgbd_box_filter_backward': (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
+    'nrgbd_gf_workspace_floats': (c_ll, [c_int, c_int, c_int, c_int, c_int, c_int]),
+    'nrgbd_guided_filter': (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_vp, c_vp, c_vp]),
+    'nrgbd_guided_filter_backward': (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_vp,
+                                             c_vp, c_vp, c_vp]),
     'nrgbd_plane_sweep_backward_packed': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp,
                                                   c_vp, c_vp, c_float, c_float, c_float, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     'nrgbd_unpack_features': (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp]),
