@@ -319,7 +319,15 @@ int nrgbd_bn_apply(const float* x, const float* scale, const float* shift, const
  * (nrgbd_split_tf32, nrgbd_pack_conv_weight_tc -> [taps][Cout_pad][Cin_pad]). Semantics otherwise
  * identical to nrgbd_conv_nhwc / nrgbd_conv_transpose2d_k4s2_nhwc. */
 int nrgbd_conv_tc_supported(int Cin_pad, int Cout_pad);   /* Cin_pad % 32 == 0, Cout_pad % 16 == 0, <= 256 */
-int nrgbd_split_tf32(const float* x, long long n, float* hi, float* lo, nrgbd_stream_t stream);
+/* Activation operands: x channels-last [n_pos][Cs_in] -> hi / lo [n_pos][Cin_pad], hi = RN_tf32(v), lo = RN_tf32(v - hi)
+ * (round to nearest, ties away from zero). Cin_pad % 32 == 0, Cs_in % 4 == 0, C <= Cin_pad <= Cs_in, x / hi / lo 16-byte
+ * aligned. Channels below C: v = x, or, with scale and shift set, v = [relu](fmaf(x, scale[c], shift[c])); channels from C
+ * up to Cin_pad: v = 0. The second form applies a conv's training-mode BatchNorm (+ReLU) to its INPUT while splitting it:
+ * x is the RAW output of the producing conv (psm_submodule.convbn :10-16 = Conv2d + BatchNorm2d, BasicBlock :31-49
+ * conv1 -> bn -> relu -> conv2) and scale / shift [C] come from nrgbd_bn_finalize of that conv's sums, which also updates
+ * the running statistics - the arithmetic of nrgbd_bn_apply_stats without that pass over the tensor. */
+int nrgbd_split_tf32(const float* x, long long n_pos, int Cs_in, int Cin_pad, int C, const float* scale, const float* shift,
+                     int relu, float* hi, float* lo, nrgbd_stream_t stream);
 int nrgbd_pack_conv_weight_tc(const float* w, int transposed, int Cout, int Cin, int taps, int Cin_pad,
                               int Cout_pad, float* hi, float* lo, nrgbd_stream_t stream);
 int nrgbd_conv_nhwc_tc(const float* x_hi, const float* x_lo, int N, int Din, int Hin, int Win, int Cin_pad,
@@ -331,34 +339,6 @@ int nrgbd_conv_transpose2d_k4s2_nhwc_tc(const float* x_hi, const float* x_lo, in
                                         int Cin_pad, int Cs_in, const float* w_hi, const float* w_lo,
                                         const float* bias, int Cout, int Cout_pad, float* y, int Cs_out,
                                         int c_off, int leaky, nrgbd_stream_t stream);
-/* v2 entries: raw fp32 activations (split into TF32 pairs in stream-ordered scratch right before the GEMM),
- * pre-split K-major weights. Cout_pad <= 128. Same semantics as the v1 entries. */
-/* Training-mode BatchNorm (+ReLU) of a conv's INPUT, folded into the operand split of the consuming tensor-core convolution: x is the RAW output
- * of the producing conv (psm_submodule.convbn :10-16 = Conv2d + BatchNorm2d, BasicBlock :31-49 conv1 -> bn -> relu -> conv2)
- * and `stats` its per-channel [sum(C) | sum of squares(C)] as written by the conv entry points. The consumer computes
- * scale = gamma / sqrt(var + eps), shift = beta - mean * scale once and applies fmaf(x, scale, shift) (+ReLU) while it
- * splits its operands - the same arithmetic as nrgbd_bn_apply_stats, without that pass over the tensor. Padding stays
- * zero. running_mean / running_var (optional) get the momentum update once. `stats` must differ from the consumer's own. */
-typedef struct nrgbd_bn_input {
-  const double* stats; double count;            /* [2*C] sums of the producing conv; number of positions N*D*H*W */
-  const float* gamma; const float* beta;        /* BatchNorm weight / bias [C] */
-  float* running_mean; float* running_var;      /* optional [C] */
-  float eps, momentum;
-  int relu, C;
-} nrgbd_bn_input;
-int nrgbd_conv_nhwc_tc2_bn_in(const float* x, int N, int Din, int Hin, int Win, int Cin_pad, int Cs_in, const float* w_hi,
-                              const float* w_lo, const float* bias, int Cout, int Cout_pad, int kd, int kh, int kw,
-                              int stride, int pad, int dilation, float* y, int Hout, int Wout, int Cs_out, int c_off,
-                              int leaky, double* stats, const nrgbd_bn_input* in_bn, nrgbd_stream_t stream);
-int nrgbd_conv_tc2_supported(int Cin_pad, int Cout_pad);
-int nrgbd_conv_nhwc_tc2(const float* x, int N, int Din, int Hin, int Win, int Cin_pad, int Cs_in,
-                        const float* w_hi, const float* w_lo, const float* bias, int Cout, int Cout_pad,
-                        int kd, int kh, int kw, int stride, int pad, int dilation, float* y, int Hout,
-                        int Wout, int Cs_out, int c_off, int leaky, double* stats, nrgbd_stream_t stream);
-int nrgbd_conv_transpose2d_k4s2_nhwc_tc2(const float* x, int N, int Hin, int Win, int Cin_pad, int Cs_in,
-                                         const float* w_hi, const float* w_lo, const float* bias, int Cout,
-                                         int Cout_pad, float* y, int Cs_out, int c_off, int leaky,
-                                         nrgbd_stream_t stream);
 /* Second-generation tensor-core path (csrc/conv_f16.cu): wgmma on SPLIT-FP16 operand pairs, fp32 accumulate.
  * Every fp32 value a is carried as two halves, a = hi + lo * 2^-11 (hi = RN_f16(a), lo = RN_f16((a - hi) * 2^11)), and a
  * product is accumulated as hi*hi + 2^-11 (hi*lo + lo*hi): the 22-bit product of the 3xTF32 path at twice the MMA rate

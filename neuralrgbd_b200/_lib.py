@@ -53,22 +53,13 @@ SIGNATURES = {
     'nrgbd_conv_transpose2d_k4s2_nhwc': (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_int, c_int,
                                                  c_vp, c_int, c_int, c_int, c_vp]),
     'nrgbd_conv_tc_supported': (c_int, [c_int, c_int]),
-    'nrgbd_split_tf32': (c_int, [c_vp, c_ll, c_vp, c_vp, c_vp]),
+    'nrgbd_split_tf32': (c_int, [c_vp, c_ll, c_int, c_int, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_vp]),
     'nrgbd_pack_conv_weight_tc': (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
     'nrgbd_conv_nhwc_tc': (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_int, c_int,
                                    c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp,
                                    c_vp]),
     'nrgbd_conv_transpose2d_k4s2_nhwc_tc': (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_int,
                                                     c_int, c_vp, c_int, c_int, c_int, c_vp]),
-    'nrgbd_conv_tc2_supported': (c_int, [c_int, c_int]),
-    'nrgbd_conv_nhwc_tc2': (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_int, c_int,
-                                    c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp,
-                                    c_vp]),
-    'nrgbd_conv_nhwc_tc2_bn_in': (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_int, c_int,
-                                          c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp,
-                                          c_vp, c_vp]),
-    'nrgbd_conv_transpose2d_k4s2_nhwc_tc2': (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_int,
-                                                     c_int, c_vp, c_int, c_int, c_int, c_vp]),
     'nrgbd_conv_h2_plan': (c_int, [c_int, c_int, ctypes.POINTER(c_int), ctypes.POINTER(c_int), ctypes.POINTER(c_int)]),
     'nrgbd_split_f16_pair': (c_int, [c_vp, c_ll, c_vp, c_vp, c_vp]),
     'nrgbd_pack_conv_weight_h2': (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
@@ -142,12 +133,6 @@ DEV_SIGNATURES = {
     'nrgbd_dev_conv_h2_set_flags': (None, [c_int]),
     'nrgbd_dev_conv_h2_set_smem_cap_kb': (None, [c_int]),
 }
-
-
-class BnInput(ctypes.Structure):
-    """include/nrgbd.h: nrgbd_bn_input."""
-    _fields_ = [('stats', c_vp), ('count', ctypes.c_double), ('gamma', c_vp), ('beta', c_vp), ('running_mean', c_vp),
-                ('running_var', c_vp), ('eps', c_float), ('momentum', c_float), ('relu', c_int), ('C', c_int)]
 
 
 _lib = None

@@ -148,10 +148,14 @@ def to_cl_padded(x, Cs):
     return y
 
 
-def split_tf32(x):
+def split_tf32(xc, C=None, scale=None, shift=None, relu=False):
+    """Channels-last fp32 [..., Cs] -> TF32 pair (hi, lo) of the same shape (nrgbd_split_tf32). Channels below C (default
+    Cs) hold x, or relu(x * scale + shift) when scale / shift [C] are given; the others hold zero."""
     L = _lib.lib()
-    hi = torch.empty_like(x); lo = torch.empty_like(x)
-    check(L.nrgbd_split_tf32(ptr(x), x.numel(), ptr(hi), ptr(lo), _st()))
+    Cs = xc.shape[-1]
+    hi = torch.empty_like(xc); lo = torch.empty_like(xc)
+    check(L.nrgbd_split_tf32(ptr(xc), xc.numel() // Cs, Cs, Cs, Cs if C is None else C, ptr(scale), ptr(shift), 1 if relu else 0,
+                             ptr(hi), ptr(lo), _st()))
     return hi, lo
 
 
@@ -171,84 +175,65 @@ def pack_weight_tc(w, transposed=False):
     return hi, lo
 
 
-def conv_tc(x, w, bias=None, stride=1, pad=0, dilation=1, leaky=False, want_stats=False, impl='v1'):
-    """Tensor-core counterpart of conv() (same arguments / returns). impl: 'v1' (pre-split activations
-    from global memory) or 'v2' (raw activations, split into scratch right before the GEMM)."""
+def _conv_tc_pair(xh, xl, x_shape, w, bias, stride, pad, dilation, leaky, want_stats):
+    """nrgbd_conv_nhwc_tc on the TF32 pair (xh, xl), channels-last [N,(D,)H,W,Cin_pad], of an input of NCHW / NCDHW shape
+    x_shape. Returns what conv_tc returns."""
     L = _lib.lib()
-    is3d = x.dim() == 5
-    N = x.shape[0]
-    Din = x.shape[2] if is3d else 1
-    Hin, Win = x.shape[-2], x.shape[-1]
-    Cout, Cin = w.shape[0], w.shape[1]
-    Cin_pad, Cout_pad = pad_to(Cin, 32), pad_to(Cout, 16)
-    xc = to_cl_padded(x, Cin_pad)
-    xh, xl = split_tf32(xc)
+    is3d = len(x_shape) == 5
+    N = x_shape[0]
+    Din = x_shape[2] if is3d else 1
+    Hin, Win = x_shape[-2], x_shape[-1]
+    Cout = w.shape[0]
+    Cin_pad, Cout_pad = xh.shape[-1], pad_to(Cout, 16)
     kd = w.shape[2] if is3d else 1
     kh, kw = w.shape[-2], w.shape[-1]
     Ho = (Hin + 2 * pad - dilation * (kh - 1) - 1) // stride + 1
     Wo = (Win + 2 * pad - dilation * (kw - 1) - 1) // stride + 1
     wh, wl = pack_weight_tc(w)
     Cs_out = pad4(Cout)
-    y = torch.zeros((N,) + ((Din,) if is3d else ()) + (Ho, Wo, Cs_out), device=x.device, dtype=torch.float32)
-    stats = torch.zeros((2, Cout), device=x.device, dtype=torch.float64) if want_stats else None
-    if impl == 'v2':
-        check(L.nrgbd_conv_nhwc_tc2(ptr(xc), N, Din, Hin, Win, Cin_pad, Cin_pad, ptr(wh), ptr(wl), ptr(bias), Cout, Cout_pad,
-                                    kd, kh, kw, stride, pad, dilation, ptr(y), Ho, Wo, Cs_out, 0, 1 if leaky else 0,
-                                    ctypes.c_void_p(stats.data_ptr()) if want_stats else None, _st()))
-    else:
-        check(L.nrgbd_conv_nhwc_tc(ptr(xh), ptr(xl), N, Din, Hin, Win, Cin_pad, Cin_pad, ptr(wh), ptr(wl), ptr(bias), Cout, Cout_pad,
-                                   kd, kh, kw, stride, pad, dilation, ptr(y), Ho, Wo, Cs_out, 0, 1 if leaky else 0,
-                                   ctypes.c_void_p(stats.data_ptr()) if want_stats else None, _st()))
+    y = torch.zeros((N,) + ((Din,) if is3d else ()) + (Ho, Wo, Cs_out), device=xh.device, dtype=torch.float32)
+    stats = torch.zeros((2, Cout), device=xh.device, dtype=torch.float64) if want_stats else None
+    check(L.nrgbd_conv_nhwc_tc(ptr(xh), ptr(xl), N, Din, Hin, Win, Cin_pad, Cin_pad, ptr(wh), ptr(wl), ptr(bias), Cout, Cout_pad,
+                               kd, kh, kw, stride, pad, dilation, ptr(y), Ho, Wo, Cs_out, 0, 1 if leaky else 0,
+                               ctypes.c_void_p(stats.data_ptr()) if want_stats else None, _st()))
     out = from_cl(y, Cout)
     return (out, stats) if want_stats else out
 
 
-def conv_transpose2d_tc(x, w, bias=None, leaky=False, impl='v1'):
+def conv_tc(x, w, bias=None, stride=1, pad=0, dilation=1, leaky=False, want_stats=False):
+    """Tensor-core counterpart of conv() (same arguments / returns): the split, then the GEMM on the TF32 pair."""
+    xh, xl = split_tf32(to_cl_padded(x, pad_to(w.shape[1], 32)))
+    return _conv_tc_pair(xh, xl, x.shape, w, bias, stride, pad, dilation, leaky, want_stats)
+
+
+def conv_transpose2d_tc(x, w, bias=None, leaky=False):
     L = _lib.lib()
     N, Cin, Hin, Win = x.shape
     Cout = w.shape[1]
     Cin_pad, Cout_pad = pad_to(Cin, 32), pad_to(Cout, 16)
-    xc = to_cl_padded(x, Cin_pad)
-    xh, xl = split_tf32(xc)
+    xh, xl = split_tf32(to_cl_padded(x, Cin_pad))
     wh, wl = pack_weight_tc(w, transposed=True)
     Cs_out = pad4(Cout)
     y = torch.zeros((N, 2 * Hin, 2 * Win, Cs_out), device=x.device, dtype=torch.float32)
-    if impl == 'v2':
-        check(L.nrgbd_conv_transpose2d_k4s2_nhwc_tc2(ptr(xc), N, Hin, Win, Cin_pad, Cin_pad, ptr(wh), ptr(wl), ptr(bias), Cout,
-                                                     Cout_pad, ptr(y), Cs_out, 0, 1 if leaky else 0, _st()))
-    else:
-        check(L.nrgbd_conv_transpose2d_k4s2_nhwc_tc(ptr(xh), ptr(xl), N, Hin, Win, Cin_pad, Cin_pad, ptr(wh), ptr(wl), ptr(bias), Cout,
-                                                    Cout_pad, ptr(y), Cs_out, 0, 1 if leaky else 0, _st()))
+    check(L.nrgbd_conv_transpose2d_k4s2_nhwc_tc(ptr(xh), ptr(xl), N, Hin, Win, Cin_pad, Cin_pad, ptr(wh), ptr(wl), ptr(bias), Cout,
+                                                Cout_pad, ptr(y), Cs_out, 0, 1 if leaky else 0, _st()))
     return from_cl(y, Cout)
 
 
 def conv_tc_bn_in(x_raw, in_stats, gamma, beta, w, bias=None, stride=1, pad=0, dilation=1, relu=True, leaky=False,
                   want_stats=False, eps=1e-5, running=None):
-    """conv(relu(batch_norm_train(x_raw))) in one kernel: x_raw [N,C,H,W] is the raw output of the producing conv and
-    in_stats its [2,C] float64 sums (conv(..., want_stats=True)); the normalisation happens in the consumer's operand
-    converter (nrgbd_conv_nhwc_tc2_bn_in). running = (running_mean, running_var) tensors to update, optional."""
+    """conv(relu(batch_norm_train(x_raw))) without a BatchNorm pass: x_raw [N,C,H,W] is the raw output of the producing conv
+    and in_stats its [2,C] float64 sums (conv(..., want_stats=True)); nrgbd_bn_finalize turns them into scale / shift and
+    the operand split applies them. running = (running_mean, running_var) tensors to update, optional."""
     L = _lib.lib()
     assert x_raw.dim() == 4
     N, Cin, Hin, Win = x_raw.shape
-    Cout = w.shape[0]
-    Cin_pad, Cout_pad = pad_to(Cin, 32), pad_to(Cout, 16)
-    xc = to_cl_padded(x_raw, Cin_pad)
-    kh, kw = w.shape[-2], w.shape[-1]
-    Ho = (Hin + 2 * pad - dilation * (kh - 1) - 1) // stride + 1
-    Wo = (Win + 2 * pad - dilation * (kw - 1) - 1) // stride + 1
-    wh, wl = pack_weight_tc(w)
-    Cs_out = pad4(Cout)
-    y = torch.zeros((N, Ho, Wo, Cs_out), device=x_raw.device, dtype=torch.float32)
-    stats = torch.zeros((2, Cout), device=x_raw.device, dtype=torch.float64) if want_stats else None
-    g = gamma.float().contiguous(); b = beta.float().contiguous()
-    d = _lib.BnInput(ctypes.c_void_p(in_stats.data_ptr()), float(N * Hin * Win), ctypes.c_void_p(g.data_ptr()), ctypes.c_void_p(b.data_ptr()),
-                     ctypes.c_void_p(running[0].data_ptr()) if running else None, ctypes.c_void_p(running[1].data_ptr()) if running else None,
-                     eps, 0.1, 1 if relu else 0, Cin)
-    check(L.nrgbd_conv_nhwc_tc2_bn_in(ptr(xc), N, 1, Hin, Win, Cin_pad, Cin_pad, ptr(wh), ptr(wl), ptr(bias), Cout, Cout_pad, 1, kh, kw,
-                                      stride, pad, dilation, ptr(y), Ho, Wo, Cs_out, 0, 1 if leaky else 0,
-                                      ctypes.c_void_p(stats.data_ptr()) if want_stats else None, ctypes.byref(d), _st()))
-    out = from_cl(y, Cout)
-    return (out, stats) if want_stats else out
+    scale = torch.empty(Cin, device=x_raw.device, dtype=torch.float32); shift = torch.empty_like(scale)
+    check(L.nrgbd_bn_finalize(ctypes.c_void_p(in_stats.data_ptr()), Cin, float(N * Hin * Win), ptr(gamma.float().contiguous()),
+                              ptr(beta.float().contiguous()), _F(eps), ptr(scale), ptr(shift), ptr(running[0]) if running else None,
+                              ptr(running[1]) if running else None, _F(0.1), _st()))
+    xh, xl = split_tf32(to_cl_padded(x_raw, pad_to(Cin, 32)), Cin, scale, shift, relu)
+    return _conv_tc_pair(xh, xl, x_raw.shape, w, bias, stride, pad, dilation, leaky, want_stats)
 
 
 # ---------------------------------------------------------------------------------------------

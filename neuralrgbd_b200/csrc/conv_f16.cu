@@ -704,9 +704,8 @@ static int conv_nhwc_h2_impl(const void* x_hi, const void* x_lo, int N, int Din,
   NRGBD_REQUIRE(x_hi && w, "null pointer");
   NRGBD_REQUIRE(Cin_pad % 32 == 0 && Cin_pad >= 32 && Cin_pad <= Cs_in && Cs_in % 8 == 0 && Cout_pad % 16 == 0 && Cout <= Cout_pad && Cout > Cout_pad - 16 &&
                     BN == (Cout_pad < 128 ? Cout_pad : 128), "channel counts not supported by the f16-pair tensor-core path");
-  NRGBD_REQUIRE(kd >= 1 && kd <= 3 && kh * kw <= WG_MAX_TAP2D && stride >= 1 && stride <= 8, "unsupported filter");
-  NRGBD_REQUIRE(Hout == (Hin + 2 * pad - dilation * (kh - 1) - 1) / stride + 1 &&
-                    Wout == (Win + 2 * pad - dilation * (kw - 1) - 1) / stride + 1, "output extent mismatch");
+  int rc = wg_check_conv_shape(Hin, Win, kd, kh, kw, stride, pad, dilation, Hout, Wout);
+  if (rc != NRGBD_OK) return rc;
   if (y_hi) {
     // the output as the operand pair of the next convolution: every Cs_out channel stored, pad channels as zeros
     NRGBD_REQUIRE(Cs_out % 32 == 0 && Cs_out >= Cout_pad && c_off == 0 && stats == nullptr && (((uintptr_t)y_hi | (uintptr_t)y_lo) & 15) == 0,
@@ -716,18 +715,12 @@ static int conv_nhwc_h2_impl(const void* x_hi, const void* x_lo, int N, int Din,
   c.tf32 = 0;
   c.x_hi = x_hi; c.x_lo = x_lo; c.N = N; c.Din = Din; c.Hin = Hin; c.Win = Win; c.Cin_pad = Cin_pad; c.Cs_in = Cs_in;
   c.w_hi = w; c.w_lo = reinterpret_cast<const __half*>(w) + (long long)Cout_pad * Cin_pad; c.w_tap_stride = 2ll * Cout_pad * Cin_pad;
-  c.n_wslices = kd * kh * kw; c.Cout_pad = Cout_pad;
+  c.Cout_pad = Cout_pad;
   c.bias = bias; c.stats = stats; c.y = y; c.y_hi = y_hi; c.y_lo = y_lo;
-  c.Cout = Cout; c.Dout = Din; c.Hout = Hout; c.Wout = Wout; c.Cs_out = Cs_out; c.c_off = c_off;
-  c.out_stride = 1; c.out_off_y = 0; c.out_off_x = 0; c.leaky = leaky;
+  c.Cout = Cout; c.Cs_out = Cs_out; c.c_off = c_off; c.leaky = leaky;
   if (aff) { c.aff_scale = aff->aff_scale; c.aff_shift = aff->aff_shift; c.res = aff->res; c.res_hi = aff->res_hi; c.res_lo = aff->res_lo; c.relu = aff->relu; }
-  c.Hy = Hout; c.Wx = Wout; c.in_stride = stride; c.n_kz = kd; c.n_tap = kh * kw;
-  for (int a = 0; a < kd; ++a) c.dz[a] = (signed char)(a - kd / 2);
-  int t = 0;
-  for (int b = 0; b < kh; ++b)
-    for (int e = 0; e < kw; ++e) { c.dy[t] = (signed char)(b * dilation - pad); c.dx[t] = (signed char)(e * dilation - pad); ++t; }
-  for (int a = 0; a < kd * kh * kw; ++a) c.wsel[a] = (unsigned char)a;
-  int rc = conv_wgmma(c, st);
+  wg_conv_taps(c, kd, kh, kw, stride, pad, dilation, Hout, Wout);
+  rc = conv_wgmma(c, st);
   if (rc != NRGBD_OK) return rc;
   NRGBD_COUNT(1);
   NRGBD_LAUNCH_CHECK();
@@ -757,25 +750,16 @@ int nrgbd_conv_transpose2d_k4s2_nhwc_h2(const void* x_hi, const void* x_lo, int 
   NRGBD_REQUIRE(x_hi && w && y, "null pointer");
   NRGBD_REQUIRE(Cin_pad % 32 == 0 && Cin_pad >= 32 && Cin_pad <= Cs_in && Cs_in % 8 == 0 && Cout_pad % 16 == 0 && Cout <= Cout_pad && Cout > Cout_pad - 16 &&
                     BN == (Cout_pad < 128 ? Cout_pad : 128), "channel counts not supported by the f16-pair tensor-core path");
-  const int kys[2][2] = {{1, 3}, {0, 2}};
-  const int dys[2][2] = {{0, -1}, {1, 0}};
   for (int py = 0; py < 2; ++py)
     for (int px = 0; px < 2; ++px) {
       WgConv c{};
       c.tf32 = 0;
-      c.x_hi = x_hi; c.x_lo = x_lo; c.N = N; c.Din = 1; c.Hin = Hin; c.Win = Win; c.Cin_pad = Cin_pad; c.Cs_in = Cs_in;
+      c.x_hi = x_hi; c.x_lo = x_lo; c.N = N; c.Hin = Hin; c.Win = Win; c.Cin_pad = Cin_pad; c.Cs_in = Cs_in;
       c.w_hi = w; c.w_lo = reinterpret_cast<const __half*>(w) + (long long)Cout_pad * Cin_pad; c.w_tap_stride = 2ll * Cout_pad * Cin_pad;
-      c.n_wslices = 16; c.Cout_pad = Cout_pad;
+      c.Cout_pad = Cout_pad;
       c.bias = bias; c.stats = nullptr; c.y = y;
-      c.Cout = Cout; c.Dout = 1; c.Hout = 2 * Hin; c.Wout = 2 * Win; c.Cs_out = Cs_out; c.c_off = c_off;
-      c.out_stride = 2; c.out_off_y = py; c.out_off_x = px; c.leaky = leaky;
-      c.Hy = Hin; c.Wx = Win; c.in_stride = 1; c.n_kz = 1; c.n_tap = 4;
-      int t = 0;
-      for (int a = 0; a < 2; ++a)
-        for (int b = 0; b < 2; ++b) {
-          c.dy[t] = (signed char)dys[py][a]; c.dx[t] = (signed char)dys[px][b];
-          c.wsel[t] = (unsigned char)(kys[py][a] * 4 + kys[px][b]); ++t;
-        }
+      c.Cout = Cout; c.Cs_out = Cs_out; c.c_off = c_off; c.leaky = leaky;
+      wg_transpose_k4s2_class(c, py, px);
       int rc = conv_wgmma(c, st);
       if (rc != NRGBD_OK) return rc;
     }

@@ -98,6 +98,7 @@ struct nrgbd_kvnet {
   Pool pool;
   double* stats = nullptr;          // [2][512] per-channel sums of the conv in flight
   double* stats_b = nullptr;        // second set: a conv that consumes one BatchNorm (fused) while producing the next
+  float* bn_coef = nullptr;         // [scale 512 | shift 512] of the BatchNorm a 3xTF32 operand split applies
   unsigned int* bn_counter = nullptr;   // f16-pair mode: the BatchNorm pass re-zeroes the statistics it consumed (no memset nodes)
   float* ws_sweep = nullptr;        // V*12
   cudaStream_t st = nullptr;
@@ -305,14 +306,29 @@ bool use_tc(Eng* e, const Act& x, int Cout) {
   return e->conv_math == 1 && nrgbd_conv_tc_supported(pad32(x.C), pad16(Cout)) && pad32(x.C) <= x.Cs;
 }
 
-// TF32 hi / lo split of an activation into two pool buffers
-void split_act(Eng* e, const Act& x, Act& hi, Act& lo) {
+// Training-mode BatchNorm `pre` + ReLU of a convolution's input, applied by its 3xTF32 operand split: the input is the RAW
+// output of the producing conv, whose per-channel sums are in `stats` (stats null: no BatchNorm)
+struct InBn { std::string pre; const double* stats = nullptr; };
+
+// TF32 hi / lo pair [pos][pad32(C)] of an activation in two pool buffers. With bn.stats set, of [relu](BatchNorm(x)): its
+// coefficients are finalised into e->bn_coef (updating the running statistics once) and applied while splitting, one pass
+// over x instead of a BatchNorm pass and the split after it.
+void split_act(Eng* e, const Act& x, const InBn& bn, Act& hi, Act& lo) {
   hi = x; lo = x; hi.p = lo.p = nullptr;
+  hi.Cs = lo.Cs = pad32(x.C);
   if (e->rc) return;
-  hi.p = e->pool.acquire((size_t)x.floats() * sizeof(float));
-  lo.p = e->pool.acquire((size_t)x.floats() * sizeof(float));
+  hi.p = e->pool.acquire((size_t)hi.floats() * sizeof(float));
+  lo.p = e->pool.acquire((size_t)lo.floats() * sizeof(float));
   if (!hi.p || !lo.p) { nrgbd_set_error("engine: out of device memory"); e->rc = NRGBD_ERR_NOMEM; return; }
-  ENG_CALL(e, nrgbd_split_tf32(x.p, x.floats(), hi.p, lo.p, (nrgbd_stream_t)e->st));
+  nrgbd_stream_t st = (nrgbd_stream_t)e->st;
+  if (!bn.stats) {
+    ENG_CALL(e, nrgbd_split_tf32(x.p, x.pos(), x.Cs, hi.Cs, hi.Cs, nullptr, nullptr, 0, hi.p, lo.p, st));
+    return;
+  }
+  const BnParams p = bn_params(e, bn.pre);
+  float *scale = e->bn_coef, *shift = e->bn_coef + 512;
+  ENG_CALL(e, nrgbd_bn_finalize(bn.stats, x.C, (double)x.pos(), p.gamma, p.beta, 1e-5f, scale, shift, p.rm, p.rv, 0.1f, st));
+  ENG_CALL(e, nrgbd_split_tf32(x.p, x.pos(), x.Cs, hi.Cs, x.C, scale, shift, 1, hi.p, lo.p, st));
 }
 
 // Output extent, algorithmic FLOPs and profile tag of a convolution; bench.py's roofline and --layer-table read the tags.
@@ -334,7 +350,7 @@ struct ConvOut {
   Act* dst = nullptr;                       // write into this activation instead
   int Cs = -1;                              // channel stride of the fresh activation
   double* stats = nullptr;                  // per-channel sums into this buffer instead
-  const nrgbd_bn_input* in_bn = nullptr;    // 3xTF32: x is the RAW output of a conv, normalised while its operands are split
+  InBn in_bn;                               // 3xTF32: x is the RAW output of a conv, normalised while its operands are split
   // f16-pair mode, no BatchNorm after the conv: the result is written only as the operand pair of the convolution that
   // consumes it (y.p is a 16-byte key of the pair, y.pair_only) - no fp32 tensor, no split pass
   bool pair_only = false;
@@ -347,6 +363,12 @@ Act conv(Eng* e, const Act& x, const std::string& wname, int Cout, int kd, int k
   nrgbd_stream_t st = (nrgbd_stream_t)e->st;
   if (x.pair_only && !use_h2(e, x)) {          // x.p is no fp32 tensor: only the f16-pair path can read x
     if (!e->rc) { nrgbd_set_error("engine: '%s' reads an activation that exists only as an operand pair", wname.c_str()); e->rc = NRGBD_ERR_BAD_ARG; }
+    return Act();
+  }
+  // only the 3xTF32 split applies an input BatchNorm; it is finalised after the memset of `stats` below, so from the
+  // output's own statistics it would read zeros
+  if (out.in_bn.stats && (out.in_bn.stats == stats || !use_tc(e, x, Cout))) {
+    if (!e->rc) { nrgbd_set_error("engine: '%s': an input BatchNorm needs the 3xTF32 path and statistics other than the output's", wname.c_str()); e->rc = NRGBD_ERR_BAD_ARG; }
     return Act();
   }
   const ConvGeom g = conv_geom(x, Cout, kd, k, stride, pad, dil);
@@ -377,19 +399,11 @@ Act conv(Eng* e, const Act& x, const std::string& wname, int Cout, int kd, int k
   }
   if (use_tc(e, x, Cout)) {
     const Packed* pt = packw(e, wname, PK_TC, Cout, x.C, taps, false);
-    if (!e->rc && out.in_bn) {
-      // x is the RAW output of the producing conv: BatchNorm + ReLU are applied in the pass that splits the operands
-      // (4 B read + 8 B written per element, against 4 + 4 for a separate BatchNorm pass and 4 + 8 for the split after it)
-      ProfScope ps(e, 0, g.flops, g.tag);
-      ENG_CALL(e, nrgbd_conv_nhwc_tc2_bn_in(x.p, x.N, x.D, x.H, x.W, pt->Cin_pad, x.Cs, pt->w, pt->lo, b, Cout, pt->Cout_pad, kd, k, k,
-                                            stride, pad, dil, y.p, g.Ho, g.Wo, y.Cs, 0, leaky ? 1 : 0, stats, out.in_bn, st));
-      return y;
-    }
     Act xh, xl;
-    split_act(e, x, xh, xl);
+    split_act(e, x, out.in_bn, xh, xl);
     if (!e->rc) {
       ProfScope ps(e, 0, g.flops, g.tag);
-      ENG_CALL(e, nrgbd_conv_nhwc_tc(xh.p, xl.p, x.N, x.D, x.H, x.W, pt->Cin_pad, x.Cs, pt->w, pt->lo, b, Cout, pt->Cout_pad, kd, k, k,
+      ENG_CALL(e, nrgbd_conv_nhwc_tc(xh.p, xl.p, x.N, x.D, x.H, x.W, pt->Cin_pad, xh.Cs, pt->w, pt->lo, b, Cout, pt->Cout_pad, kd, k, k,
                                      stride, pad, dil, y.p, g.Ho, g.Wo, y.Cs, 0, leaky ? 1 : 0, stats, st));
     }
     release(e, xh); release(e, xl);
@@ -484,17 +498,6 @@ void bn_train(Eng* e, Act& y, const std::string& pre, const double* stats, const
                                    y.pos(), y.Cs, y.C, y.p, (nrgbd_stream_t)e->st));
 }
 
-// 3xTF32 descriptor of training-mode BatchNorm `pre` + ReLU on t, the RAW output of the conv whose sums are in `stats`:
-// applied by the convolution that reads t while it splits its operands (nrgbd_conv_nhwc_tc2_bn_in)
-nrgbd_bn_input bn_input(Eng* e, const std::string& pre, const double* stats, const Act& t) {
-  const BnParams p = bn_params(e, pre);
-  nrgbd_bn_input bn;
-  bn.stats = stats; bn.count = (double)t.pos();
-  bn.gamma = p.gamma; bn.beta = p.beta; bn.running_mean = p.rm; bn.running_var = p.rv;
-  bn.eps = 1e-5f; bn.momentum = 0.1f; bn.relu = 1; bn.C = t.C;
-  return bn;
-}
-
 // Conv (no bias) + BatchNorm(batch statistics) [+ ReLU] [+ residual]; BN applied in place.
 // `pre` is the Sequential(Conv, BN) prefix: weights pre.0.weight, pre.1.{weight,bias,running_*}.
 // out_use (f16-pair mode only): 0 = the result is read as fp32 only; 1 = also by a convolution (the BatchNorm pass emits the
@@ -525,20 +528,15 @@ Act convbn(Eng* e, const Act& x, const std::string& pre, int Cout, int kd, int k
   return y;
 }
 
-// Whether conv `Cin -> Cout` at this activation takes the 3xTF32 path that can fold an input BN into its operand split
-bool takes_tc2(Eng* e, const Act& x, int Cout) {
-  return use_tc(e, x, Cout) && nrgbd_conv_tc2_supported(pad32(x.C), pad16(Cout));
-}
-
 // psm_submodule.BasicBlock :31-49
 // fp32_out: the block's output is read as an fp32 tensor by something other than a convolution / residual add (f16-pair mode:
 // otherwise only its operand pair is written)
 Act basic_block(Eng* e, Act& x, const std::string& pre, int planes, int stride, int dil, bool down, bool fp32_out = true) {
   const int p1 = dil > 1 ? dil : 1;                  // psm_submodule.convbn :13
-  // Fused form (3xTF32 path): conv1 leaves its RAW output and per-channel sums; BN1 + ReLU are applied by conv2 while it
-  // splits its operands (nrgbd_conv_nhwc_tc2_bn_in) - one read + one write of the activation less per block.
+  // Fused form (3xTF32 path): conv1 leaves its RAW output and per-channel sums; BN1 + ReLU are applied by the split of
+  // conv2's operands (split_act) - one read + one write of the activation less per block.
   Act probe = x; probe.C = planes; probe.Cs = pad32(planes);
-  const bool fused = takes_tc2(e, x, planes) && takes_tc2(e, probe, planes);
+  const bool fused = use_tc(e, x, planes) && use_tc(e, probe, planes);
   Act t;
   if (fused) {
     ConvOut raw; raw.stats = e->stats_b;
@@ -553,8 +551,7 @@ Act basic_block(Eng* e, Act& x, const std::string& pre, int planes, int stride, 
   }
   Act o;
   if (fused) {
-    const nrgbd_bn_input bn = bn_input(e, pre + ".conv1.0.1", e->stats_b, t);
-    ConvOut bn_in; bn_in.in_bn = &bn;
+    ConvOut bn_in; bn_in.in_bn = {pre + ".conv1.0.1", e->stats_b};
     o = conv(e, t, pre + ".conv2.0.weight", planes, 1, 3, 1, p1, dil, nullptr, false, true, bn_in);
     bn_train(e, o, pre + ".conv2.1", e->stats, res->p, false);
   } else {
@@ -585,15 +582,13 @@ void feature_cnn(Eng* e, const Act& x0, Act& l1_out, Act& feat_out) {
   // operand split of the conv that consumes them (the raw 5x240x320x32 tensors are read once instead of read+written+read).
   Act c;
   Act probe32 = x0; probe32.C = 32; probe32.Cs = pad32(32); probe32.H = (x0.H + 2 - 3) / 2 + 1; probe32.W = (x0.W + 2 - 3) / 2 + 1;
-  if (takes_tc2(e, probe32, 32)) {
+  if (use_tc(e, probe32, 32)) {
     ConvOut oa; oa.Cs = pad32(32); oa.stats = e->stats_b;
     Act a = conv(e, x0, P + ".firstconv.0.0.weight", 32, 1, 3, 2, 1, 1, nullptr, false, true, oa);
-    const nrgbd_bn_input bn_a = bn_input(e, P + ".firstconv.0.1", e->stats_b, a);
-    ConvOut ob; ob.in_bn = &bn_a;
+    ConvOut ob; ob.in_bn = {P + ".firstconv.0.1", e->stats_b};
     Act b = conv(e, a, P + ".firstconv.2.0.weight", 32, 1, 3, 1, 1, 1, nullptr, false, true, ob);
     release(e, a);
-    const nrgbd_bn_input bn_b = bn_input(e, P + ".firstconv.2.1", e->stats, b);
-    ConvOut oc; oc.stats = e->stats_b; oc.in_bn = &bn_b;
+    ConvOut oc; oc.stats = e->stats_b; oc.in_bn = {P + ".firstconv.2.1", e->stats};
     c = conv(e, b, P + ".firstconv.4.0.weight", 32, 1, 3, 1, 1, 1, nullptr, false, true, oc);
     release(e, b);
     bn_train(e, c, P + ".firstconv.4.1", e->stats_b, nullptr, true);
@@ -667,17 +662,11 @@ void conv_transpose(Eng* e, const Act& x, const std::string& wname, const char* 
   }
   if (use_tc(e, x, Cout)) {
     const Packed* pt = packw(e, wname, PK_TC, Cout, x.C, 16, true);
-    if (!e->rc && nrgbd_conv_tc2_supported(pt->Cin_pad, pt->Cout_pad)) {
-      ProfScope ps(e, 0, g.flops, g.tag);
-      ENG_CALL(e, nrgbd_conv_transpose2d_k4s2_nhwc_tc2(x.p, x.N, x.H, x.W, pt->Cin_pad, x.Cs, pt->w, pt->lo, tb, Cout, pt->Cout_pad,
-                                                       dst.p, dst.Cs, 0, 1, st));
-      return;
-    }
     Act xh, xl;
-    split_act(e, x, xh, xl);
+    split_act(e, x, InBn(), xh, xl);
     if (!e->rc) {
       ProfScope ps(e, 0, g.flops, g.tag);
-      ENG_CALL(e, nrgbd_conv_transpose2d_k4s2_nhwc_tc(xh.p, xl.p, x.N, x.H, x.W, pt->Cin_pad, x.Cs, pt->w, pt->lo, tb, Cout, pt->Cout_pad,
+      ENG_CALL(e, nrgbd_conv_transpose2d_k4s2_nhwc_tc(xh.p, xl.p, x.N, x.H, x.W, pt->Cin_pad, xh.Cs, pt->w, pt->lo, tb, Cout, pt->Cout_pad,
                                                       dst.p, dst.Cs, 0, 1, st));
     }
     release(e, xh); release(e, xl);
@@ -829,6 +818,7 @@ int nrgbd_kvnet_create(int H, int W, int D, int V, int feature_dim, int kv_featu
   const size_t hw = (size_t)e->h * e->w;
   bool ok = cudaMalloc((void**)&e->stats, sizeof(double) * 2 * 512) == cudaSuccess &&
             cudaMalloc((void**)&e->stats_b, sizeof(double) * 2 * 512) == cudaSuccess &&
+            cudaMalloc((void**)&e->bn_coef, sizeof(float) * 2 * 512) == cudaSuccess &&
             cudaMalloc((void**)&e->bn_counter, sizeof(unsigned int)) == cudaSuccess &&
             cudaMalloc((void**)&e->eval_coef, sizeof(float) * 1024 * NRGBD_BN_EVAL_MAX) == cudaSuccess &&
             cudaMalloc((void**)&e->ws_sweep, sizeof(float) * 12 * V) == cudaSuccess &&
@@ -848,7 +838,7 @@ int nrgbd_kvnet_destroy(nrgbd_kvnet* e) {
   for (auto& kv : e->params) if (kv.second.owned) cudaFree(kv.second.p);
   for (auto& kv : e->packed) free_packed(kv.second);
   for (int i = 0; i < 2; ++i) { cudaFree(e->cam[i].K); cudaFree(e->cam[i].rays); }
-  cudaFree(e->d_planes); cudaFree(e->stats); cudaFree(e->stats_b); cudaFree(e->bn_counter); cudaFree(e->eval_coef); cudaFree(e->ws_sweep);
+  cudaFree(e->d_planes); cudaFree(e->stats); cudaFree(e->stats_b); cudaFree(e->bn_coef); cudaFree(e->bn_counter); cudaFree(e->eval_coef); cudaFree(e->ws_sweep);
   cudaFree(e->bv_cur_hwd); cudaFree(e->dpv_hwd); cudaFree(e->prior_hwd); cudaFree(e->depth); cudaFree(e->conf);
   cudaFree(e->x0_buf); cudaFree(e->rt_buf); cudaFree(e->ref_cur_hwd); cudaFree(e->ref_kv_hwd);
   drop_graphs(e);

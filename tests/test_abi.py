@@ -58,34 +58,17 @@ def test_missing_library_fails_loudly(monkeypatch):
         assert 'no fallback' in str(e)
 
 
-def test_header_is_plain_c_and_struct_layout_matches_ctypes(tmp_path):
-    """include/nrgbd.h must be consumable from C (the boundary is a C ABI, not C++), and the one struct that crosses it
-    must have the layout the ctypes mirror assumes."""
+def test_header_is_plain_c():
+    """include/nrgbd.h must be consumable from C: the boundary is a C ABI, not C++."""
     import shutil
     import subprocess
     gcc = shutil.which('gcc')
     if gcc is None:
         import pytest
         pytest.skip('no C compiler')
-    hdr_dir = os.path.join(ROOT, 'include')
-    r = subprocess.run([gcc, '-fsyntax-only', '-x', 'c', '-std=c99', '-Wall', '-Werror', os.path.join(hdr_dir, 'nrgbd.h')],
+    r = subprocess.run([gcc, '-fsyntax-only', '-x', 'c', '-std=c99', '-Wall', '-Werror', os.path.join(ROOT, 'include', 'nrgbd.h')],
                        capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
-    src = tmp_path / 'layout.c'
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "nrgbd.h"\n'
-                   'int main(void){printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(nrgbd_bn_input),'
-                   'offsetof(nrgbd_bn_input,stats),offsetof(nrgbd_bn_input,count),offsetof(nrgbd_bn_input,gamma),'
-                   'offsetof(nrgbd_bn_input,beta),offsetof(nrgbd_bn_input,running_mean),offsetof(nrgbd_bn_input,running_var),'
-                   'offsetof(nrgbd_bn_input,eps),offsetof(nrgbd_bn_input,momentum),offsetof(nrgbd_bn_input,relu),'
-                   'offsetof(nrgbd_bn_input,C));return 0;}\n')
-    exe = tmp_path / 'layout'
-    r = subprocess.run([gcc, '-I', hdr_dir, str(src), '-o', str(exe)], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    got = [int(v) for v in subprocess.run([str(exe)], capture_output=True, text=True).stdout.split()]
-    B = _lib.BnInput
-    want = [ctypes.sizeof(B)] + [getattr(B, f).offset for f in ('stats', 'count', 'gamma', 'beta', 'running_mean', 'running_var',
-                                                                 'eps', 'momentum', 'relu', 'C')]
-    assert got == want
 
 
 def test_c_program_links_and_uses_the_library(tmp_path):

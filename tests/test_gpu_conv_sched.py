@@ -136,11 +136,11 @@ def test_conv2d_tf32_sched_vs_oracle(cfg):
     w = (rng.standard_normal((cfg['Cout'], cfg['Cin'], 3, 3)) / math.sqrt(cfg['Cin'] * 9)).astype(np.float32)
     b = rng.standard_normal(cfg['Cout']).astype(np.float32)
     ref = N.leaky_relu(N.conv2d(x, w, b, 1, cfg['p'], cfg['d']))
-    y, st = convops.conv_tc(T(x), T(w), T(b), 1, cfg['p'], cfg['d'], leaky=True, want_stats=True, impl='v2')
+    y, st = convops.conv_tc(T(x), T(w), T(b), 1, cfg['p'], cfg['d'], leaky=True, want_stats=True)
     assert y.shape == ref.shape and rel_err(y.cpu().numpy(), ref) <= 6e-6
     check_stats(st, y)
     for flags in (8, 32, 40):
         set_flags(flags)
-        y2 = convops.conv_tc(T(x), T(w), T(b), 1, cfg['p'], cfg['d'], leaky=True, impl='v2')
+        y2 = convops.conv_tc(T(x), T(w), T(b), 1, cfg['p'], cfg['d'], leaky=True)
         assert torch.equal(y2, y)
     set_flags(0)

@@ -79,15 +79,12 @@ def main():
                                     ptr(y), Ho, Wo, Cso, 0, 0, ctypes.c_void_p(stats.data_ptr()), st()))
 
         def split():
-            check(L.nrgbd_split_tf32(ptr(x), x.numel(), ptr(xh), ptr(xl), st()))
+            check(L.nrgbd_split_tf32(ptr(x), N * D * H * W, Cs, Cs, Cs, None, None, 0, ptr(xh), ptr(xl), st()))
 
         def tc():
             check(L.nrgbd_conv_nhwc_tc(ptr(xh), ptr(xl), N, D, H, W, Cs, Cs, ptr(wh), ptr(wl), None, Cout, convops.pad_to(Cout, 16), kd, k, k,
                                        s, p, d, ptr(y2), Ho, Wo, Cso, 0, 0, ctypes.c_void_p(stats.data_ptr()), st()))
-        def tc2():
-            check(L.nrgbd_conv_nhwc_tc2(ptr(x), N, D, H, W, Cs, Cs, ptr(wh), ptr(wl), None, Cout, convops.pad_to(Cout, 16), kd, k, k,
-                                        s, p, d, ptr(y3), Ho, Wo, Cso, 0, 0, ctypes.c_void_p(stats.data_ptr()), st()))
-        y3 = torch.zeros_like(y)
+
         y4 = torch.zeros_like(y)
         wp2, cin_p2, cout_p2, bn2 = convops.pack_weight_h2(w)
         ph = torch.empty(x.shape, device=dev, dtype=torch.float16); pl = torch.empty_like(ph)
@@ -125,12 +122,11 @@ def main():
             t_h2 = safe(h2)
             print(json.dumps(dict(layer=name, h2_us=t_h2, h2_tflops=flops / t_h2 / 1e6)), flush=True)
             continue
-        t_simt = safe(simt, 3 if quick else 10); t_split = safe(split); t_tc = safe(tc, 3 if quick else 10); t_tc2 = safe(tc2)
+        t_simt = safe(simt, 3 if quick else 10); t_split = safe(split); t_tc = safe(tc, 3 if quick else 10)
         t_split_h2 = safe(split_h2); t_h2 = safe(h2)
         err = float((y - y2).abs().max() / y.abs().max())
         rec = dict(layer=name, gflop=flops / 1e9, simt_us=t_simt, simt_tflops=flops / t_simt / 1e6, split_us=t_split, tc_us=t_tc,
-                   tc_tflops=flops / t_tc / 1e6, tc_vs_simt_relerr=err, tc2_us=t_tc2,
-                   tc2_tflops=flops / t_tc2 / 1e6, tc2_vs_simt_relerr=float((y - y3).abs().max() / y.abs().max()),
+                   tc_tflops=flops / t_tc / 1e6, tc_vs_simt_relerr=err,
                    h2_us=t_h2, h2_split_us=t_split_h2, h2_tflops=flops / t_h2 / 1e6,
                    h2_vs_simt_relerr=float((y - y4).abs().max() / y.abs().max()))
         out.append(rec)
