@@ -17,15 +17,12 @@ Cases (steps: 0 = first window):
     first window + one steady step re-seeded with the train-mode prior of reference_outputs.npz;
   - r1_256_d16: t_win_r = 1 (V = 2), train mode: first window + one re-seeded steady step.
 """
-import os
-
 import numpy as np
 
 from neuralrgbd_b200 import arch, synth
-from tests import cases
+from tests import cases, harness
 from tests import cases_twin as CT
 
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 F16_CASES = ['c2_640x480_d64', 'stream_256_d16', 'eval_256_d16', 'r1_256_d16']
 MODE = {'c2_640x480_d64': 'train', 'stream_256_d16': 'train', 'eval_256_d16': 'eval', 'r1_256_d16': 'train'}
 FREE_RUNNING = {'stream_256_d16'}
@@ -62,7 +59,7 @@ def cam(make_cam, c):
 
 def running_stats():
     """The running statistics make_golden_eval.py warmed for kvnet_256_d16 (state_dict name -> array)."""
-    g = np.load(os.path.join(GOLDEN, 'eval_outputs.npz'))
+    g = harness.golden('eval_outputs.npz')
     pre = 'eval/kvnet_256_d16/rs/'
     return {k[len(pre):]: np.asarray(g[k]) for k in g.files if k.startswith(pre)}
 
@@ -78,11 +75,10 @@ def reseed_prior(name, step):
     """The reference's train-mode prior of a re-seeded steady step (step 1 of the non-streaming cases)."""
     assert step == 1 and name not in FREE_RUNNING
     if name == 'c2_640x480_d64':
-        return np.load(os.path.join(GOLDEN, 'configs_priors_c23_640x480_d64_v4_stream30.npz'))[
-            'cfg/c23_640x480_d64_v4_stream30/step0/BV_predict_next_full']
+        return harness.reference_prior('c23_640x480_d64_v4_stream30', step)
     if name == 'eval_256_d16':
-        return np.load(os.path.join(GOLDEN, 'reference_outputs.npz'))['kvnet/kvnet_256_d16/step0/BV_predict_next_full']
-    return CT.prior('r1_256_d16', 1)
+        return harness.reference_prior('kvnet_256_d16', step)
+    return CT.prior('r1_256_d16', step)
 
 
 def tc_layers(specs):

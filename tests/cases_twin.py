@@ -8,14 +8,8 @@ Steady steps are re-seeded with a train-mode prior of the reference that the rep
 (D, h, w): the r = 2 case of the same frame size (reference_outputs.npz, configs_priors_<case>.npz). A prior is a
 [1, D, h, w] log-DPV and does not depend on the window radius, so any valid one serves as K-Net's input.
 """
-import os
-
-import numpy as np
-
 from neuralrgbd_b200 import arch, synth
-from tests import cases
-
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
+from tests import cases, harness
 
 TWIN_CFG = {
     'r1_256_d16': dict(seed=71, H=256, W=256, D=16, t_win_r=1, wseed=5, n_steps=3, prior_of='kvnet_256_d16'),
@@ -48,8 +42,4 @@ def twin_cam(make_cam, c):
 
 def prior(name, step):
     """The reference's train-mode prior that re-seeds steady step `step` >= 1 of case `name`."""
-    src = TWIN_CFG[name]['prior_of']
-    if src in cases.KVNET_CASES:
-        return np.load(os.path.join(GOLDEN, 'reference_outputs.npz'))['kvnet/%s/step%d/BV_predict_next_full' % (src, step - 1)]
-    assert step == 1, step
-    return np.load(os.path.join(GOLDEN, 'configs_priors_%s.npz' % src))['cfg/%s/step0/BV_predict_next_full' % src]
+    return harness.reference_prior(TWIN_CFG[name]['prior_of'], step)

@@ -1,22 +1,17 @@
 """f-1 on the device: autograd through the est_swp_volume_v4 mirror against torch autograd through the reference
 (golden), the oracle, and directional-derivative / linearity properties at the BASELINE sweep shape."""
-import os
-
 import numpy as np
 import pytest
 import torch
 
 from oracle import planesweep_oracle as O
-from tests import cases
-from tests.conftest import ROOT
+from tests import cases, harness
 
 pytestmark = pytest.mark.gpu
 T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()     # noqa: E731
 
 
-@pytest.fixture(scope='module')
-def gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'sweep_backward.npz'))
+gold = harness.golden_fixture('sweep_backward.npz')
 
 
 def _cam(w, h):

@@ -17,8 +17,6 @@ Gates are on probabilities (DESIGN.md 'tolerance domain'):
    implementations already differ by 2.5 mm in the first window).
 Measured deviations are written to $NRGBD_PARITY_DIR/parity_configs_<conv_math>.json when that variable is set.
 """
-import contextlib
-import io
 import json
 import os
 
@@ -27,7 +25,7 @@ import pytest
 import torch
 
 from oracle import planesweep_oracle as O
-from tests import cases
+from tests import cases, harness
 from tests.conftest import maxabs, ROOT
 
 pytestmark = pytest.mark.gpu
@@ -40,39 +38,6 @@ TOL_KNET = 5e-4
 TOL_DEPTH_MM = 1.0
 
 
-def cam_torch(cam):
-    c = dict(cam)
-    c['unit_ray_array_2D'] = torch.from_numpy(cam['unit_ray_array_2D'])
-    c['intrinsic_M_cuda'] = torch.from_numpy(cam['intrinsic_M_cuda'])
-    return c
-
-
-def build_model(c, cam, conv_math):
-    from neuralrgbd_b200.models.KVNET import KVNET
-    with contextlib.redirect_stdout(io.StringIO()):
-        m = KVNET(feature_dim=64, cam_intrinsics=cam, d_candi=c['d'], sigma_soft_max=c['sigma'], KVNet_feature_dim=64,
-                  d_upsample_ratio_KV_net=None, t_win_r=c['t_win_r'], if_refined=True)
-    m.load_state_dict({k: torch.from_numpy(np.asarray(v)) for k, v in c['sd'].items()})
-    m = m.to(dev)
-    m.conv_math = conv_math
-    return m
-
-
-def _dump(name, conv_math, rows):
-    d = os.environ.get('NRGBD_PARITY_DIR')
-    if not d:
-        return
-    try:
-        os.makedirs(d, exist_ok=True)
-        path = os.path.join(d, 'parity_configs_%s.json' % conv_math)
-        cur = json.load(open(path)) if os.path.exists(path) else {}
-        cur[name] = rows
-        with open(path, 'w') as f:
-            json.dump(cur, f, indent=1, sort_keys=True)
-    except OSError:
-        pass
-
-
 def _floors(name, n_steps):
     """Per-step fp32-vs-fp32 floor {DPV prob, depth mm} as a running maximum; None where nothing is recorded."""
     rec = {}
@@ -80,7 +45,7 @@ def _floors(name, n_steps):
     if os.path.exists(p):
         for r in json.load(open(p))['steps']:
             rec[r['step']] = (max(r['DPV_prob'], r.get('prior_next_prob', 0.0), r.get('dmap_refined_prob', 0.0)), r['depth_mm'])
-    pc = json.load(open(os.path.join(ROOT, 'tests', 'golden', 'PINNING_configs.json')))['cases']
+    pc = harness.pinning('PINNING_configs.json')
     for k in range(n_steps):
         c = pc.get('cfg/%s/step%d' % (name, k))
         if c and 'oracle_DPV_prob' in c and k not in rec:
@@ -110,8 +75,8 @@ def test_config_stream_free_running_vs_reference(name, conv_math):
     from neuralrgbd_b200.mutils import misc
     gold = _golden(name)
     c = cases.big_case(name)
-    cam = cam_torch(cases.big_cam(O.make_cam_intrinsics, c))
-    model = torch.nn.DataParallel(build_model(c, cam, conv_math), device_ids=[0])       # as test_KVNet.py:163
+    cam = harness.cam_tensors(cases.big_cam(O.make_cam_intrinsics, c))
+    model = torch.nn.DataParallel(harness.engine_kvnet(c, cam, c['sd'], conv_math), device_ids=[0])       # as test_KVNet.py:163
     r = c['t_win_r']
     bv_pred = None
     rows = []
@@ -153,7 +118,7 @@ def test_config_stream_free_running_vs_reference(name, conv_math):
         rw['gate_knet_prob'] = max(TOL_KNET, 4.0 * f_prob)
         rw['gate_depth_mm'] = max(TOL_DEPTH_MM, 4.0 * f_mm)
         rw['floor_prob'], rw['floor_depth_mm'] = f_prob, f_mm
-    _dump(name, conv_math, rows)
+    harness.parity_dump('configs_%s' % conv_math, name, rows)
     msg = ' worst=' + json.dumps(worst)
     assert worst['dnet'] <= TOL_DNET, msg
     for rw in rows:
@@ -175,15 +140,15 @@ def test_config_steady_step_reseeded_with_reference_prior(name, conv_math):
         pytest.skip('prior fixture missing')
     prior = np.load(ppath)['cfg/%s/step0/BV_predict_next_full' % name]
     c = cases.big_case(name)
-    cam = cam_torch(cases.big_cam(O.make_cam_intrinsics, c))
-    model = build_model(c, cam, conv_math)
+    cam = harness.cam_tensors(cases.big_cam(O.make_cam_intrinsics, c))
+    model = harness.engine_kvnet(c, cam, c['sd'], conv_math)
     ref_f, src_f, poses = cases.window(c, c['t_win_r'] + 1)
     with torch.no_grad():
         full = model(T(ref_f), T(src_f), T(poses), torch.zeros(1), cam_intrinsics=[cam], BV_predict=T(prior))
     row = {}
     for nm, a in zip(NAMES4, full):
         row[nm] = maxabs(np.exp(cases.subsample(a.cpu().numpy())), np.exp(gold['cfg/%s/step1/%s' % (name, nm)]))
-    _dump(name + '/reseeded_step1', conv_math, row)
+    harness.parity_dump('configs_%s' % conv_math, name + '/reseeded_step1', row)
     assert row['BV_cur'] <= TOL_DNET and row['dmap_cur_refined'] <= TOL_DNET, row
     # one K-Net step: the default arithmetic sits at north_star's 1e-4 (0.9e-4 .. 1.1e-4 between runs: the BatchNorm sums are
     # accumulated with atomics); the fp32-vs-fp32 floor at this shape is 1.5e-4 (sub-sampled) / 3.0e-4 (full arrays)

@@ -8,15 +8,11 @@ import pytest
 import torch
 
 from oracle import kvnet_oracle as N
+from tests.harness import rel_err
 
 pytestmark = pytest.mark.gpu
 dev = 'cuda:0'
 T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)     # noqa: E731
-
-
-def rel_err(a, b):
-    a = np.asarray(a, np.float64); b = np.asarray(b, np.float64)
-    return float(np.abs(a - b).max() / (np.abs(b).max() + 1e-30))
 
 
 def test_split_f16_pair_keeps_22_bits():

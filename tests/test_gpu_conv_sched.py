@@ -12,6 +12,7 @@ import pytest
 import torch
 
 from oracle import kvnet_oracle as N
+from tests.harness import rel_err
 
 pytestmark = pytest.mark.gpu
 dev = 'cuda:0'
@@ -19,11 +20,6 @@ T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)     # noqa: E731
 
 # nrgbd_dev_conv_h2_set_flags bits: 8 always the 16 x 8 tile, 32 one tile per CTA
 SCHED_FLAGS = (8, 32)
-
-
-def rel_err(a, b):
-    a = np.asarray(a, np.float64); b = np.asarray(b, np.float64)
-    return float(np.abs(a - b).max() / (np.abs(b).max() + 1e-30))
 
 
 def set_flags(flags):

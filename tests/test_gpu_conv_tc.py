@@ -9,15 +9,11 @@ import torch
 
 from oracle import kvnet_oracle as N
 from tests.conftest import maxabs
+from tests.harness import rel_err
 
 pytestmark = pytest.mark.gpu
 dev = 'cuda:0'
 T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)     # noqa: E731
-
-
-def rel_err(a, b):
-    a = np.asarray(a, np.float64); b = np.asarray(b, np.float64)
-    return float(np.abs(a - b).max() / (np.abs(b).max() + 1e-30))
 
 
 def test_split_tf32_is_exact_to_22_bits():

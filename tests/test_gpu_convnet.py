@@ -17,17 +17,13 @@ import torch
 
 from oracle import planesweep_oracle as O
 from oracle import kvnet_oracle as N
-from tests import cases
+from tests import cases, harness
 from tests.conftest import maxabs
+from tests.harness import rel_err
 
 pytestmark = pytest.mark.gpu
 dev = 'cuda:0'
 T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)     # noqa: E731
-
-
-def rel_err(a, b):
-    a = np.asarray(a, np.float64); b = np.asarray(b, np.float64)
-    return float(np.abs(a - b).max() / (np.abs(b).max() + 1e-30))
 
 
 @pytest.mark.parametrize('cfg', [
@@ -110,13 +106,6 @@ def test_pool_and_upsample_vs_oracle():
         assert maxabs(convops.upsample_bilinear_ac(T(s), (64, 96)).cpu().numpy(), N.upsample_bilinear_ac(s, (64, 96))) <= 5e-6
 
 
-def cam_torch(cam):
-    c = dict(cam)
-    c['unit_ray_array_2D'] = torch.from_numpy(cam['unit_ray_array_2D'])
-    c['intrinsic_M_cuda'] = torch.from_numpy(cam['intrinsic_M_cuda'])
-    return c
-
-
 def build_model(c, cam):
     from neuralrgbd_b200.models.KVNET import KVNET
     with contextlib.redirect_stdout(io.StringIO()):
@@ -133,7 +122,7 @@ def test_kvnet_forward_streaming_vs_reference(golden, name, conv_math):
     live-reference fixtures; each step is fed the REFERENCE's prior so deviations do not compound."""
     from neuralrgbd_b200.test_utils.test_KVNet import test as kv_test
     c = cases.kvnet_case(name)
-    cam = cam_torch(cases.cam_for(O.make_cam_intrinsics, c['W'] // 4, c['H'] // 4))
+    cam = harness.cam_tensors(cases.cam_for(O.make_cam_intrinsics, c['W'] // 4, c['H'] // 4))
     base = build_model(c, cam)
     base.conv_math = conv_math        # exact fp32 CUDA-core path / wgmma 3xTF32 tensor-core path: same gates
     model = torch.nn.DataParallel(base, device_ids=[0])      # as test_KVNet.py:163
@@ -189,11 +178,11 @@ def test_kvnet_vs_oracle_first_window(conv_math):
     """Engine vs the numpy oracle on a fresh seed (not in the fixtures)."""
     c = cases.kvnet_case('kvnet_256x320_d8')
     cam_np = cases.cam_for(O.make_cam_intrinsics, c['W'] // 4, c['H'] // 4)
-    model = build_model(c, cam_torch(cam_np))
+    model = build_model(c, harness.cam_tensors(cam_np))
     model.conv_math = conv_math
     ref_f, src_f, poses = cases.window(c, 3)
     with torch.no_grad():
-        got = model(T(ref_f), T(src_f), T(poses), torch.zeros(1), cam_intrinsics=[cam_torch(cam_np)], BV_predict=None)
+        got = model(T(ref_f), T(src_f), T(poses), torch.zeros(1), cam_intrinsics=[harness.cam_tensors(cam_np)], BV_predict=None)
     orc = N.kvnet_forward(c['sd'], ref_f, src_f, poses, cam_np, c['d'], c['sigma'])
     assert maxabs(np.exp(got[2].cpu().numpy()), np.exp(orc[2])) <= 1e-4
     assert maxabs(np.exp(got[0].cpu().numpy()), np.exp(orc[0])) <= 1e-4
@@ -204,7 +193,7 @@ def test_kvnet_load_state_dict_after_forward(conv_math):
     """New weights loaded into a module whose engine has run reach every packed copy of them: the next K-Net step
     matches a fresh module built with those weights (the f16 modes keep K-Net's last layer in a second, per-tap packing)."""
     c = cases.kvnet_case('kvnet_256_d16')
-    cam = cam_torch(cases.cam_for(O.make_cam_intrinsics, c['W'] // 4, c['H'] // 4))
+    cam = harness.cam_tensors(cases.cam_for(O.make_cam_intrinsics, c['W'] // 4, c['H'] // 4))
     rng = np.random.RandomState(11)
     sd_b = {k: (v * (1 + 0.1 * rng.standard_normal(v.shape))).astype(v.dtype) if v.dtype.kind == 'f' else v
             for k, v in ((k, np.asarray(v)) for k, v in c['sd'].items())}

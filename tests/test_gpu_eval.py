@@ -12,13 +12,8 @@
    in f16x3 a steady eval step launches exactly 13 fewer BatchNorm-pass kernels than a steady train step.
 Measured deviations are written to $NRGBD_PARITY_DIR/parity_eval.json when that variable is set.
 """
-import contextlib
-import io
 import json
 import math
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -26,16 +21,13 @@ import torch
 
 from oracle import kvnet_oracle as N
 from oracle import planesweep_oracle as O
-from tests import cases
+from tests import cases, harness
 from tests import oracle_eval as E
-from tests.conftest import ROOT, maxabs
+from tests.conftest import maxabs
+from tests.harness import NAMES4, T, rel_err
 
 pytestmark = pytest.mark.gpu
-dev = 'cuda:0'
-T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)     # noqa: E731
-NAMES4 = ['dmap_cur_refined', 'dmap_refined', 'BV_cur', 'DPV']
 SUB_LIMIT = 8000          # the fixture's strided samples (make_golden_eval.py)
-DEPTH_LIMIT = 2000
 TOL_SUMSQ_REL = 1e-4      # full-array check: relative deviation of the sum of squared probabilities
 TOL_FIRST = 1e-4
 TOL_DEPTH_MM = 1.0
@@ -44,29 +36,9 @@ TOL_KNET = 5e-4
 MODES = ['f16x3', 'tf32x3', 'fp32']
 
 
-def rel_err(a, b):
-    a = np.asarray(a, np.float64); b = np.asarray(b, np.float64)
-    return float(np.abs(a - b).max() / (np.abs(b).max() + 1e-30))
-
-
 def set_flags(flags):
     from neuralrgbd_b200 import _lib
     _lib.dev_lib().nrgbd_dev_conv_h2_set_flags(flags)
-
-
-def _dump(key, row):
-    d = os.environ.get('NRGBD_PARITY_DIR')
-    if not d:
-        return
-    try:
-        os.makedirs(d, exist_ok=True)
-        path = os.path.join(d, 'parity_eval.json')
-        cur = json.load(open(path)) if os.path.exists(path) else {}
-        cur[key] = row
-        with open(path, 'w') as f:
-            json.dump(cur, f, indent=1, sort_keys=True)
-    except OSError:
-        pass
 
 
 # ---- op level ----------------------------------------------------------------------------------------------------------
@@ -149,61 +121,12 @@ def _case(name):
     return c, cam
 
 
-def _cam_t(cam):
-    return dict(cam, unit_ray_array_2D=torch.from_numpy(cam['unit_ray_array_2D']), intrinsic_M_cuda=torch.from_numpy(cam['intrinsic_M_cuda']))
-
-
-def _gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'eval_outputs.npz'))
-
-
-def _pin():
-    return json.load(open(os.path.join(ROOT, 'tests', 'golden', 'PINNING_eval.json')))['cases']
-
-
 def _eval_sd(c, gold, name):
     """The case's weights with the running statistics the reference produced (make_golden_eval.py)."""
     sd = {k: np.asarray(v) for k, v in c['sd'].items()}
     pre = 'eval/%s/rs/' % name
     sd.update({k[len(pre):]: np.asarray(gold[k]) for k in gold.files if k.startswith(pre)})
     return sd
-
-
-def _model(c, cam_t, sd, conv_math):
-    from neuralrgbd_b200.models.KVNET import KVNET
-    with contextlib.redirect_stdout(io.StringIO()):
-        m = KVNET(feature_dim=64, cam_intrinsics=cam_t, d_candi=c['d'], sigma_soft_max=c['sigma'], KVNet_feature_dim=64,
-                  d_upsample_ratio_KV_net=None, t_win_r=c['t_win_r'], if_refined=True)
-    m.load_state_dict({k: torch.from_numpy(v) for k, v in sd.items()})
-    m = m.to(dev)
-    m.conv_math = conv_math
-    return m
-
-
-def _forward(m, c, cam_t, step, prior):
-    ref_f, src_f, poses = cases.window(c, c['t_win_r'] + step)
-    with torch.no_grad():
-        return m(T(ref_f), T(src_f), T(poses), torch.zeros(1), cam_intrinsics=[cam_t], BV_predict=None if prior is None else T(prior))
-
-
-def _compare(gold, key, full, d):
-    """Max-abs probability deviation on the stored samples (the first window stores BV_cur / dmap_cur_refined, which its
-    filtered outputs equal; a steady step its filtered DPV / dmap_refined), the sum of squared probabilities of every full
-    array, and the expected depth in mm."""
-    row = {}
-    aliases = {'DPV': 'BV_cur', 'dmap_refined': 'dmap_cur_refined'} if key.endswith('/step0') else {}
-    for nm, a in zip(NAMES4, full):
-        a = a.cpu().numpy()
-        assert np.isfinite(a).all(), (key, nm)
-        k = '%s/%s' % (key, aliases.get(nm, nm))
-        if k in gold.files:
-            row[nm] = maxabs(np.exp(cases.subsample_to(a, SUB_LIMIT)), np.exp(gold[k]))
-        st, gs = cases.stats(np.exp(a.astype(np.float64))), gold['%s/%s_stats' % (key, nm)]
-        row[nm + '_sumsq_rel'] = abs(st[1] - gs[1]) / gs[1]
-    from neuralrgbd_b200.mutils import misc
-    dep = misc.depth_val_regression(full[3], d).cpu().numpy()
-    row['depth_mm'] = 1000.0 * maxabs(cases.subsample_to(dep, DEPTH_LIMIT), gold[key + '/depth'])
-    return row
 
 
 def _knet_gate(pin, name, key, conv_math):
@@ -220,31 +143,25 @@ def _knet_gate(pin, name, key, conv_math):
 RESEEDED = [('kvnet_256_d16', 1), ('kvnet_256_d16', 2), ('c23_640x480_d64_v4_stream30', 1)]
 
 
-def _prior(name, step):
-    if name in cases.KVNET_CASES:
-        return np.load(os.path.join(ROOT, 'tests', 'golden', 'reference_outputs.npz'))['kvnet/%s/step%d/BV_predict_next_full' % (name, step - 1)]
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'configs_priors_%s.npz' % name))['cfg/%s/step0/BV_predict_next_full' % name]
-
-
 @pytest.mark.parametrize('conv_math', MODES)
 @pytest.mark.parametrize('name', ['kvnet_256_d16', 'c23_640x480_d64_v4_stream30'])
 def test_engine_eval_vs_reference(name, conv_math):
-    gold, pin = _gold(), _pin()
+    gold, pin = harness.golden('eval_outputs.npz'), harness.pinning('PINNING_eval.json')
     c, cam = _case(name)
-    cam_t = _cam_t(cam)
-    m = _model(c, cam_t, _eval_sd(c, gold, name), conv_math).eval()
+    cam_t = harness.cam_tensors(cam)
+    m = harness.engine_kvnet(c, cam_t, _eval_sd(c, gold, name), conv_math).eval()
     before = {k: v.clone() for k, v in m.state_dict().items()}
     rows = {}
-    full = _forward(m, c, cam_t, 0, None)
-    rows['step0'] = r0 = _compare(gold, 'eval/%s/step0' % name, full, c['d'])
+    full = harness.engine_forward(m, c, cam_t, 0, None)[1]
+    rows['step0'] = r0 = harness.compare_outputs(gold, 'eval/%s/step0' % name, full, c['d'])
     for nm, s in RESEEDED:
         if nm != name:
             continue
         key = 'eval/%s/step%d' % (name, s)
-        full = _forward(m, c, cam_t, s, _prior(name, s))
-        rows['step%d' % s] = r = _compare(gold, key, full, c['d'])
+        full = harness.engine_forward(m, c, cam_t, s, harness.reference_prior(name, s))[1]
+        rows['step%d' % s] = r = harness.compare_outputs(gold, key, full, c['d'])
         r['gate'] = _knet_gate(pin, name, key, conv_math)
-    _dump('%s/%s' % (name, conv_math), rows)
+    harness.parity_dump('eval', '%s/%s' % (name, conv_math), rows)
     msg = json.dumps(rows)
     assert max(r0[nm] for nm in NAMES4) <= TOL_FIRST and r0['depth_mm'] <= TOL_DEPTH_MM, msg
     for k, r in rows.items():
@@ -263,18 +180,18 @@ def test_engine_eval_train_eval_on_one_engine():
     """eval -> train -> eval: the train forward matches the train-mode fixture and updates the running statistics; the
     second eval forward normalises with the updated statistics (checked against the eval oracle fed those buffers)."""
     name = 'kvnet_256_d16'
-    gold = _gold()
-    ref_gold = np.load(os.path.join(ROOT, 'tests', 'golden', 'reference_outputs.npz'))
+    gold = harness.golden('eval_outputs.npz')
+    ref_gold = harness.golden('reference_outputs.npz')
     c, cam = _case(name)
-    cam_t = _cam_t(cam)
-    m = _model(c, cam_t, {k: np.asarray(v) for k, v in c['sd'].items()}, 'f16x3')
-    prior_eval = _prior(name, 1)
+    cam_t = harness.cam_tensors(cam)
+    m = harness.engine_kvnet(c, cam_t, {k: np.asarray(v) for k, v in c['sd'].items()}, 'f16x3')
+    prior_eval = harness.reference_prior(name, 1)
     m.eval()
-    e1 = _forward(m, c, cam_t, 1, prior_eval)
+    e1 = harness.engine_forward(m, c, cam_t, 1, prior_eval)[1]
     # train mode, the steady step of the train fixture (its own prior): K-Net's BatchNorm3d and the downsample layers update
     m.train()
     sd0 = {k: v.clone() for k, v in m.state_dict().items()}
-    t = _forward(m, c, cam_t, 1, prior_eval)
+    t = harness.engine_forward(m, c, cam_t, 1, prior_eval)[1]
     for nm, a in zip(NAMES4, t):
         e = maxabs(np.exp(cases.subsample(a.cpu().numpy())), np.exp(ref_gold['kvnet/%s/step1/%s' % (name, nm)]))
         assert e <= (1e-4 if nm in ('BV_cur', 'dmap_cur_refined') else 5e-4), (nm, e)
@@ -282,7 +199,7 @@ def test_engine_eval_train_eval_on_one_engine():
     moved = [k for k in sd0 if k.endswith('running_mean') and not k.startswith('d_net.') and not torch.equal(sd0[k], sd1[k])]
     assert len(moved) == 13, moved
     m.eval()
-    e2 = _forward(m, c, cam_t, 1, prior_eval)
+    e2 = harness.engine_forward(m, c, cam_t, 1, prior_eval)[1]
     assert not torch.equal(e1[3], e2[3])                        # the updated statistics are used
     sd2 = m.state_dict()
     assert all(torch.equal(sd1[k].cpu(), sd2[k].cpu()) for k in sd1)
@@ -291,22 +208,16 @@ def test_engine_eval_train_eval_on_one_engine():
                         BV_predict=prior_eval, training=False)
     sub = lambda a: cases.subsample_to(a, SUB_LIMIT)     # noqa: E731  (sampled as every other comparison here)
     row = {nm: maxabs(np.exp(sub(a.cpu().numpy())), np.exp(sub(b))) for nm, a, b in zip(NAMES4, e2, o)}
-    _dump('%s/eval_train_eval' % name, row)
+    harness.parity_dump('eval', '%s/eval_train_eval' % name, row)
     assert row['BV_cur'] <= TOL_FIRST and row['dmap_cur_refined'] <= TOL_FIRST, row
     assert row['DPV'] <= 5e-4 and row['dmap_refined'] <= 5e-4, row
 
 
 def test_reference_test_runs_eval_model_unmodified():
-    from oracle import fetch_reference
-    ref_code = fetch_reference.code_dir()
-    assert ref_code, 'no copy of the reference: oracle/_ref is made by __graft_entry__.build() (oracle/fetch_reference.py)'
-    r = subprocess.run([sys.executable, os.path.join(ROOT, 'tests', 'dropin_eval_driver.py'), ref_code],
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, (r.stdout[-1500:], r.stderr[-3000:])
-    out = json.loads(r.stdout.strip().splitlines()[-1])
-    _dump('dropin', out)
+    out = harness.run_reference_driver('step', 'eval', timeout=900)
+    harness.parity_dump('eval', 'dropin', out)
     assert out['class'] == 'neuralrgbd_b200.models.KVNET' and out['training'] is False
-    pin = _pin()
+    pin = harness.pinning('PINNING_eval.json')
     assert out['steps'][0]['DPV'] <= TOL_FIRST, out
     for s, st in enumerate(out['steps'][1:], 1):                     # re-seeded K-Net steps: the gate of the engine test
         assert st['DPV'] <= _knet_gate(pin, 'kvnet_256_d16', 'eval/kvnet_256_d16/step%d' % s, 'f16x3'), out
@@ -317,26 +228,26 @@ def test_eval_step_has_13_fewer_bn_passes():
     from torch.profiler import profile, ProfilerActivity
     from neuralrgbd_b200 import _lib
     name = 'kvnet_256_d16'
-    gold = _gold()
+    gold = harness.golden('eval_outputs.npz')
     c, cam = _case(name)
-    cam_t = _cam_t(cam)
-    m = _model(c, cam_t, _eval_sd(c, gold, name), 'f16x3')
-    prior = _prior(name, 1)
+    cam_t = harness.cam_tensors(cam)
+    m = harness.engine_kvnet(c, cam_t, _eval_sd(c, gold, name), 'f16x3')
+    prior = harness.reference_prior(name, 1)
 
     def count(training):
         m.train(training)
-        _forward(m, c, cam_t, 1, prior)                       # warm (eager) step of this mode
+        harness.engine_forward(m, c, cam_t, 1, prior)                       # warm (eager) step of this mode
         ent = next(iter(m._engines.values()))
         _lib.lib().nrgbd_kvnet_set_option(ent['h'], b'use_graph', 0)     # kernels by name, outside a graph
         torch.cuda.synchronize()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            _forward(m, c, cam_t, 1, prior)
+            harness.engine_forward(m, c, cam_t, 1, prior)
             torch.cuda.synchronize()
         names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
         _lib.lib().nrgbd_kvnet_set_option(ent['h'], b'use_graph', 1)
         return sum('bn_apply' in n for n in names), sum('conv_wg_kernel' in n for n in names)
     bn_train, conv_train = count(True)
     bn_eval, conv_eval = count(False)
-    _dump('bn_launches', {'train': bn_train, 'eval': bn_eval, 'conv_train': conv_train, 'conv_eval': conv_eval})
+    harness.parity_dump('eval', 'bn_launches', {'train': bn_train, 'eval': bn_eval, 'conv_train': conv_train, 'conv_eval': conv_eval})
     assert bn_train - bn_eval == 13, (bn_train, bn_eval)
     assert conv_train == conv_eval, (conv_train, conv_eval)

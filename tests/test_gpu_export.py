@@ -7,16 +7,13 @@ import pytest
 import torch
 
 from oracle import export_oracle as E
-from tests import cases
-from tests.conftest import ROOT
+from tests import cases, harness
 from tests.test_oracle_export import parse_pgm16
 
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(scope='module')
-def gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'export_outputs.npz'))
+gold = harness.golden_fixture('export_outputs.npz')
 
 
 @pytest.mark.parametrize('name', cases.EXPORT_CASES)

@@ -14,14 +14,9 @@
    f16x3 and the pool is smaller; the reference's unmodified test() runs with conv_math='f16'.
 Measured deviations are written to $NRGBD_PARITY_DIR/parity_f16.json when that variable is set.
 """
-import contextlib
 import ctypes
-import io
 import json
 import math
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -29,37 +24,16 @@ import torch
 import torch.nn.functional as Fn
 
 from oracle import planesweep_oracle as O
-from tests import cases
+from tests import cases, harness
 from tests import cases_f16 as CF
-from tests.conftest import ROOT, maxabs
+from tests.conftest import maxabs
+from tests.harness import DEV as dev, T, rel_err
 
 pytestmark = pytest.mark.gpu
-dev = 'cuda:0'
-T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)     # noqa: E731
 TOL_REL = 6e-6
 G16X3_FIRST = 1e-4        # f16x3's gates: first windows (probability), test_gpu_twin.py / test_gpu_eval.py
 G16X3_STEADY = 3e-4       # the largest of f16x3's steady-step gates at these shapes (twice the pinned fp32 floor)
 G16X3_DEPTH_MM = 1.0
-
-
-def _dump(key, row):
-    d = os.environ.get('NRGBD_PARITY_DIR')
-    if not d:
-        return
-    try:
-        os.makedirs(d, exist_ok=True)
-        path = os.path.join(d, 'parity_f16.json')
-        cur = json.load(open(path)) if os.path.exists(path) else {}
-        cur[key] = row
-        with open(path, 'w') as f:
-            json.dump(cur, f, indent=1, sort_keys=True)
-    except OSError:
-        pass
-
-
-def rel_err(a, b):
-    a = np.asarray(a, np.float64); b = np.asarray(b, np.float64)
-    return float(np.abs(a - b).max() / (np.abs(b).max() + 1e-30))
 
 
 def r16(a):
@@ -220,28 +194,9 @@ def test_split_bn_and_volume_with_null_lo():
 
 
 # ---- engine ------------------------------------------------------------------------------------------------------------
-def _gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'f16_outputs.npz'))
-
-
-def _pin():
-    return json.load(open(os.path.join(ROOT, 'tests', 'golden', 'PINNING_f16.json')))['cases']
-
-
-def _cam_t(cam):
-    return dict(cam, unit_ray_array_2D=torch.from_numpy(cam['unit_ray_array_2D']), intrinsic_M_cuda=torch.from_numpy(cam['intrinsic_M_cuda']))
-
-
-def _model(c, cam_t, conv_math):
-    from neuralrgbd_b200.models.KVNET import KVNET
-    with contextlib.redirect_stdout(io.StringIO()):
-        m = KVNET(feature_dim=64, cam_intrinsics=cam_t, d_candi=c['d'], sigma_soft_max=c['sigma'], KVNet_feature_dim=64,
-                  d_upsample_ratio_KV_net=None, t_win_r=c['t_win_r'])
-    m.load_state_dict({k: torch.from_numpy(v) for k, v in CF.state_dict(c).items()}, strict=True)
-    m = m.to(dev)
-    m.conv_math = conv_math
-    m.train(CF.MODE[c['name']] == 'train')
-    return m
+def _case_model(c, cam_t, conv_math):
+    """The engine KVNET of f16 case `c`: the case's state dict and train / eval mode."""
+    return harness.engine_kvnet(c, cam_t, CF.state_dict(c), conv_math, train=CF.MODE[c['name']] == 'train')
 
 
 class _Recorder(torch.nn.Module):
@@ -258,7 +213,7 @@ class _Recorder(torch.nn.Module):
 def _run(c, cam_t, conv_math):
     """The case's steps through the package's test() (re-seeded or free-running as the fixture) -> list of 4 outputs."""
     from neuralrgbd_b200.test_utils import test_KVNet
-    rec = _Recorder(_model(c, cam_t, conv_math))
+    rec = _Recorder(_case_model(c, cam_t, conv_math))
     outs, prior = [], None
     for k in range(c['n_steps']):
         if k and c['name'] not in CF.FREE_RUNNING:
@@ -286,9 +241,9 @@ def _depth(a, d):
 
 @pytest.mark.parametrize('name', CF.F16_CASES)
 def test_engine_f16_vs_emulated_reference(name):
-    gold, pin = _gold(), _pin()
+    gold, pin = harness.golden('f16_outputs.npz'), harness.pinning('PINNING_f16.json')
     c = CF.f16_case(name)
-    cam_t = _cam_t(CF.cam(O.make_cam_intrinsics, c))
+    cam_t = harness.cam_tensors(CF.cam(O.make_cam_intrinsics, c))
     outs = _run(c, cam_t, 'f16')
     rows = {}
     for k, full in enumerate(outs):
@@ -314,7 +269,7 @@ def test_engine_f16_vs_emulated_reference(name):
         row['depth_fp32_gate_mm'] = 2.0 * p['f16_vs_fp32']['DPV']['depth_mm'] + row['depth_gate_mm']
         row['depth_ref_tf32_vs_fp32_mm'] = p['tf32_vs_fp32']['DPV']['depth_mm']
         rows['step%d' % k] = row
-    _dump('engine/%s' % name, rows)
+    harness.parity_dump('f16', 'engine/%s' % name, rows)
     print(json.dumps(rows, indent=1))
     msg = json.dumps(rows)
     for r in rows.values():
@@ -325,24 +280,22 @@ def test_engine_f16_vs_emulated_reference(name):
         assert r['depth_mm'] <= r['depth_gate_mm'] and r['depth_fp32_mm'] <= r['depth_fp32_gate_mm'], msg
 
 
-def _forward(m, c, cam_t, step, prior):
-    ref_f, src_f, poses = cases.window(c, c['t_win_r'] + step)
-    with torch.no_grad():
-        return [t.clone() for t in m(T(ref_f), T(src_f), T(poses), torch.zeros(1), cam_intrinsics=[cam_t],
-                                     BV_predict=None if prior is None else T(prior))]
+def _outputs(m, c, cam_t, step, prior):
+    """harness.engine_forward's outputs, cloned: the tests below compare the outputs of successive forwards."""
+    return [t.clone() for t in harness.engine_forward(m, c, cam_t, step, prior)[1]]
 
 
 def test_f16x3_unchanged_after_f16():
     """One module in .eval() (no atomics: deterministic): f16x3, then f16, then f16x3 again - the f16x3 outputs of a first
     window and a steady step are bit-identical to the first run's, and f16 differs from them."""
     c = CF.f16_case('eval_256_d16')
-    cam_t = _cam_t(CF.cam(O.make_cam_intrinsics, c))
+    cam_t = harness.cam_tensors(CF.cam(O.make_cam_intrinsics, c))
     prior = CF.reseed_prior('eval_256_d16', 1)
-    m = _model(c, cam_t, 'f16x3')
+    m = _case_model(c, cam_t, 'f16x3')
     runs = {}
     for i, mode in enumerate(['f16x3', 'f16', 'f16x3']):
         m.conv_math = mode
-        runs[i] = _forward(m, c, cam_t, 0, None) + _forward(m, c, cam_t, 1, prior)
+        runs[i] = _outputs(m, c, cam_t, 0, None) + _outputs(m, c, cam_t, 1, prior)
     assert all(torch.equal(a, b) for a, b in zip(runs[0], runs[2]))
     assert not torch.equal(runs[0][3], runs[1][3]) and not torch.equal(runs[0][7], runs[1][7])
 
@@ -350,14 +303,14 @@ def test_f16x3_unchanged_after_f16():
 def _launches(c, cam_t, conv_math, prior):
     from torch.profiler import profile, ProfilerActivity
     from neuralrgbd_b200 import _lib
-    m = _model(c, cam_t, conv_math)
-    _forward(m, c, cam_t, 0, None)
-    _forward(m, c, cam_t, 1, prior)
+    m = _case_model(c, cam_t, conv_math)
+    _outputs(m, c, cam_t, 0, None)
+    _outputs(m, c, cam_t, 1, prior)
     ent = next(iter(m._engines.values()))
     _lib.lib().nrgbd_kvnet_set_option(ent['h'], b'use_graph', 0)
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        _forward(m, c, cam_t, 1, prior)
+        _outputs(m, c, cam_t, 1, prior)
         torch.cuda.synchronize()
     names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
     counts = {k: sum(k in n for n in names) for k in ('conv_igemm_kernel', 'conv_wg_kernel', 'split_f16_pair_kernel', 'bn_apply_stats_kernel')}
@@ -369,10 +322,10 @@ def test_f16_takes_the_f16x3_path():
     """A steady 256x256 frame launches the same kernels in f16 as in f16x3: the same tensor-core convolutions, fp32-path
     convolutions, split passes and BatchNorm passes."""
     c = CF.f16_case('eval_256_d16')
-    cam_t = _cam_t(CF.cam(O.make_cam_intrinsics, c))
+    cam_t = harness.cam_tensors(CF.cam(O.make_cam_intrinsics, c))
     prior = CF.reseed_prior('eval_256_d16', 1)
     a, b = _launches(c, cam_t, 'f16x3', prior), _launches(c, cam_t, 'f16', prior)
-    _dump('launches', {'f16x3': a, 'f16': b})
+    harness.parity_dump('f16', 'launches', {'f16x3': a, 'f16': b})
     assert a == b, (a, b)
     assert a['conv_wg_kernel'] > 0 and a['conv_igemm_kernel'] == 1
 
@@ -382,39 +335,33 @@ def test_f16_workspace_smaller_at_c2_c3():
     convolutions read: strictly smaller in f16 than in f16x3."""
     from neuralrgbd_b200 import _lib
     c = CF.f16_case('c2_640x480_d64')
-    cam_t = _cam_t(CF.cam(O.make_cam_intrinsics, c))
+    cam_t = harness.cam_tensors(CF.cam(O.make_cam_intrinsics, c))
     prior = CF.reseed_prior('c2_640x480_d64', 1)
     ws = {}
     for mode in ('f16x3', 'f16'):
-        m = _model(c, cam_t, mode)
-        _forward(m, c, cam_t, 0, None)
-        _forward(m, c, cam_t, 1, prior)
+        m = _case_model(c, cam_t, mode)
+        _outputs(m, c, cam_t, 0, None)
+        _outputs(m, c, cam_t, 1, prior)
         ent = next(iter(m._engines.values()))
         ws[mode] = _lib.lib().nrgbd_kvnet_workspace_bytes(ent['h'])
         del m
         torch.cuda.empty_cache()
-    _dump('workspace_bytes', ws)
+    harness.parity_dump('f16', 'workspace_bytes', ws)
     assert 0 < ws['f16'] < ws['f16x3'], ws
 
 
 def test_bad_conv_math_lists_all_modes():
     c = CF.f16_case('r1_256_d16')
-    cam_t = _cam_t(CF.cam(O.make_cam_intrinsics, c))
-    m = _model(c, cam_t, 'f8')
+    cam_t = harness.cam_tensors(CF.cam(O.make_cam_intrinsics, c))
+    m = _case_model(c, cam_t, 'f8')
     with pytest.raises(ValueError, match="'fp32', 'tf32x3', 'f16x3' or 'f16'"):
-        _forward(m, c, cam_t, 0, None)
+        _outputs(m, c, cam_t, 0, None)
 
 
 def test_reference_test_runs_unmodified_in_f16():
-    from oracle import fetch_reference
-    ref_code = fetch_reference.code_dir()
-    assert ref_code, 'no copy of the reference: oracle/_ref is made by __graft_entry__.build() (oracle/fetch_reference.py)'
-    r = subprocess.run([sys.executable, os.path.join(ROOT, 'tests', 'dropin_f16_driver.py'), ref_code],
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, (r.stdout[-1500:], r.stderr[-3000:])
-    out = json.loads(r.stdout.strip().splitlines()[-1])
-    _dump('dropin', out)
-    pin = _pin()
+    out = harness.run_reference_driver('step', 'f16', timeout=900)
+    harness.parity_dump('f16', 'dropin', out)
+    pin = harness.pinning('PINNING_f16.json')
     assert out['class'] == 'neuralrgbd_b200.models.KVNET' and out['conv_math'] == 'f16'
     assert len(out['steps']) == 2 and all(s['prior_finite'] for s in out['steps']), out
     for k, s in enumerate(out['steps']):

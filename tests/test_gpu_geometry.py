@@ -17,19 +17,13 @@ import torch
 
 from oracle import planesweep_oracle as O
 from tests import cases
+from tests.harness import cam_tensors
 from tests.conftest import maxabs
 
 pytestmark = pytest.mark.gpu
 
 dev = 'cuda:0'
 T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)     # noqa: E731
-
-
-def cam_torch(cam):
-    c = dict(cam)
-    c['unit_ray_array_2D'] = torch.from_numpy(cam['unit_ray_array_2D'])
-    c['intrinsic_M_cuda'] = torch.from_numpy(cam['intrinsic_M_cuda'])
-    return c
 
 
 @pytest.fixture(scope='module')
@@ -42,7 +36,7 @@ def H():
 def test_sweep_vs_oracle_and_reference(H, golden, name):
     c = cases.sweep_case(name)
     cam = cases.cam_for(O.make_cam_intrinsics, c['w'], c['h'])
-    got = H.est_swp_volume_v4(T(c['ref']), T(c['src']), c['d'], T(c['R']), T(c['t']), cam_torch(cam), c['sigma'],
+    got = H.est_swp_volume_v4(T(c['ref']), T(c['src']), c['d'], T(c['R']), T(c['t']), cam_tensors(cam), c['sigma'],
                               feat_dist=c['feat_dist'])
     assert got.shape == (1, len(c['d']), c['h'], c['w']) and got.dtype == torch.float32 and got.is_cuda
     got = got.cpu().numpy()
@@ -60,7 +54,7 @@ def test_sweep_bad_metric_raises(H):
     c = cases.sweep_case('ragged_v3_d7_c5')
     cam = cases.cam_for(O.make_cam_intrinsics, c['w'], c['h'])
     with pytest.raises(Exception, match='undefined metric'):
-        H.est_swp_volume_v4(T(c['ref']), T(c['src']), c['d'], T(c['R']), T(c['t']), cam_torch(cam), 10., 'L3')
+        H.est_swp_volume_v4(T(c['ref']), T(c['src']), c['d'], T(c['R']), T(c['t']), cam_tensors(cam), 10., 'L3')
 
 
 def test_sweep_inputs_not_mutated_and_noncontiguous_poses(H):
@@ -70,8 +64,8 @@ def test_sweep_inputs_not_mutated_and_noncontiguous_poses(H):
     P = T(poses[None])
     ref, src = T(c['ref']), T(c['src'])
     ref0, src0 = ref.clone(), src.clone()
-    a = H.est_swp_volume_v4(ref, src, c['d'], P[0, :, :3, :3], P[0, :, :3, 3], cam_torch(cam), c['sigma'])
-    b = H.est_swp_volume_v4(ref, src, c['d'], T(c['R']), T(c['t']), cam_torch(cam), c['sigma'])
+    a = H.est_swp_volume_v4(ref, src, c['d'], P[0, :, :3, :3], P[0, :, :3, 3], cam_tensors(cam), c['sigma'])
+    b = H.est_swp_volume_v4(ref, src, c['d'], T(c['R']), T(c['t']), cam_tensors(cam), c['sigma'])
     assert torch.equal(a, b) and torch.equal(ref, ref0) and torch.equal(src, src0)
 
 
@@ -87,7 +81,7 @@ def test_sweep_full_size_properties(H):
     src = np.repeat(ref[:, None], V, axis=1)
     d = synth.d_candidates(D)
     R = np.tile(np.eye(3, dtype=np.float32), (V, 1, 1)); t = np.zeros((V, 3), np.float32)
-    c0 = H.est_swp_volume_v4(T(ref), T(src), d, T(R), T(t), cam_torch(cam), 10.)
+    c0 = H.est_swp_volume_v4(T(ref), T(src), d, T(R), T(t), cam_tensors(cam), 10.)
     assert float(c0.max()) <= 1e-8
     # translated views of a fronto-parallel plane at depth d[k]: src_v(u) = ref(u - fx*tx_v/d_k)
     k = 20
@@ -103,7 +97,7 @@ def test_sweep_full_size_properties(H):
         x0 = np.floor(x).astype(int); fr = (x - x0).astype(np.float32)
         srcs.append(big[:, :, x0] * (1 - fr) + big[:, :, x0 + 1] * fr)
     src2 = np.stack(srcs)[None].astype(np.float32)
-    c2 = H.est_swp_volume_v4(T(ref2), T(src2), d, T(R), T(t2), cam_torch(cam), 10.)
+    c2 = H.est_swp_volume_v4(T(ref2), T(src2), d, T(R), T(t2), cam_tensors(cam), 10.)
     bv = dpv.log_softmax_planes(c2, sign=-1.0)
     p = bv.exp()
     assert float((p.sum(1) - 1).abs().max()) <= 1e-5
@@ -116,7 +110,7 @@ def test_warp_vs_oracle_and_reference(H, golden, name):
     c = cases.warp_case(name)
     cam = cases.cam_for(O.make_cam_intrinsics, c['w'], c['h'])
     got = H.warp_img_feats_v3([T(i) for i in c['imgs']], c['d'], [T(r) for r in c['R']], [T(t) for t in c['t']],
-                              cam_torch(cam))
+                              cam_tensors(cam))
     assert isinstance(got, list) and len(got) == len(c['imgs'])
     assert got[0].shape == (3, len(c['d']), c['h'], c['w'])
     got = np.stack([g.cpu().numpy() for g in got])
@@ -135,7 +129,7 @@ def test_warp_tensor_branch_and_wide_channels(H):
     rng = np.random.RandomState(9)
     from neuralrgbd_b200 import synth
     img = synth.smooth_image(rng, 6, c['h'], c['w'])[None]
-    got = H.warp_img_feats_v3(T(img), c['d'], T(c['R'][0]), T(c['t'][0]), cam_torch(cam))
+    got = H.warp_img_feats_v3(T(img), c['d'], T(c['R'][0]), T(c['t'][0]), cam_tensors(cam))
     assert got.shape == (6, len(c['d']), c['h'], c['w'])
     orc = O.warp_img_feats_v3([img], c['d'], [c['R'][0]], [c['t'][0]], cam)[0]
     assert maxabs(got.cpu().numpy(), orc) <= 2e-5
@@ -145,14 +139,14 @@ def test_warp_tensor_branch_and_wide_channels(H):
 def test_resample_vs_oracle_and_reference(H, golden, name):
     c = cases.resample_case(name)
     cam = cases.cam_for(O.make_cam_intrinsics, c['w'], c['h'])
-    got = H.resample_vol_cuda(T(c['vol']), T(c['rel']), cam_torch(cam), c['d'], d_candi_new=c['d_new'],
+    got = H.resample_vol_cuda(T(c['vol']), T(c['rel']), cam_tensors(cam), c['d'], d_candi_new=c['d_new'],
                               padding_value=c['pad'])
     assert got.shape == c['vol'].shape[1:]
     got = got.cpu().numpy()
     orc = O.resample_vol_cuda(c['vol'], c['rel'], cam, c['d'], d_candi_new=c['d_new'], padding_value=c['pad'])
     assert maxabs(got, orc) <= 1e-5
     assert maxabs(cases.subsample(got), golden['resample/%s/vol' % name]) <= 1e-5
-    clamped = H.resample_vol_cuda(T(c['vol']), T(c['rel']), cam_torch(cam), c['d'], d_candi_new=c['d_new'],
+    clamped = H.resample_vol_cuda(T(c['vol']), T(c['rel']), cam_tensors(cam), c['d'], d_candi_new=c['d_new'],
                                   padding_value=c['pad'], clamp=(-1000., 0.)).cpu().numpy()
     assert maxabs(clamped, np.clip(got, -1000., 0.)) == 0.0
 

@@ -7,20 +7,14 @@
  * Plain inputs, inputs that require grad and torch.no_grad() give the same launches and bit-identical values; two
    runs give identical results; the reference's asserts are kept.
  * The reference's own models.KVNET.KVNET(refineNet_name='DGF') trained under train_utils/train_KVNet.py's L1 loss with
-   the mirrors and GuidedFilter patched in, against the unpatched reference (tests/gf_kvnet_driver.py).
+   the mirrors and GuidedFilter patched in, against the unpatched reference (tests/reference_driver.py grad gf).
 Measured deviations are written to $NRGBD_PARITY_DIR/parity_gf.json when that variable is set.
 """
-import json
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
 
-from tests import cases_gf as CG, oracle_gf as OG
-from tests.conftest import ROOT
+from tests import cases_gf as CG, oracle_gf as OG, harness
 from tests.test_oracle_gf import sumsq_allowance
 
 pytestmark = pytest.mark.gpu
@@ -36,29 +30,8 @@ REL = 2e-5
 FLOOR_X = 3.0
 
 
-def _dump(key, row):
-    d = os.environ.get('NRGBD_PARITY_DIR')
-    if not d:
-        return
-    try:
-        os.makedirs(d, exist_ok=True)
-        path = os.path.join(d, 'parity_gf.json')
-        cur = json.load(open(path)) if os.path.exists(path) else {}
-        cur[key] = row
-        with open(path, 'w') as f:
-            json.dump(cur, f, indent=1, sort_keys=True)
-    except OSError:
-        pass
-
-
-@pytest.fixture(scope='module')
-def gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'gf_outputs.npz'))
-
-
-@pytest.fixture(scope='module')
-def pin():
-    return json.load(open(os.path.join(ROOT, 'tests', 'golden', 'PINNING_gf.json')))['cases']
+gold = harness.golden_fixture('gf_outputs.npz')
+pin = harness.pinning_fixture('PINNING_gf.json')
 
 
 def _gate(gold, pin, key, mine, orc):
@@ -67,7 +40,7 @@ def _gate(gold, pin, key, mine, orc):
     e_orc = float(np.abs(mine.astype(np.float64) - orc).max())
     e_ref = float(np.abs(CG.sub(mine).astype(np.float64) - gold[key]).max())
     s, want = CG.summary(mine), gold[key + '/stats']
-    _dump(key, {'vs_oracle': e_orc, 'vs_reference_sample': e_ref, 'floor': p['maxabs_oracle'], 'max_ref': p['max_ref'],
+    harness.parity_dump('gf', key, {'vs_oracle': e_orc, 'vs_reference_sample': e_ref, 'floor': p['maxabs_oracle'], 'max_ref': p['max_ref'],
                 'gate': allow, 'rel_vs_oracle': e_orc / p['max_ref']})
     assert list(mine.shape) == p['shape']
     assert e_orc <= allow, (key, e_orc, allow)
@@ -82,7 +55,7 @@ def _gate(gold, pin, key, mine, orc):
 def _exact(gold, key, mine, orc):
     assert np.array_equal(mine, orc), (key, int((mine != orc).sum()), float(np.abs(mine.astype(np.float64) - orc).max()))
     assert np.array_equal(CG.sub(mine), gold[key])
-    _dump(key, {'mismatch_oracle': 0})
+    harness.parity_dump('gf', key, {'mismatch_oracle': 0})
 
 
 @pytest.mark.parametrize('name', CG.CASES)
@@ -136,16 +109,6 @@ def test_only_one_input_requires_grad():
 
 
 # ---- the no-grad path, determinism, errors -------------------------------------------------------------------------
-def _launches(fn):
-    from neuralrgbd_b200 import _lib
-    L = _lib.lib()
-    torch.cuda.synchronize()
-    L.nrgbd_reset_launch_count()
-    out = fn()
-    torch.cuda.synchronize()
-    return L.nrgbd_launch_count(), out
-
-
 @pytest.mark.parametrize('op', ['GuidedFilter', 'BoxFilter'])
 def test_no_grad_path_unchanged(op):
     from neuralrgbd_b200.models.GF.box_filter import BoxFilter
@@ -157,10 +120,10 @@ def test_no_grad_path_unchanged(op):
     else:
         m, want = BoxFilter(1), 2
         fn = lambda rg: m(T(c['y']).requires_grad_(rg))                                     # noqa: E731
-    n0, plain = _launches(lambda: fn(False))
+    n0, plain = harness.launch_count(lambda: fn(False))
     with torch.no_grad():
-        n1, nog = _launches(lambda: fn(True))
-    n2, withgrad = _launches(lambda: fn(True))
+        n1, nog = harness.launch_count(lambda: fn(True))
+    n2, withgrad = harness.launch_count(lambda: fn(True))
     assert n0 == n1 == n2 == want, (n0, n1, n2, want)
     assert plain.grad_fn is None and nog.grad_fn is None and withgrad.requires_grad
     assert torch.equal(plain, nog) and torch.equal(plain, withgrad.detach())
@@ -175,7 +138,7 @@ def test_backward_launches_and_run_to_run():
     for _ in range(2):
         x, y = T(c['x']).requires_grad_(True), T(c['y']).requires_grad_(True)
         out = gf(x, y)
-        n, _ = _launches(lambda: out.backward(T(c['g'])))
+        n, _ = harness.launch_count(lambda: out.backward(T(c['g'])))
         assert n == 10
         res.append((out.detach(), x.grad, y.grad))
     for a, b in zip(*res):
@@ -210,14 +173,8 @@ def test_reference_kvnet_dgf_training_step():
     """train_utils/train_KVNet.py's L1 loss with its variance terms on the reference's own KVNET(refineNet_name='DGF'),
     a first window and one steady step, with the f-5 mirrors, depth_var and GuidedFilter patched in: every parameter
     gets a gradient within test_gpu_grad.py's gate of the unpatched reference."""
-    from oracle import fetch_reference
-    ref_code = fetch_reference.code_dir()
-    assert ref_code, 'no copy of the reference: oracle/_ref is made by __graft_entry__.build() (oracle/fetch_reference.py)'
-    r = subprocess.run([sys.executable, os.path.join(ROOT, 'tests', 'gf_kvnet_driver.py'), ref_code],
-                       capture_output=True, text=True, timeout=1200, cwd=ROOT)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-    res = json.loads(r.stdout.strip().splitlines()[-1])
-    _dump('kvnet_dgf_l1_var', res)
+    res = harness.run_reference_driver('grad', 'gf', timeout=1200)
+    harness.parity_dump('gf', 'kvnet_dgf_l1_var', res)
     assert res['restored'] is True
     assert res['dgf_is_mirror'] is True and res['same_state_dict_keys'] is True
     assert res['dgf_calls'] > 0

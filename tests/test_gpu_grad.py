@@ -5,21 +5,15 @@
  * The no-grad path: the same launches and bit-identical outputs whether or not the inputs require grad, under
    torch.no_grad() or not; the autograd path's forward value is the no-grad one, bit for bit.
  * The reference's own models.KVNET.KVNET (refineNet_name='DGF') trained for one step with the mirrors patched into
-   warping.homography / mutils.misc against the unpatched reference (tests/grad_kvnet_driver.py).
+   warping.homography / mutils.misc against the unpatched reference (tests/reference_driver.py grad geometry).
 Measured deviations are written to $NRGBD_PARITY_DIR/parity_grad.json when that variable is set.
 """
-import json
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
 
 from oracle import planesweep_oracle as O
-from tests import cases, cases_grad as CG, oracle_grad as OG
-from tests.conftest import ROOT
+from tests import cases, cases_grad as CG, oracle_grad as OG, harness
 
 pytestmark = pytest.mark.gpu
 T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()     # noqa: E731
@@ -33,29 +27,8 @@ T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()     # noqa: E731
 REL = {'warp': 2e-5, 'resample': 2e-6, 'regression': 1e-6}
 
 
-def _dump(key, row):
-    d = os.environ.get('NRGBD_PARITY_DIR')
-    if not d:
-        return
-    try:
-        os.makedirs(d, exist_ok=True)
-        path = os.path.join(d, 'parity_grad.json')
-        cur = json.load(open(path)) if os.path.exists(path) else {}
-        cur[key] = row
-        with open(path, 'w') as f:
-            json.dump(cur, f, indent=1, sort_keys=True)
-    except OSError:
-        pass
-
-
-@pytest.fixture(scope='module')
-def gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'grad_outputs.npz'))
-
-
-@pytest.fixture(scope='module')
-def pin():
-    return json.load(open(os.path.join(ROOT, 'tests', 'golden', 'PINNING_grad.json')))['cases']
+gold = harness.golden_fixture('grad_outputs.npz')
+pin = harness.pinning_fixture('PINNING_grad.json')
 
 
 def _cam(w, h):
@@ -76,7 +49,7 @@ def _gate(gold, pin, key, mine, orc):
     e_orc = float(np.abs(mine.astype(np.float64) - orc).max())
     e_ref = float(np.abs(CG.sub(mine).astype(np.float64) - gold[key + '/g']).max())
     s, want = CG.summary(mine), gold[key + '/stats']
-    _dump(key, {'vs_oracle': e_orc, 'vs_reference_sample': e_ref, 'floor': p['maxabs_oracle'], 'max_ref': p['max_ref'],
+    harness.parity_dump('grad', key, {'vs_oracle': e_orc, 'vs_reference_sample': e_ref, 'floor': p['maxabs_oracle'], 'max_ref': p['max_ref'],
                 'gate': allow})
     assert list(mine.shape) == p['shape']
     assert e_orc <= allow, (key, e_orc, allow)
@@ -205,16 +178,6 @@ def test_regression_conf_has_no_gradient():
 
 
 # ---- the no-grad path -----------------------------------------------------------------------------------------------
-def _launches(fn):
-    from neuralrgbd_b200 import _lib
-    L = _lib.lib()
-    torch.cuda.synchronize()
-    L.nrgbd_reset_launch_count()
-    out = fn()
-    torch.cuda.synchronize()
-    return L.nrgbd_launch_count(), out
-
-
 def _calls():
     from neuralrgbd_b200.warping import homography as H
     from neuralrgbd_b200.mutils import misc as M
@@ -237,10 +200,10 @@ def _calls():
 @pytest.mark.parametrize('op', ['warp', 'resample', 'regression'])
 def test_no_grad_path_unchanged(op):
     name, fn, want = [x for x in _calls() if x[0] == op][0]
-    n0, plain = _launches(lambda: fn(False))
+    n0, plain = harness.launch_count(lambda: fn(False))
     with torch.no_grad():
-        n1, nog = _launches(lambda: fn(True))
-    n2, withgrad = _launches(lambda: fn(True))
+        n1, nog = harness.launch_count(lambda: fn(True))
+    n2, withgrad = harness.launch_count(lambda: fn(True))
     flat = lambda o: [x.detach() for x in (o if isinstance(o, (list, tuple)) else [o])]   # noqa: E731
     assert n0 == n1 == n2 == want, (n0, n1, n2, want)
     for a, b, c in zip(flat(plain), flat(nog), flat(withgrad)):
@@ -254,14 +217,8 @@ def test_reference_kvnet_dgf_gradients_with_mirrors():
     """One training step of the reference's KVNET(refineNet_name='DGF'): the D-Net / K-Net parameters get their loss
     gradient only through depth_val_regression (models/KVNET.py:129,176) and the propagated prior (resample_vol_cuda).
     With the mirrors patched in, every parameter gets a gradient, and it matches the unpatched reference."""
-    from oracle import fetch_reference
-    ref_code = fetch_reference.code_dir()
-    assert ref_code, 'no copy of the reference: oracle/_ref is made by __graft_entry__.build() (oracle/fetch_reference.py)'
-    r = subprocess.run([sys.executable, os.path.join(ROOT, 'tests', 'grad_kvnet_driver.py'), ref_code],
-                       capture_output=True, text=True, timeout=1200, cwd=ROOT)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-    res = json.loads(r.stdout.strip().splitlines()[-1])
-    _dump('kvnet_dgf', res)
+    res = harness.run_reference_driver('grad', 'geometry', timeout=1200)
+    harness.parity_dump('grad', 'kvnet_dgf', res)
     assert not res['missing'], res['missing']
     assert res['restored'] is True                  # the reference's own functions are back after the patched run
     params = res['params']

@@ -2,31 +2,20 @@
 mirrors against (i) the outputs of the unmodified reference and of torch autograd through it (tests/golden/lba_outputs.npz,
 tests/golden/make_golden_lba.py) and (ii) the numpy oracle; plus the optimiser-facing behaviour: autograd through the mirror
 gives the pose gradients ICP/opt_pose_numerical.py:99-160 steps on, and a few Adam steps reduce a photometric loss."""
-import os
-
 import numpy as np
 import pytest
 import torch
 
 from oracle import planesweep_oracle as O
-from tests import cases
-from tests.conftest import ROOT, maxabs
+from tests import cases, harness
+from tests.conftest import maxabs
 
 pytestmark = pytest.mark.gpu
 dev = 'cuda:0'
 T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)     # noqa: E731
 
 
-def cam_torch(cam):
-    c = dict(cam)
-    c['unit_ray_array_2D'] = torch.from_numpy(cam['unit_ray_array_2D'])
-    c['intrinsic_M_cuda'] = torch.from_numpy(cam['intrinsic_M_cuda'])
-    return c
-
-
-@pytest.fixture(scope='module')
-def gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'lba_outputs.npz'))
+gold = harness.golden_fixture('lba_outputs.npz')
 
 
 @pytest.mark.parametrize('name', cases.LBA_CASES)
@@ -34,7 +23,7 @@ def test_back_warp_forward_vs_reference_and_oracle(gold, name):
     import neuralrgbd_b200.warping.homography as H
     c = cases.lba_case(name)
     cam_np = cases.cam_for(O.make_cam_intrinsics, c['w'], c['h'])
-    cam = cam_torch(cam_np)
+    cam = harness.cam_tensors(cam_np)
     out = H.back_warp_th_Rt_msrc(T(c['imgs']), T(c['dmap']), T(c['Rs']), T(c['ts']), cam).cpu().numpy()
     assert out.shape == gold[name + '/warp_msrc'].shape
     assert maxabs(out, gold[name + '/warp_msrc']) <= 2e-5                      # the live reference
@@ -47,7 +36,7 @@ def test_back_warp_forward_vs_reference_and_oracle(gold, name):
 def test_back_warp_gradients_vs_reference_autograd(gold, name):
     import neuralrgbd_b200.warping.homography as H
     c = cases.lba_case(name)
-    cam = cam_torch(cases.cam_for(O.make_cam_intrinsics, c['w'], c['h']))
+    cam = harness.cam_tensors(cases.cam_for(O.make_cam_intrinsics, c['w'], c['h']))
     img = T(c['imgs'][:1]).requires_grad_(True)
     R = T(c['Rs'][0]).requires_grad_(True)
     t = T(c['ts'][0]).requires_grad_(True)
@@ -65,7 +54,7 @@ def test_pose_refinement_step_reduces_the_photometric_loss():
     import neuralrgbd_b200.warping.homography as H
     c = cases.lba_case('lba_v3_c3_48x64')
     cam_np = cases.cam_for(O.make_cam_intrinsics, c['w'], c['h'])
-    cam = cam_torch(cam_np)
+    cam = harness.cam_tensors(cam_np)
     rng = np.random.RandomState(3)
     from neuralrgbd_b200 import synth
     src = synth.smooth_image(rng, 3, c['h'], c['w'])[None]

@@ -15,30 +15,15 @@ import numpy as np
 import pytest
 import torch
 
-from tests import cases
+from tests import cases, harness
 from tests import cases_lba_opt as LC
 from tests.conftest import ROOT
 
 pytestmark = pytest.mark.gpu
 dev = 'cuda:0'
-GOLD = os.path.join(ROOT, 'tests', 'golden')
 
-
-@pytest.fixture(scope='module')
-def gold():
-    return np.load(os.path.join(GOLD, 'lba_opt_outputs.npz'))
-
-
-@pytest.fixture(scope='module')
-def pin():
-    return json.load(open(os.path.join(GOLD, 'PINNING_lba_opt.json')))['cases']
-
-
-def cam_torch(cam):
-    c = dict(cam)
-    c['unit_ray_array_2D'] = torch.from_numpy(cam['unit_ray_array_2D'])
-    c['intrinsic_M_cuda'] = torch.from_numpy(cam['intrinsic_M_cuda'])
-    return c
+gold = harness.golden_fixture('lba_opt_outputs.npz')
+pin = harness.pinning_fixture('PINNING_lba_opt.json')
 
 
 def run(c, on_gpu=True, fn=None):
@@ -47,7 +32,7 @@ def run(c, on_gpu=True, fn=None):
     fn = fn or (M.local_BA_direct_parallel if c['entry'] == 'parallel' else M.local_BA_direct)
     buf = io.StringIO()
     with contextlib.redirect_stdout(buf):
-        poses = fn(T(c['ref']), [T(s) for s in c['srcs']], T(c['dmap']), T(c['conf']), [cam_torch(k) for k in c['cams']], c['dw_scales'],
+        poses = fn(T(c['ref']), [T(s) for s in c['srcs']], T(c['dmap']), T(c['conf']), [harness.cam_tensors(k) for k in c['cams']], c['dw_scales'],
                    list(c['poses_init']), c['max_iter'], c['step'], c['opt_vars'])
     return np.stack([p.numpy() for p in poses]), buf.getvalue().splitlines()
 
@@ -195,5 +180,5 @@ def test_dropin_routes_the_reference_optimiser():
     assert r.returncode == 0, r.stderr[-3000:]
     out = json.loads(r.stdout.strip().splitlines()[-1])
     assert out['module'] == 'neuralrgbd_b200.ICP.opt_pose_numerical'
-    p = json.load(open(os.path.join(GOLD, 'PINNING_lba_opt.json')))['cases'][name]
+    p = harness.pinning('PINNING_lba_opt.json')[name]
     assert out['diff'] <= max(1e-4, 4 * p['final_pose_maxabs']), out

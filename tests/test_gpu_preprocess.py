@@ -1,21 +1,16 @@
 """f-4 on the device: resize + normalise kernel bit-exact against the oracle / the reference transform, and the
 resident sliding window."""
-import os
-
 import numpy as np
 import pytest
 import torch
 
 from oracle import preprocess_oracle as P
-from tests import cases
-from tests.conftest import ROOT
+from tests import cases, harness
 
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(scope='module')
-def gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'preprocess_outputs.npz'))
+gold = harness.golden_fixture('preprocess_outputs.npz')
 
 
 @pytest.mark.parametrize('name', cases.PREPROCESS_CASES)

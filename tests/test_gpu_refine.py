@@ -10,12 +10,7 @@
  * Eval mode with each configuration, the reference's unmodified test(), and no R-Net kernel for if_refined=False.
 Measured deviations are written to $NRGBD_PARITY_DIR/parity_refine.json when that variable is set.
 """
-import contextlib
-import io
 import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -23,13 +18,12 @@ import torch
 
 from neuralrgbd_b200 import arch
 from oracle import planesweep_oracle as O
-from tests import cases
+from tests import cases, harness
 from tests import oracle_refine as R
-from tests.conftest import ROOT, maxabs
+from tests.conftest import maxabs
+from tests.harness import DEV as dev, T
 
 pytestmark = pytest.mark.gpu
-dev = 'cuda:0'
-T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)     # noqa: E731
 SUB_LIMIT = 8000
 TOL_FIRST = 1e-4
 TOL_KNET_F16 = 1.5e-4
@@ -39,29 +33,6 @@ TOL_DEPTH_MM = 1.0
 TOL_SELF_M = 1e-5          # engine DGF vs the oracle's filter on the engine's own low-resolution DPV
 MODES = ['f16x3', 'tf32x3', 'fp32']
 STEPS = {'kvnet_256_d16': 3, 'c23_640x480_d64_v4_stream30': 2}
-
-
-def _dump(key, row):
-    d = os.environ.get('NRGBD_PARITY_DIR')
-    if not d:
-        return
-    try:
-        os.makedirs(d, exist_ok=True)
-        path = os.path.join(d, 'parity_refine.json')
-        cur = json.load(open(path)) if os.path.exists(path) else {}
-        cur[key] = row
-        with open(path, 'w') as f:
-            json.dump(cur, f, indent=1, sort_keys=True)
-    except OSError:
-        pass
-
-
-def _gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'refine_outputs.npz'))
-
-
-def _pin():
-    return json.load(open(os.path.join(ROOT, 'tests', 'golden', 'PINNING_refine.json')))['cases']
 
 
 # ---- op level ----------------------------------------------------------------------------------------------------------
@@ -76,11 +47,11 @@ def test_guided_filter_kernel_vs_oracle(name):
     y = run()
     got = y.cpu().numpy()
     want = R.dgf_refine(g['dmap'], g['img'], g['sd'])
-    ref = _gold()['refine/gf/%s/out' % name]
+    ref = harness.golden('refine_outputs.npz')['refine/gf/%s/out' % name]
     row = {'oracle_m': maxabs(got, want), 'reference_m': maxabs(got, ref), 'bitexact_oracle': bool(np.array_equal(got, want))}
-    _dump('gf/%s' % name, row)
+    harness.parity_dump('refine', 'gf/%s' % name, row)
     assert np.array_equal(got, want), row
-    assert row['reference_m'] <= _pin()['gf/%s' % name]['oracle_m'], row
+    assert row['reference_m'] <= harness.pinning('PINNING_refine.json')['gf/%s' % name]['oracle_m'], row
     assert torch.equal(run(), y), 'not bit-identical from run to run'
 
 
@@ -97,10 +68,6 @@ def _case(name):
     return c, cam, wseed
 
 
-def _cam_t(cam):
-    return dict(cam, unit_ray_array_2D=torch.from_numpy(cam['unit_ray_array_2D']), intrinsic_M_cuda=torch.from_numpy(cam['intrinsic_M_cuda']))
-
-
 KW = {'DGF': dict(if_refined=True, refineNet_name='DGF'), 'none': dict(if_refined=False),
       'DPV_up': dict(if_refined=True, refineNet_name='DPV', if_upsample_d=True)}
 
@@ -112,30 +79,6 @@ def _sd(c, wseed, cfg):
                                    upsample_d=cfg == 'DPV_up')
         sd.update({k: v for k, v in rn.items() if k.startswith('r_net.')})
     return sd
-
-
-def _model(c, cam_t, sd, cfg, conv_math):
-    from neuralrgbd_b200.models.KVNET import KVNET
-    with contextlib.redirect_stdout(io.StringIO()):
-        m = KVNET(feature_dim=64, cam_intrinsics=cam_t, d_candi=c['d'], sigma_soft_max=c['sigma'], KVNet_feature_dim=64,
-                  d_upsample_ratio_KV_net=None, t_win_r=c['t_win_r'], **KW[cfg])
-    m.load_state_dict({k: torch.from_numpy(v) for k, v in sd.items()}, strict=True)
-    m = m.to(dev)
-    m.conv_math = conv_math
-    return m
-
-
-def _prior(name, step):
-    if name in cases.KVNET_CASES:
-        return np.load(os.path.join(ROOT, 'tests', 'golden', 'reference_outputs.npz'))['kvnet/%s/step%d/BV_predict_next_full' % (name, step - 1)]
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'configs_priors_%s.npz' % name))['cfg/%s/step0/BV_predict_next_full' % name]
-
-
-def _forward(m, c, cam_t, step, prior):
-    ref_f, src_f, poses = cases.window(c, c['t_win_r'] + step)
-    with torch.no_grad():
-        out = m(T(ref_f), T(src_f), T(poses), torch.zeros(1), cam_intrinsics=[cam_t], BV_predict=None if prior is None else T(prior))
-    return ref_f, out
 
 
 def _self_check(out_refined, lowres, ref_f, d, sd):
@@ -150,15 +93,15 @@ def _self_check(out_refined, lowres, ref_f, d, sd):
 @pytest.mark.parametrize('name', ['kvnet_256_d16', 'c23_640x480_d64_v4_stream30'])
 @pytest.mark.parametrize('cfg', ['DGF', 'none'])
 def test_engine_refine_vs_reference(cfg, name, conv_math):
-    gold, pin = _gold(), _pin()
+    gold, pin = harness.golden('refine_outputs.npz'), harness.pinning('PINNING_refine.json')
     c, cam, wseed = _case(name)
-    cam_t = _cam_t(cam)
+    cam_t = harness.cam_tensors(cam)
     sd = _sd(c, wseed, cfg)
-    m = _model(c, cam_t, sd, cfg, conv_math)
+    m = harness.engine_kvnet(c, cam_t, sd, conv_math, **KW[cfg])
     rows = {}
     for k in range(STEPS[name]):
-        prior = _prior(name, k) if k else None
-        ref_f, out = _forward(m, c, cam_t, k, prior)
+        prior = harness.reference_prior(name, k) if k else None
+        ref_f, out = harness.engine_forward(m, c, cam_t, k, prior)
         key = 'refine/%s/%s/step%d' % (cfg, name, k)
         lowres = out[2] if k == 0 else out[3]
         a = lowres.cpu().numpy()
@@ -184,7 +127,7 @@ def test_engine_refine_vs_reference(cfg, name, conv_math):
                 r['dmap_cur_m'] = maxabs(cases.subsample_to(out[0].cpu().numpy()[0, 0], SUB_LIMIT), gold[key + '/dmap_cur'])
                 r['self_cur_m'] = _self_check(out[0], out[2], ref_f, c['d'], sd)
         rows['step%d' % k] = r
-    _dump('%s/%s/%s' % (cfg, name, conv_math), rows)
+    harness.parity_dump('refine', '%s/%s/%s' % (cfg, name, conv_math), rows)
     msg = json.dumps(rows)
     for r in rows.values():
         assert r['prob'] <= r['prob_gate'], msg
@@ -208,15 +151,15 @@ def test_engine_upsample_d_vs_reference(name, conv_math):
     numpy regression of the same array."""
     from neuralrgbd_b200.mutils import misc
     from neuralrgbd_b200.test_utils import export_res
-    gold, pin = _gold(), _pin()
+    gold, pin = harness.golden('refine_outputs.npz'), harness.pinning('PINNING_refine.json')
     c, cam, wseed = _case(name)
-    cam_t = _cam_t(cam)
-    m = _model(c, cam_t, _sd(c, wseed, 'DPV_up'), 'DPV_up', conv_math)
+    cam_t = harness.cam_tensors(cam)
+    m = harness.engine_kvnet(c, cam_t, _sd(c, wseed, 'DPV_up'), conv_math, **KW['DPV_up'])
     dup4 = _dup4(c['d'])
     rows = {}
     for k in range(STEPS[name]):
-        prior = _prior(name, k) if k else None
-        _, out = _forward(m, c, cam_t, k, prior)
+        prior = harness.reference_prior(name, k) if k else None
+        _, out = harness.engine_forward(m, c, cam_t, k, prior)
         key = 'refine/DPV_up/%s/step%d' % (name, k)
         ref = out[0] if k == 0 else out[1]
         assert ref.shape == (1, 4 * c['D'], c['H'], c['W']) and out[2].shape == (1, c['D'], c['H'] // 4, c['W'] // 4)
@@ -235,7 +178,7 @@ def test_engine_upsample_d_vs_reference(name, conv_math):
         num = O.depth_val_regression(a, dup4)[0]
         r['mirrors_vs_numpy_m'] = max(maxabs(dep, num), maxabs(exp_dep, num))
         rows['step%d' % k] = r
-    _dump('DPV_up/%s/%s' % (name, conv_math), rows)
+    harness.parity_dump('refine', 'DPV_up/%s/%s' % (name, conv_math), rows)
     msg = json.dumps(rows)
     for r in rows.values():
         assert r['prob'] <= r['prob_gate'] and r['sumsq_rel'] <= 1e-4, msg
@@ -265,12 +208,12 @@ def test_eval_mode_each_configuration(cfg):
     """.eval() with each configuration: the running-statistics BatchNorm path with the new refinements; nothing moves."""
     name = 'kvnet_256_d16'
     c, cam, wseed = _case(name)
-    cam_t = _cam_t(cam)
+    cam_t = harness.cam_tensors(cam)
     sd = _sd(c, wseed, cfg)
-    m = _model(c, cam_t, sd, cfg, 'f16x3').eval()
+    m = harness.engine_kvnet(c, cam_t, sd, 'f16x3', **KW[cfg]).eval()
     before = {k: v.clone() for k, v in m.state_dict().items()}
     for k in range(2):
-        ref_f, out = _forward(m, c, cam_t, k, _prior(name, k) if k else None)
+        ref_f, out = harness.engine_forward(m, c, cam_t, k, harness.reference_prior(name, k) if k else None)
         lowres = out[2] if k == 0 else out[3]
         assert torch.isfinite(lowres).all()
         if cfg == 'none':
@@ -286,16 +229,10 @@ def test_eval_mode_each_configuration(cfg):
 
 @pytest.mark.parametrize('cfg', ['DGF', 'none', 'DPV_up'])
 def test_reference_test_runs_unmodified(cfg):
-    from oracle import fetch_reference
-    ref_code = fetch_reference.code_dir()
-    assert ref_code, 'no copy of the reference: oracle/_ref is made by __graft_entry__.build() (oracle/fetch_reference.py)'
-    pin = _pin()
+    pin = harness.pinning('PINNING_refine.json')
     for mode in ('train', 'eval'):
-        r = subprocess.run([sys.executable, os.path.join(ROOT, 'tests', 'dropin_refine_driver.py'), ref_code, cfg, mode],
-                           capture_output=True, text=True, timeout=900)
-        assert r.returncode == 0, (r.stdout[-1500:], r.stderr[-3000:])
-        out = json.loads(r.stdout.strip().splitlines()[-1])
-        _dump('dropin/%s/%s' % (cfg, mode), out)
+        out = harness.run_reference_driver('step', 'refine', cfg, mode, timeout=900)
+        harness.parity_dump('refine', 'dropin/%s/%s' % (cfg, mode), out)
         assert out['class'] == 'neuralrgbd_b200.models.KVNET'
         assert all(s['finite'] for s in out['steps'])
         if mode == 'eval':
@@ -322,8 +259,8 @@ def test_no_rnet_launches_when_unrefined():
     L = _lib.lib()
     name = 'kvnet_256_d16'
     c, cam, wseed = _case(name)
-    cam_t = _cam_t(cam)
-    prior = _prior(name, 1)
+    cam_t = harness.cam_tensors(cam)
+    prior = harness.reference_prior(name, 1)
 
     def steady_launches(m, call):
         for _ in range(3):                   # eager warm-up, capture, replay
@@ -332,14 +269,9 @@ def test_no_rnet_launches_when_unrefined():
             torch.cuda.synchronize()
         return L.nrgbd_launch_count()
 
-    fwd = lambda m: _forward(m, c, cam_t, 1, prior)      # noqa: E731
-    n_none = steady_launches(_model(c, cam_t, _sd(c, wseed, 'none'), 'none', 'f16x3'), fwd)
-    from neuralrgbd_b200.models.KVNET import KVNET
-    with contextlib.redirect_stdout(io.StringIO()):
-        m_dpv = KVNET(feature_dim=64, cam_intrinsics=cam_t, d_candi=c['d'], sigma_soft_max=c['sigma'], KVNet_feature_dim=64,
-                      d_upsample_ratio_KV_net=None, t_win_r=2)
-    m_dpv.load_state_dict({k: torch.from_numpy(np.asarray(v)) for k, v in c['sd'].items()})
-    m_dpv = m_dpv.to(dev)
+    fwd = lambda m: harness.engine_forward(m, c, cam_t, 1, prior)      # noqa: E731
+    n_none = steady_launches(harness.engine_kvnet(c, cam_t, _sd(c, wseed, 'none'), 'f16x3', **KW['none']), fwd)
+    m_dpv = harness.engine_kvnet(c, cam_t, c['sd'], 'f16x3')
     n_dpv = steady_launches(m_dpv, fwd)
 
     def null_refined(m):
@@ -353,5 +285,5 @@ def test_no_rnet_launches_when_unrefined():
         _lib.check(L.nrgbd_kvnet_forward(ent['h'], ptr(frames), ptr(T(poses)[0].contiguous()), ptr(T(prior)[0].contiguous()), None,
                                          None, ptr(bv_cur), ptr(dpv), None, None, st))
     n_null = steady_launches(m_dpv, null_refined)
-    _dump('launches', {'none': n_none, 'dpv': n_dpv, 'dpv_null_refined': n_null})
+    harness.parity_dump('refine', 'launches', {'none': n_none, 'dpv': n_dpv, 'dpv_null_refined': n_null})
     assert n_none == n_null < n_dpv, (n_none, n_null, n_dpv)

@@ -7,20 +7,14 @@
  * Plain inputs, inputs that require grad and torch.no_grad() give the same launches and bit-identical values.
  * A tensor on a second device stays there.
  * The reference's own models.KVNET.KVNET(refineNet_name='DGF') trained with train_utils/train_KVNet.py's L1 loss,
-   variance terms included, with the mirrors patched in, against the unpatched reference (tests/stats_kvnet_driver.py).
+   variance terms included, with the mirrors patched in, against the unpatched reference (tests/reference_driver.py grad stats).
 Measured deviations are written to $NRGBD_PARITY_DIR/parity_stats.json when that variable is set.
 """
-import json
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
 
-from tests import cases_stats as CS, oracle_stats as OS
-from tests.conftest import ROOT
+from tests import cases_stats as CS, oracle_stats as OS, harness
 
 pytestmark = pytest.mark.gpu
 T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()     # noqa: E731
@@ -34,29 +28,8 @@ T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()     # noqa: E731
 REL = {'var/out': 2e-6, 'var/g_bv': 2e-6, 'var/g_mean': 1e-5, 'stats/out': 1e-5, 'stats/g_bv': 1e-5}
 
 
-def _dump(key, row):
-    d = os.environ.get('NRGBD_PARITY_DIR')
-    if not d:
-        return
-    try:
-        os.makedirs(d, exist_ok=True)
-        path = os.path.join(d, 'parity_stats.json')
-        cur = json.load(open(path)) if os.path.exists(path) else {}
-        cur[key] = row
-        with open(path, 'w') as f:
-            json.dump(cur, f, indent=1, sort_keys=True)
-    except OSError:
-        pass
-
-
-@pytest.fixture(scope='module')
-def gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'stats_outputs.npz'))
-
-
-@pytest.fixture(scope='module')
-def pin():
-    return json.load(open(os.path.join(ROOT, 'tests', 'golden', 'PINNING_stats.json')))['cases']
+gold = harness.golden_fixture('stats_outputs.npz')
+pin = harness.pinning_fixture('PINNING_stats.json')
 
 
 def _gate(gold, pin, key, mine, orc):
@@ -66,7 +39,7 @@ def _gate(gold, pin, key, mine, orc):
     e_orc = float(np.abs(mine.astype(np.float64) - orc).max())
     e_ref = float(np.abs(CS.sub(mine).astype(np.float64) - gold[key]).max())
     s, want = CS.summary(mine), gold[key + '/stats']
-    _dump(key, {'vs_oracle': e_orc, 'vs_reference_sample': e_ref, 'floor': p['maxabs_oracle'], 'max_ref': p['max_ref'],
+    harness.parity_dump('stats', key, {'vs_oracle': e_orc, 'vs_reference_sample': e_ref, 'floor': p['maxabs_oracle'], 'max_ref': p['max_ref'],
                 'gate': allow})
     assert list(mine.shape) == p['shape']
     assert e_orc <= allow, (key, e_orc, allow)
@@ -131,7 +104,7 @@ def test_extreme_indices(gold, name):
             a = np.take_along_axis(ps, got[:, None], 1)[:, 0]
             b = np.take_along_axis(ps, want[:, None], 1)[:, 0]
             assert np.abs(a - b).max() <= 1e-6 * np.abs(p).max()
-            _dump('index/%s/%s' % (name, kind), {'mismatch_sample': int((got != want).sum())})
+            harness.parity_dump('stats', 'index/%s/%s' % (name, kind), {'mismatch_sample': int((got != want).sum())})
 
 
 def test_extreme_nan_and_ties():
@@ -148,16 +121,6 @@ def test_extreme_nan_and_ties():
 
 
 # ---- the no-grad path -----------------------------------------------------------------------------------------------
-def _launches(fn):
-    from neuralrgbd_b200 import _lib
-    L = _lib.lib()
-    torch.cuda.synchronize()
-    L.nrgbd_reset_launch_count()
-    out = fn()
-    torch.cuda.synchronize()
-    return L.nrgbd_launch_count(), out
-
-
 @pytest.mark.parametrize('op', ['depth_var', 'dpv_statistics'])
 def test_no_grad_path_unchanged(op):
     from neuralrgbd_b200.mutils import misc as M
@@ -167,10 +130,10 @@ def test_no_grad_path_unchanged(op):
         fn, want = (lambda rg: M.depth_var(T(c['bv']).requires_grad_(rg), mean, c['d'])), 1
     else:
         fn, want = (lambda rg: M.dpv_statistics(T(c['bv']).requires_grad_(rg), c['d'], CS.ALL_STATS)), 4
-    n0, plain = _launches(lambda: fn(False))
+    n0, plain = harness.launch_count(lambda: fn(False))
     with torch.no_grad():
-        n1, nog = _launches(lambda: fn(True))
-    n2, withgrad = _launches(lambda: fn(True))
+        n1, nog = harness.launch_count(lambda: fn(True))
+    n2, withgrad = harness.launch_count(lambda: fn(True))
     assert n0 == n1 == n2 == want, (n0, n1, n2, want)
     assert plain.grad_fn is None and nog.grad_fn is None and withgrad.requires_grad
     assert torch.equal(plain, nog) and torch.equal(plain, withgrad.detach())
@@ -208,14 +171,8 @@ def test_reference_kvnet_l1_loss_with_variance():
     KVNET(refineNet_name='DGF') for a first window and one steady step: with the f-5 mirrors and depth_var patched in,
     every parameter gets a gradient and it matches the unpatched reference. The variance terms on their own reach every
     D-Net and K-Net parameter only through depth_var and depth_val_regression: they are checked separately."""
-    from oracle import fetch_reference
-    ref_code = fetch_reference.code_dir()
-    assert ref_code, 'no copy of the reference: oracle/_ref is made by __graft_entry__.build() (oracle/fetch_reference.py)'
-    r = subprocess.run([sys.executable, os.path.join(ROOT, 'tests', 'stats_kvnet_driver.py'), ref_code],
-                       capture_output=True, text=True, timeout=1200, cwd=ROOT)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-    res = json.loads(r.stdout.strip().splitlines()[-1])
-    _dump('kvnet_dgf_l1_var', res)
+    res = harness.run_reference_driver('grad', 'stats', timeout=1200)
+    harness.parity_dump('stats', 'kvnet_dgf_l1_var', res)
     assert res['restored'] is True
     for part in ('full', 'var_only'):
         rr = res[part]

@@ -6,20 +6,15 @@ neuralrgbd_b200.camera.make_cam_intrinsics (product: the dict handed to the engi
 oracle.planesweep_oracle.make_cam_intrinsics (the function every other fixture's inputs are built with) must
 reproduce it BIT FOR BIT - same float64 expressions, same float32 casts.
 """
-import os
-
 import numpy as np
 import pytest
 
 from neuralrgbd_b200 import camera
 from oracle import planesweep_oracle as O
-from tests import cases
-from tests.conftest import ROOT
+from tests import cases, harness
 
 
-@pytest.fixture(scope='module')
-def gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'camera_outputs.npz'))
+gold = harness.golden_fixture('camera_outputs.npz')
 
 
 def _np(x):

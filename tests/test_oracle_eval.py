@@ -1,23 +1,16 @@
 """CPU checks of the eval-mode oracle (tests/oracle_eval.py) against the eval fixtures of the unmodified reference
 (tests/golden/make_golden_eval.py), and of which layers eval mode touches."""
-import json
-import os
-
 import numpy as np
 import pytest
 
 from oracle import kvnet_oracle as N
 from oracle import planesweep_oracle as O
-from tests import cases
+from tests import cases, harness
 from tests import oracle_eval as E
-from tests.conftest import ROOT, maxabs
+from tests.conftest import maxabs
 
 NAME = 'kvnet_256_d16'
 NAMES4 = ['dmap_cur_refined', 'dmap_refined', 'BV_cur', 'DPV']
-
-
-def _gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'eval_outputs.npz'))
 
 
 def _sd(c, gold):
@@ -28,7 +21,7 @@ def _sd(c, gold):
 
 
 def test_fixture_holds_warmed_running_statistics():
-    gold = _gold()
+    gold = harness.golden('eval_outputs.npz')
     rs = [k for k in gold.files if k.startswith('eval/%s/rs/' % NAME) and '/rs/d_net.' not in k]   # d_net.*: the same tensors
     assert len(rs) == 3 * 13
     for k in rs:
@@ -41,12 +34,12 @@ def test_fixture_holds_warmed_running_statistics():
 
 @pytest.mark.parametrize('step', [0, 1])
 def test_eval_oracle_vs_reference_fixture(step):
-    gold = _gold()
-    pin = json.load(open(os.path.join(ROOT, 'tests', 'golden', 'PINNING_eval.json')))['cases']
+    gold = harness.golden('eval_outputs.npz')
+    pin = harness.pinning('PINNING_eval.json')
     c = cases.kvnet_case(NAME)
     cam = cases.cam_for(O.make_cam_intrinsics, c['W'] // 4, c['H'] // 4)
     ref_f, src_f, poses = cases.window(c, 2 + step)
-    ref_gold = np.load(os.path.join(ROOT, 'tests', 'golden', 'reference_outputs.npz'))
+    ref_gold = harness.golden('reference_outputs.npz')
     prior = ref_gold['kvnet/%s/step%d/BV_predict_next_full' % (NAME, step - 1)] if step else None      # as recorded
     o = E.kvnet_forward(_sd(c, gold), ref_f, src_f, poses, cam, c['d'], c['sigma'], BV_predict=prior, training=False)
     key = 'eval/%s/step%d' % (NAME, step)
@@ -61,7 +54,7 @@ def test_eval_oracle_vs_reference_fixture(step):
 def test_untracked_layers_keep_batch_statistics_in_eval_mode():
     """Only layers whose running_mean is in the state_dict change in eval mode: the feature CNN up to layer1 (no tracked
     layer) is bit-identical to train mode, layer2 (tracked downsample) is not; K-Net (all tracked) is not."""
-    gold = _gold()
+    gold = harness.golden('eval_outputs.npz')
     c = cases.kvnet_case(NAME)
     P = N.Params(_sd(c, gold))
     pre = 'feature_extractor.feature_extraction'

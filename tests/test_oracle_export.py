@@ -8,13 +8,10 @@ import pytest
 
 from neuralrgbd_b200 import _lib
 from oracle import export_oracle as E
-from tests import cases
-from tests.conftest import ROOT
+from tests import cases, harness
 
 
-@pytest.fixture(scope='module')
-def gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'export_outputs.npz'))
+gold = harness.golden_fixture('export_outputs.npz')
 
 
 def parse_pgm16(b):

@@ -7,31 +7,20 @@
  * The pinned deviations are consistent: the TF32- and f16-emulated references both differ from fp32 by more than the
    f16 oracle does from its reference on first-window probabilities.
 """
-import json
-import os
-
 import numpy as np
 import pytest
 
 from neuralrgbd_b200 import arch
 from oracle import planesweep_oracle as O
-from tests import cases
+from tests import cases, harness
 from tests import cases_f16 as CF
 from tests import oracle_f16 as OF
-from tests.conftest import ROOT, maxabs
-
-
-def _gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'f16_outputs.npz'))
-
-
-def _pin():
-    return json.load(open(os.path.join(ROOT, 'tests', 'golden', 'PINNING_f16.json')))['cases']
+from tests.conftest import maxabs
 
 
 def test_hooked_layers_are_the_engine_tensor_core_layers():
     specs = arch.kvnet_param_specs(64, 16, 2, 64, 'DPV', False)
-    hooked = sorted(_gold()['f16/hooked_layers'].tolist())
+    hooked = sorted(harness.golden('f16_outputs.npz')['f16/hooked_layers'].tolist())
     tc = CF.tc_layers(specs)
     assert hooked == tc
     convs = [n for n, s, _ in specs if len(s) >= 4 and n.endswith('.weight') and not n.startswith('d_net.')]
@@ -46,7 +35,7 @@ def test_round_tf32():
 
 @pytest.mark.parametrize('name', ['stream_256_d16', 'eval_256_d16', 'r1_256_d16'])
 def test_oracle_f16_first_window_matches_fixture(name):
-    gold, pin = _gold(), _pin()
+    gold, pin = harness.golden('f16_outputs.npz'), harness.pinning('PINNING_f16.json')
     c = CF.f16_case(name)
     cam = CF.cam(O.make_cam_intrinsics, c)
     ref_f, src_f, poses = cases.window(c, c['t_win_r'])
@@ -59,7 +48,7 @@ def test_oracle_f16_first_window_matches_fixture(name):
 
 
 def test_pinned_deviations_are_consistent():
-    pin = _pin()
+    pin = harness.pinning('PINNING_f16.json')
     for name in CF.F16_CASES:
         p = pin['f16/%s/step0' % name]
         for nm in ('BV_cur', 'dmap_cur_refined'):

@@ -6,7 +6,6 @@ the host side of their mirrors in neuralrgbd_b200.models.GF:
  * the mirrors' constructor, attributes, asserts and CPU-tensor error, and the install / uninstall round trip of the
    new install_as_reference_modules() entries on the reference's own modules."""
 import json
-import os
 import subprocess
 import sys
 
@@ -14,18 +13,12 @@ import numpy as np
 import pytest
 import torch
 
-from tests import cases_gf as CG, oracle_gf as OG
+from tests import cases_gf as CG, oracle_gf as OG, harness
 from tests.conftest import ROOT
 
 
-@pytest.fixture(scope='module')
-def gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'gf_outputs.npz'))
-
-
-@pytest.fixture(scope='module')
-def pin():
-    return json.load(open(os.path.join(ROOT, 'tests', 'golden', 'PINNING_gf.json')))['cases']
+gold = harness.golden_fixture('gf_outputs.npz')
+pin = harness.pinning_fixture('PINNING_gf.json')
 
 
 def _check(gold, pin, key, mine):

@@ -5,17 +5,15 @@ tests/golden/reference_outputs.npz was produced by the UNMODIFIED reference
 measured deviation is <=5e-5, tests/golden/PINNING.json), resample bit-exact,
 pipeline outputs on PROBABILITIES (see DESIGN.md 'tolerance domain').
 """
-import json
 import math
-import os
 
 import numpy as np
 import pytest
 
 from oracle import planesweep_oracle as O
 from oracle import kvnet_oracle as N
-from tests import cases
-from tests.conftest import maxabs, ROOT
+from tests import cases, harness
+from tests.conftest import maxabs
 
 
 @pytest.mark.parametrize('name', cases.SWEEP_CASES)
@@ -102,7 +100,7 @@ def test_kvnet_first_window_matches_reference(golden):
 def test_pinning_record_within_bounds():
     """The deviations measured when the fixtures were generated stay inside the
     documented envelope (DESIGN.md)."""
-    pin = json.load(open(os.path.join(ROOT, 'tests', 'golden', 'PINNING.json')))['cases']
+    pin = harness.pinning('PINNING.json')
     for k, v in pin.items():
         if k.startswith('sweep/'):
             assert v['logdpv_maxabs'] <= 1e-4 and v['prob_maxabs'] <= 1e-5

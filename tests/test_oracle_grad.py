@@ -4,26 +4,16 @@
    same taps, and the taps against the pinned fp32 forward of oracle/planesweep_oracle.py;
  * the properties the kernels rely on: the six faces of a resampled volume get zero gradient, the clamp mask is the one
    of torch.clamp's backward, and the regression's extra slices get zero."""
-import json
-import os
-
 import numpy as np
 import pytest
 import torch
 
 from oracle import planesweep_oracle as O
-from tests import cases, cases_grad as CG, oracle_grad as OG
-from tests.conftest import ROOT
+from tests import cases, cases_grad as CG, oracle_grad as OG, harness
 
 
-@pytest.fixture(scope='module')
-def gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'grad_outputs.npz'))
-
-
-@pytest.fixture(scope='module')
-def pin():
-    return json.load(open(os.path.join(ROOT, 'tests', 'golden', 'PINNING_grad.json')))['cases']
+gold = harness.golden_fixture('grad_outputs.npz')
+pin = harness.pinning_fixture('PINNING_grad.json')
 
 
 def _cam(w, h):

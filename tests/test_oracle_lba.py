@@ -1,19 +1,14 @@
 """f-3, oracle first: the numpy restatement of the LBA depth-map back-warp and of its pose / image gradients against the
 unmodified reference (forward) and torch autograd through it (backward): tests/golden/lba_outputs.npz. The device
 kernels for this row are not built yet (DESIGN.md 7); this pins the checker they will be tested against."""
-import os
-
 import numpy as np
 import pytest
 
 from oracle import planesweep_oracle as O
-from tests import cases
-from tests.conftest import ROOT
+from tests import cases, harness
 
 
-@pytest.fixture(scope='module')
-def gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'lba_outputs.npz'))
+gold = harness.golden_fixture('lba_outputs.npz')
 
 
 @pytest.mark.parametrize('name', cases.LBA_CASES)

@@ -11,20 +11,12 @@ import pytest
 import torch
 
 from oracle import lba_opt_oracle as LO
-from tests import cases_lba_opt as LC
+from tests import cases_lba_opt as LC, harness
 from tests.conftest import ROOT
 
-GOLD = os.path.join(ROOT, 'tests', 'golden')
 
-
-@pytest.fixture(scope='module')
-def gold():
-    return np.load(os.path.join(GOLD, 'lba_opt_outputs.npz'))
-
-
-@pytest.fixture(scope='module')
-def pin():
-    return json.load(open(os.path.join(GOLD, 'PINNING_lba_opt.json')))['cases']
+gold = harness.golden_fixture('lba_opt_outputs.npz')
+pin = harness.pinning_fixture('PINNING_lba_opt.json')
 
 
 @pytest.mark.parametrize('name', LC.LBA_OPT_CASES)

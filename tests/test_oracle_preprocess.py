@@ -1,17 +1,12 @@
 """f-4: the input-stage oracle (PIL NEAREST + ToTensor + Normalize restated) is bit-identical to the reference transform."""
-import os
-
 import numpy as np
 import pytest
 
 from oracle import preprocess_oracle as P
-from tests import cases
-from tests.conftest import ROOT
+from tests import cases, harness
 
 
-@pytest.fixture(scope='module')
-def gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'preprocess_outputs.npz'))
+gold = harness.golden_fixture('preprocess_outputs.npz')
 
 
 @pytest.mark.parametrize('name', cases.PREPROCESS_CASES)

@@ -5,29 +5,19 @@ and the depth-upsampled DPV R-Net (if_upsample_d=True) against the reference's o
 import contextlib
 import io
 import json
-import os
 
 import numpy as np
 import pytest
 import torch
 
 from neuralrgbd_b200 import arch
-from tests import oracle_refine as R
-from tests.conftest import ROOT
+from tests import oracle_refine as R, harness
 
 CONFIGS = {'DPV': dict(if_refined=True, refineNet_name='DPV'), 'DGF': dict(if_refined=True, refineNet_name='DGF'),
            'none': dict(if_refined=False), 'none_DGF': dict(if_refined=False, refineNet_name='DGF'),
            'DPV_upsample_d': dict(if_refined=True, refineNet_name='DPV', if_upsample_d=True)}
 REFINE = {'DPV': 'DPV', 'DGF': 'DGF', 'none': None, 'none_DGF': None, 'DPV_upsample_d': 'DPV'}
 UPSAMPLE = {'DPV_upsample_d': True}
-
-
-def _gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'refine_outputs.npz'))
-
-
-def _pin():
-    return json.load(open(os.path.join(ROOT, 'tests', 'golden', 'PINNING_refine.json')))['cases']
 
 
 def _model(D=16, **cfg):
@@ -46,8 +36,8 @@ def _model(D=16, **cfg):
 def test_guided_filter_oracle_vs_reference(name):
     """RefineNet_DGF alone on seeded inputs; bit-exact wherever the fixture recorded it so."""
     g = R.gf_case(name)
-    ref = _gold()['refine/gf/%s/out' % name]
-    pin = _pin()['gf/%s' % name]
+    ref = harness.golden('refine_outputs.npz')['refine/gf/%s/out' % name]
+    pin = harness.pinning('PINNING_refine.json')['gf/%s' % name]
     o = R.dgf_refine(g['dmap'], g['img'], g['sd'])
     if pin['oracle_bitexact']:
         assert np.array_equal(o, ref)
@@ -65,7 +55,7 @@ def test_box_filter_counts_are_the_analytic_window_sizes():
 
 @pytest.mark.parametrize('cfg', list(CONFIGS))
 def test_state_dict_matches_reference(cfg):
-    gold = _gold()
+    gold = harness.golden('refine_outputs.npz')
     m, printed = _model(**CONFIGS[cfg])
     sd = m.state_dict()
     assert list(sd.keys()) == list(gold['refine/sd/%s/keys' % cfg])
@@ -95,6 +85,6 @@ def test_upsample_ratio_raises_and_upsample_d_only_widens_dpv():
         _model(d_upsample_ratio_KV_net=2)
     # if_upsample_d is ignored unless the configuration is DPV, as in the reference
     m, _ = _model(if_refined=True, refineNet_name='DGF', if_upsample_d=True)
-    assert list(m.state_dict().keys()) == list(_gold()['refine/sd/DGF/keys'])
+    assert list(m.state_dict().keys()) == list(harness.golden('refine_outputs.npz')['refine/sd/DGF/keys'])
     m, _ = _model(if_refined=False, if_upsample_d=True)
-    assert list(m.state_dict().keys()) == list(_gold()['refine/sd/none/keys'])
+    assert list(m.state_dict().keys()) == list(harness.golden('refine_outputs.npz')['refine/sd/none/keys'])

@@ -5,25 +5,15 @@ host-side logic of their mirrors in neuralrgbd_b200.mutils.misc:
  * torch.autograd.gradcheck (float64 central differences) of each oracle backward against its float64 forward;
  * the reference's behaviour the mirror keeps: names selected by identity, 'variance' before 'E_mean', 'min' without
    BV_log, the channel concat over N, the asserts."""
-import json
-import os
-
 import numpy as np
 import pytest
 import torch
 
-from tests import cases_stats as CS, oracle_stats as OS
-from tests.conftest import ROOT
+from tests import cases_stats as CS, oracle_stats as OS, harness
 
 
-@pytest.fixture(scope='module')
-def gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'stats_outputs.npz'))
-
-
-@pytest.fixture(scope='module')
-def pin():
-    return json.load(open(os.path.join(ROOT, 'tests', 'golden', 'PINNING_stats.json')))['cases']
+gold = harness.golden_fixture('stats_outputs.npz')
+pin = harness.pinning_fixture('PINNING_stats.json')
 
 
 def _check(gold, pin, key, mine):

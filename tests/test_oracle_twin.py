@@ -3,29 +3,24 @@
 import contextlib
 import io
 import json
-import os
 
 import numpy as np
 import pytest
 import torch
 
 from oracle import planesweep_oracle as O
-from tests import cases
+from tests import cases, harness
 from tests import cases_twin as CT
 from tests import oracle_eval as E
-from tests.conftest import ROOT, maxabs
+from tests.conftest import maxabs
 
 NAMES4 = ['dmap_cur_refined', 'dmap_refined', 'BV_cur', 'DPV']
-
-
-def _gold():
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'twin_outputs.npz'))
 
 
 @pytest.mark.parametrize('r,cin', [(1, 10), (2, 16), (3, 22), (4, 28)])
 def test_state_dict_matches_reference(r, cin):
     from neuralrgbd_b200.models.KVNET import KVNET
-    gold = _gold()
+    gold = harness.golden('twin_outputs.npz')
     c = CT.twin_case('r1_256_d16')
     cam = CT.twin_cam(O.make_cam_intrinsics, c)
     with contextlib.redirect_stdout(io.StringIO()):
@@ -42,8 +37,8 @@ def test_state_dict_matches_reference(r, cin):
 @pytest.mark.parametrize('step', [0, 1])
 @pytest.mark.parametrize('name', ['r1_256_d16', 'r3_256_d16'])
 def test_oracle_vs_reference_fixture(name, step, mode):
-    gold = _gold()
-    pin = json.load(open(os.path.join(ROOT, 'tests', 'golden', 'PINNING_twin.json')))['cases']
+    gold = harness.golden('twin_outputs.npz')
+    pin = harness.pinning('PINNING_twin.json')
     c = CT.twin_case(name)
     cam = CT.twin_cam(O.make_cam_intrinsics, c)
     sd = {k: np.asarray(v) for k, v in c['sd'].items()}
