@@ -8,7 +8,7 @@ Follows /root/reference/code/test_utils/export_res.py:
   export_res_img (maps part)  :43-75   Depth_val_vol[0, d] = 1 * d_candi[d] (:49-52); conf = exp(max_d BV) (:56-59);
                                        (map * scale).astype(np.uint16) (:74-75)
   export2pgm                  mio/imgIO.py:9-10  PIL fromarray(uint16).convert('I').save('*.pgm')
-Pinned against the live reference by tests/golden/make_golden_export.py -> tests/golden/export_outputs.npz
+Pinned against the live reference by tests/golden/make_golden.py export -> tests/golden/export_outputs.npz
 (floating point: torch's vectorised exp / sum order differ from the plain loops here by <= 2 ulp, so the
 uint16 maps are pinned to +-1 LSB and the float maps to 2e-6 relative; the PGM byte format is pinned exactly).
 """

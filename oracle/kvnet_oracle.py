@@ -3,7 +3,7 @@
 TEST INFRASTRUCTURE ONLY (see planesweep_oracle.py header for the rules).
 
 numpy float32 restatement (im2col + BLAS sgemm) of:
-  models/psm_submodule.py:10-16,31-49,76-167   feature CNN (batch-statistics BN)
+  models/psm_submodule.py:10-16,31-49,76-167   feature CNN (batch-statistics BN; running statistics in .eval())
   models/basic.py:53-139                        K-Net (conv3d + BN3d residual stack)
   models/basic.py:223-323                       D-Net forward
   models/Refine.py:24-107                       R-Net (RefineNet_DPV_upsample)
@@ -159,60 +159,89 @@ class Params:
         return self.sd[name]
 
 
-def _convbn(P, pre, x, stride, pad, dilation):
+def batch_norm_eval(x, gamma, beta, running_mean, running_var, eps=BN_EPS):
+    """nn.BatchNorm{2,3}d.forward in eval mode (ATen's CPU transform, batch_norm_cpu_collect_linear_and_constant_terms),
+    per channel in float32:
+        alpha = (1 / sqrt(running_var + eps)) * gamma,   beta' = beta - running_mean * alpha,   y = x * alpha + beta'
+    The running buffers are only read."""
+    x = np.asarray(x, f32)
+    invstd = f32(1) / np.sqrt(np.asarray(running_var, f32) + f32(eps))
+    alpha = (invstd * np.asarray(gamma, f32)).astype(f32)
+    beta2 = (np.asarray(beta, f32) - np.asarray(running_mean, f32) * alpha).astype(f32)
+    shp = (1, -1) + (1,) * (x.ndim - 2)
+    return (x * alpha.reshape(shp) + beta2.reshape(shp)).astype(f32)
+
+
+def tracked(P, pre):
+    """Whether BatchNorm `pre` tracks running statistics: the state_dict holds its running_mean, as in the reference's
+    module tree. Tracked: the 11 BatchNorm3d of K-Net (psm_submodule.convbn_3d :19-23, used by basic.py:71-94) and the
+    downsample BatchNorm2d of the feature CNN's layer2.0 and layer3.0 (psm_submodule.py:128-131). Every other layer
+    comes from psm_submodule.convbn (:10-16) with bn_running_avg=False."""
+    return (pre + '.running_mean') in P.sd
+
+
+def bn(P, pre, x, training=True):
+    """BatchNorm `pre` (pre.weight, pre.bias): running statistics in eval mode for a tracked layer, batch statistics
+    otherwise (also in eval mode: nn.BatchNorm with track_running_stats=False)."""
+    if not training and tracked(P, pre):
+        return batch_norm_eval(x, P(pre + '.weight'), P(pre + '.bias'), P(pre + '.running_mean'), P(pre + '.running_var'))
+    return batch_norm(x, P(pre + '.weight'), P(pre + '.bias'))
+
+
+def _convbn(P, pre, x, stride, pad, dilation, training=True):
     """psm_submodule.convbn :10-16 -> Sequential(Conv2d(bias=False), BatchNorm2d)."""
     w = P(pre + '.0.weight')
     p = dilation if dilation > 1 else pad
     y = conv2d(x, w, None, stride, p, dilation)
-    return batch_norm(y, P(pre + '.1.weight'), P(pre + '.1.bias'))
+    return bn(P, pre + '.1', y, training)
 
 
-def _basic_block(P, pre, x, stride, pad, dilation, has_down):
+def _basic_block(P, pre, x, stride, pad, dilation, has_down, training=True):
     """psm_submodule.BasicBlock :31-49 (no ReLU after the residual add)."""
-    out = relu(_convbn(P, pre + '.conv1.0', x, stride, pad, dilation))
-    out = _convbn(P, pre + '.conv2', out, 1, pad, dilation)
+    out = relu(_convbn(P, pre + '.conv1.0', x, stride, pad, dilation, training))
+    out = _convbn(P, pre + '.conv2', out, 1, pad, dilation, training)
     if has_down:
         sc = conv2d(x, P(pre + '.downsample.0.weight'), None, stride, 0, 1)
-        x = batch_norm(sc, P(pre + '.downsample.1.weight'), P(pre + '.downsample.1.bias'))
+        x = bn(P, pre + '.downsample.1', sc, training)
     return out + x
 
 
-def _layer(P, pre, x, blocks, stride, dilation, has_down):
+def _layer(P, pre, x, blocks, stride, dilation, has_down, training=True):
     for i in range(blocks):
         x = _basic_block(P, '%s.%d' % (pre, i), x, stride if i == 0 else 1, 1, dilation,
-                         has_down and i == 0)
+                         has_down and i == 0, training)
     return x
 
 
-def feature_extraction(P, pre, x):
+def feature_extraction(P, pre, x, training=True):
     """psm_submodule.feature_extraction.forward :141-167 (multi_scale=True).
     pre = 'feature_extractor.feature_extraction'. Returns (layer1 out @1/2, feat @1/4)."""
-    o = relu(_convbn(P, pre + '.firstconv.0', x, 2, 1, 1))
-    o = relu(_convbn(P, pre + '.firstconv.2', o, 1, 1, 1))
-    o = relu(_convbn(P, pre + '.firstconv.4', o, 1, 1, 1))
-    l1 = _layer(P, pre + '.layer1', o, 3, 1, 1, False)
-    raw = _layer(P, pre + '.layer2', l1, 16, 2, 1, True)
-    o = _layer(P, pre + '.layer3', raw, 3, 1, 1, True)
-    skip = _layer(P, pre + '.layer4', o, 3, 1, 2, False)
+    o = relu(_convbn(P, pre + '.firstconv.0', x, 2, 1, 1, training))
+    o = relu(_convbn(P, pre + '.firstconv.2', o, 1, 1, 1, training))
+    o = relu(_convbn(P, pre + '.firstconv.4', o, 1, 1, 1, training))
+    l1 = _layer(P, pre + '.layer1', o, 3, 1, 1, False, training)
+    raw = _layer(P, pre + '.layer2', l1, 16, 2, 1, True, training)
+    o = _layer(P, pre + '.layer3', raw, 3, 1, 1, True, training)
+    skip = _layer(P, pre + '.layer4', o, 3, 1, 2, False, training)
     hw = skip.shape[2:]
     branches = []
     for name, k in (('branch1', 64), ('branch2', 32), ('branch3', 16), ('branch4', 8)):
         b = avg_pool2d(skip, k)
-        b = relu(_convbn(P, '%s.%s.1' % (pre, name), b, 1, 0, 1))
+        b = relu(_convbn(P, '%s.%s.1' % (pre, name), b, 1, 0, 1, training))
         branches.append(upsample_bilinear_ac(b, hw))
     b1, b2, b3, b4 = branches
     cat = np.concatenate((raw, skip, b4, b3, b2, b1), axis=1)
-    o = relu(_convbn(P, pre + '.lastconv.0', cat, 1, 1, 1))
+    o = relu(_convbn(P, pre + '.lastconv.0', cat, 1, 1, 1, training))
     feat = conv2d(o, P(pre + '.lastconv.2.weight'), None, 1, 0, 1)
     return l1, feat
 
 
-def d_net(P, ref_frame, src_frames, src_cam_poses, cam_intrinsics, d_candi, sigma, feat_dist='L2'):
+def d_net(P, ref_frame, src_frames, src_cam_poses, cam_intrinsics, d_candi, sigma, feat_dist='L2', training=True):
     """models/basic.py:223-323 with use_img_intensity=True, BV_log=True,
     output_features=True, BV_predict=None."""
     assert src_frames.shape[0] == 1
     l1, feats = feature_extraction(P, 'feature_extractor.feature_extraction',
-                                   np.concatenate((src_frames[0], ref_frame), axis=0))
+                                   np.concatenate((src_frames[0], ref_frame), axis=0), training)
     feat_ref_l1 = l1[-1:]
     feat_src = feats[:-1][None]
     feat_ref = feats[-1:]
@@ -226,10 +255,10 @@ def d_net(P, ref_frame, src_frames, src_cam_poses, cam_intrinsics, d_candi, sigm
     return BV, [feat_ref[:, :-3], feat_ref_l1]
 
 
-def kv_net(P, vol, pre='kv_net'):
+def kv_net(P, vol, pre='kv_net', training=True):
     """models/basic.py:113-139 (if_normalize=False, up_sample_ratio=None)."""
     def cb(name, x):
-        return batch_norm(conv3d(x, P(name + '.0.weight')), P(name + '.1.weight'), P(name + '.1.bias'))
+        return bn(P, name + '.1', conv3d(x, P(name + '.0.weight')), training)
     c0 = relu(cb(pre + '.dres0.0', vol))
     c0 = relu(cb(pre + '.dres0.2', c0))
     c = c0
@@ -261,13 +290,15 @@ def r_net(P, dpv_raw, img_features, pre='r_net'):
 
 
 def kvnet_forward(sd, ref_frame, src_frames, src_cam_poses, cam_intrinsics, d_candi, sigma,
-                  BV_predict=None, t_win_r=2, cam_intrinsics_call=None):
+                  BV_predict=None, t_win_r=2, cam_intrinsics_call=None, training=True):
     """models/KVNET.py:93-185 (if_refined=True, refineNet_name='DPV').
     cam_intrinsics: the dict captured at construction (used by D-Net, KVNET.py:64-67);
     cam_intrinsics_call: the per-call dict used by the K-Net image warp (:160-161),
-    defaults to the same. Returns (dmap_cur_refined, dmap_refined, BV_cur, DPV)."""
+    defaults to the same. training=False is the module in .eval(): the BatchNorm layers that track running
+    statistics use them (tracked), every other layer keeps batch statistics.
+    Returns (dmap_cur_refined, dmap_refined, BV_cur, DPV)."""
     P = sd if isinstance(sd, Params) else Params(sd)
-    BV_cur, feats = d_net(P, ref_frame, src_frames, src_cam_poses, cam_intrinsics, d_candi, sigma)
+    BV_cur, feats = d_net(P, ref_frame, src_frames, src_cam_poses, cam_intrinsics, d_candi, sigma, training=training)
     feats.append(ref_frame)
     dmap_cur_refined = r_net(P, np.exp(BV_cur), feats)
     if BV_predict is None or not G.valid_dpv(BV_predict):
@@ -283,7 +314,7 @@ def kvnet_forward(sd, ref_frame, src_frames, src_cam_poses, cam_intrinsics, d_ca
     D = len(d_candi)
     ref_rep = np.repeat(ref_dw[0][:, None], D, axis=1)
     vol = np.concatenate((np.concatenate(warped, axis=0), ref_rep, BV_cur - BV_predict), axis=0)[None]
-    gain = kv_net(P, vol)
+    gain = kv_net(P, vol, training=training)
     DPV = G.log_softmax(gain[:, 0] + BV_predict, axis=1)
     dmap_refined = r_net(P, np.exp(DPV), feats)
     return dmap_cur_refined, dmap_refined, BV_cur, DPV

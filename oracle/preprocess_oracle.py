@@ -7,7 +7,7 @@ not vendored under /root/reference (requirements.txt pins no versions); their al
   * Pillow libImaging/Geometry.c ImagingScaleAffine, nearest filter: xo = 0.5*scale; for each output sample take
     (int)xo, then xo += scale (double accumulation);
   * torchvision to_tensor: uint8 HWC -> float32 CHW, .div(255); Normalize: .sub_(mean).div_(std), fp32.
-Pinned bit-exactly against Pillow 12.2 / torchvision 0.26 run here: tests/golden/make_golden_preprocess.py.
+Pinned bit-exactly against Pillow 12.2 / torchvision 0.26 run here: tests/golden/make_golden.py preprocess.
 """
 import numpy as np
 

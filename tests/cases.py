@@ -132,7 +132,7 @@ KVNET_CASES = ['kvnet_256_d16', 'kvnet_256x320_d8']
 
 
 # ---- the BASELINE.json configurations at (or standing in for) their full sizes ----------------------------------
-# Fixtures: tests/golden/make_golden_configs.py (live reference, FREE-RUNNING: every step is fed the reference's own
+# Fixtures: tests/golden/make_golden.py configs (live reference, FREE-RUNNING: every step is fed the reference's own
 # propagated prior; the engine under test feeds its own, so the comparison includes the drift of the recursion).
 KITTI = dict(fx=721.5377, fy=721.5377, cx=624.0, cy=188.0)     # KITTI-like pinhole centred on the 1248x376 frame
 BIG_CFG = {
@@ -201,6 +201,13 @@ def stats(a):
     return np.array([a[fin].sum(), np.square(a[fin]).sum(), float(fin.sum())], np.float64)
 
 
+def summary(a):
+    """Full-array statistics stored beside a strided sample: sum, sum of squares, finite count, max |a| (finite values)."""
+    a = np.asarray(a, np.float64)
+    fin = np.isfinite(a)
+    return np.concatenate([stats(a), [float(np.abs(a[fin]).max()) if fin.any() else 0.0]])
+
+
 # ---- output stage (SURVEY 8 f-2): a refined log-DPV, its plane depths and the (normalised) reference image --------
 def export_case(name):
     """-> bv [1, D, H, W] float32 log-probabilities, d_candi float64 [D], img [1, 3, H, W] float32."""
@@ -250,7 +257,7 @@ def lba_case(name):
 LBA_CASES = ['lba_v1_c5_37x53', 'lba_v3_c3_48x64']
 
 
-# ---- a14: calibrations pushed through the reference's intrinsics recipe (tests/golden/make_golden_camera.py) -------
+# ---- a14: calibrations pushed through the reference's intrinsics recipe (tests/golden/make_golden.py camera) -------
 CAMERA_CASES = {
     '7scenes_to_160x120': dict(width=640, height=480, fx=585.0, fy=585.0, cx=320.0, cy=240.0, out_size=[160, 120]),
     'scannet_to_96x64': dict(width=1296, height=968, fx=1170.187988, fy=1170.187988, cx=647.75, cy=483.75, out_size=[96, 64]),

@@ -1,4 +1,4 @@
-"""Seeded cases of conv_math='f16' (numpy only): shared by tests/golden/make_golden_f16.py, which runs the unmodified
+"""Seeded cases of conv_math='f16' (numpy only): shared by tests/golden/make_golden.py f16, which runs the unmodified
 reference on them with its convolutions' operands rounded, and by the tests.
 
 Arithmetic emulated on the reference (forward pre-hooks on the convolution modules):
@@ -13,7 +13,7 @@ Cases (steps: 0 = first window):
     train-mode prior (configs_priors_c23_640x480_d64_v4_stream30.npz);
   - stream_256_d16: 256x256, D = 16, 6 frames free-running in train mode (each step fed the arithmetic's own propagated
     prior);
-  - eval_256_d16: kvnet_256_d16 in .eval() with the running statistics make_golden_eval.py warmed (eval_outputs.npz):
+  - eval_256_d16: kvnet_256_d16 in .eval() with the running statistics make_golden.py eval warmed (eval_outputs.npz):
     first window + one steady step re-seeded with the train-mode prior of reference_outputs.npz;
   - r1_256_d16: t_win_r = 1 (V = 2), train mode: first window + one re-seeded steady step.
 """
@@ -58,7 +58,7 @@ def cam(make_cam, c):
 
 
 def running_stats():
-    """The running statistics make_golden_eval.py warmed for kvnet_256_d16 (state_dict name -> array)."""
+    """The running statistics make_golden.py eval warmed for kvnet_256_d16 (state_dict name -> array)."""
     g = harness.golden('eval_outputs.npz')
     pre = 'eval/kvnet_256_d16/rs/'
     return {k[len(pre):]: np.asarray(g[k]) for k in g.files if k.startswith(pre)}

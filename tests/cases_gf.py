@@ -2,7 +2,7 @@
 models/GF, as RefineNet_DGF (models/Refine.py:587-641) uses them and beyond: ragged sizes, the KVNET-DGF 480x640 shape,
 flat guides, wider boxes, N = 2, three channels with and without a broadcast guide, and a larger eps.
 
-Shared by tests/golden/make_golden_gf.py (which runs the unmodified reference and torch autograd through it on them) and
+Shared by tests/golden/make_golden.py gf (which runs the unmodified reference and torch autograd through it on them) and
 the tests. Every input and every upstream gradient is regenerated from its seed; the fixtures hold outputs and gradients.
 """
 import numpy as np
@@ -53,10 +53,3 @@ SUB_LIMIT = 2500        # values per stored array (strided, cases.subsample_to)
 
 def sub(a):
     return cases.subsample_to(a, SUB_LIMIT)
-
-
-def summary(a):
-    """Full-array statistics stored beside the strided sample: sum, sum of squares, finite count, max |a|."""
-    a = np.asarray(a, np.float64)
-    fin = np.isfinite(a)
-    return np.concatenate([cases.stats(a), [float(np.abs(a[fin]).max()) if fin.any() else 0.0]])

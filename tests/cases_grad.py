@@ -1,7 +1,7 @@
 """Seeded cases for the gradients of the geometry mirrors (numpy only): the image / feature warp
 (warp_img_feats_v3 / _mgpu), the DPV resample (resample_vol_cuda) and the depth regression (depth_val_regression).
 
-Shared by tests/golden/make_golden_grad.py (which runs torch autograd through the unmodified reference on them) and the
+Shared by tests/golden/make_golden.py grad (which runs torch autograd through the unmodified reference on them) and the
 tests. Every input and every upstream gradient is regenerated from its seed; the fixtures hold gradients only.
 """
 import math
@@ -105,9 +105,3 @@ SUB_LIMIT = 8000        # values per stored gradient array (strided, cases.subsa
 
 def sub(a):
     return cases.subsample_to(a, SUB_LIMIT)
-
-
-def summary(a):
-    """Full-array statistics stored beside the strided sample: sum, sum of squares, finite count, max |a|."""
-    a = np.asarray(a, np.float64)
-    return np.concatenate([cases.stats(a), [float(np.abs(a).max())]])

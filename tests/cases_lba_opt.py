@@ -1,6 +1,6 @@
 """Seeded scenes for the LBA pose optimiser (ICP/opt_pose_numerical.py local_BA_direct(_parallel)), numpy only.
 
-Shared by tests/golden/make_golden_lba_opt.py (which runs the live reference on them and commits its outputs), the tests and
+Shared by tests/golden/make_golden.py lba_opt (which runs the live reference on them and commits its outputs), the tests and
 tools/bench_lba.py. Every input is regenerated from its seed, so the fixtures hold reference outputs only.
 """
 import math

@@ -1,6 +1,6 @@
 """Seeded cases for the DPV statistics mirrors (numpy only): mutils.misc.depth_var and mutils.misc.dpv_statistics.
 
-Shared by tests/golden/make_golden_stats.py (which runs the unmodified reference and torch autograd through it on them)
+Shared by tests/golden/make_golden.py stats (which runs the unmodified reference and torch autograd through it on them)
 and the tests. Every input and every upstream gradient is regenerated from its seed; the fixtures hold outputs and
 gradients only.
 """
@@ -75,10 +75,3 @@ SUB_LIMIT = 2500        # values per stored array (strided, cases.subsample_to)
 
 def sub(a):
     return cases.subsample_to(a, SUB_LIMIT)
-
-
-def summary(a):
-    """Full-array statistics stored beside the strided sample: sum, sum of squares, finite count, max |a|."""
-    a = np.asarray(a, np.float64)
-    fin = np.isfinite(a)
-    return np.concatenate([cases.stats(a), [float(np.abs(a[fin]).max()) if fin.any() else 0.0]])

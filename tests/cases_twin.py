@@ -1,7 +1,7 @@
 """Seeded KVNET cases at temporal window radii other than 2 (numpy only).
 
 KVNET(t_win_r=r) reads V = 2r source views per reference frame, and K-Net's first layer takes 3(2r + 1) + 1 = 3V + 4
-channels: 10 at r = 1, 22 at r = 3 (16 at the default r = 2, 28 at r = 4). Shared by tests/golden/make_golden_twin.py (which
+channels: 10 at r = 1, 22 at r = 3 (16 at the default r = 2, 28 at r = 4). Shared by tests/golden/make_golden.py twin (which
 runs the unmodified reference on them) and the tests. Every input is regenerated from its seed.
 
 Steady steps are re-seeded with a train-mode prior of the reference that the repository already holds at the same

@@ -1,4 +1,4 @@
-"""CPU oracle of KVNET.forward in conv_math='f16' (numpy float32, TEST INFRASTRUCTURE ONLY): tests/oracle_eval.py's
+"""CPU oracle of KVNET.forward in conv_math='f16' (numpy float32, TEST INFRASTRUCTURE ONLY): oracle/kvnet_oracle.py's
 KVNET with every convolution that the engine runs on tensor cores computed on RN_f16-rounded operands,
 sum RN_f16(x) * RN_f16(w) accumulated in fp32. The 3-input-channel first layer of the feature CNN stays fp32. Everything
 else (bias, BatchNorm, residual adds, the sweep, softmax, R-Net's activations) is the fp32 oracle unchanged.
@@ -11,7 +11,6 @@ import contextlib
 import numpy as np
 
 from oracle import kvnet_oracle as N
-from tests import oracle_eval as E
 
 f32 = np.float32
 
@@ -43,7 +42,7 @@ def f16_convolutions():
 
 
 def kvnet_forward(sd, ref_frame, src_frames, src_cam_poses, cam, d_candi, sigma, BV_predict=None, training=False):
-    """oracle_eval.kvnet_forward with conv_math='f16' convolutions."""
+    """kvnet_oracle.kvnet_forward with conv_math='f16' convolutions."""
     with f16_convolutions():
-        return E.kvnet_forward(sd, ref_frame, src_frames, src_cam_poses, cam, d_candi, sigma, BV_predict=BV_predict,
+        return N.kvnet_forward(sd, ref_frame, src_frames, src_cam_poses, cam, d_candi, sigma, BV_predict=BV_predict,
                                training=training)

@@ -100,7 +100,7 @@ def dgf_refine(dmap, img, sd, pre='r_net.'):
     return guided_filter(x, y, 1, 1e-8)
 
 
-# ---- seeded inputs of the guided filter alone (tests/golden/make_golden_refine.py, tests/test_gpu_refine.py) -----------
+# ---- seeded inputs of the guided filter alone (tests/golden/make_golden.py refine, tests/test_gpu_refine.py) -----------
 GF_CASES = ['gf_ragged_13x17_x4', 'gf_ragged_37x53_x2', 'gf_textured_120x160_x4', 'gf_flat_120x160_x4']
 
 

@@ -1,7 +1,7 @@
 """GPU parity at the BASELINE.json configurations' real sizes (SURVEY 8d C2..C5; VERDICT r1 'missing #1').
 
 Fixtures: tests/golden/configs_*.npz, produced by the UNMODIFIED reference driven free-running through its own
-test_utils/test_KVNet.py:test (tests/golden/make_golden_configs.py). Here the engine is driven the same way and
+test_utils/test_KVNet.py:test (tests/golden/make_golden.py configs). Here the engine is driven the same way and
 feeds ITS OWN propagated prior from step to step, so the per-step numbers below include the drift of the K-Net
 recursion over the whole stream (30 frames for configs[2]) - nothing is re-seeded. One extra case re-seeds a single
 steady step with the reference's full prior to separate the per-step deviation from the accumulated one.
@@ -11,7 +11,7 @@ Gates are on probabilities (DESIGN.md 'tolerance domain'):
  * K-Net outputs (filtered DPV, its refinement, the propagated prior) and the expected depth: the K-Net recursion amplifies fp32
    rounding noise from step to step, for ANY two fp32 implementations. The floor is measured at these shapes between the
    live reference and the independent numpy oracle, both free-running (tests/golden/PINNING_drift_<case>.json from
-   tests/golden/make_golden_drift.py; PINNING_configs.json for cases without a drift record): the gate at step k is
+   tests/golden/make_golden.py drift; PINNING_configs.json for cases without a drift record): the gate at step k is
    max(base, 4 x the largest floor seen up to step k), base = 5e-4 on probabilities / 1 mm on depth (north_star's 1e-4 and
    1 mm are met at step 0 and by the re-seeded single step at the ScanNet shapes; at KITTI's 0.46 m plane spacing two fp32
    implementations already differ by 2.5 mm in the first window).

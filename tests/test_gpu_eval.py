@@ -3,7 +3,7 @@
  * Op level: nrgbd_conv_nhwc_h2_affine against the fp32 numpy oracle at the 6e-6 convolution gate of test_gpu_conv_h2.py
    (3-D k3 64 -> 64 with / without a pair residual and ReLU, pair output, both tile orientations; 2-D 1x1 stride 2 with
    fp32 output), bit-identical from run to run and under the schedule switches 8 / 32 (test_gpu_conv_sched.py).
- * Engine against the eval fixtures of tests/golden/make_golden_eval.py (unmodified reference, warmed running statistics),
+ * Engine against the eval fixtures of tests/golden/make_golden.py eval (unmodified reference, warmed running statistics),
    in all three conv_math modes: first window at 1e-4 on probabilities and 1 mm on depth; a steady K-Net step re-seeded with
    the reference's train-mode prior at train mode's gate for that step (C3: 1.5e-4 in f16x3, 5e-4 otherwise), and at twice
    the measured fp32-vs-fp32 floor of PINNING_eval.json at the 16-plane shape; every full array through the relative
@@ -22,12 +22,11 @@ import torch
 from oracle import kvnet_oracle as N
 from oracle import planesweep_oracle as O
 from tests import cases, harness
-from tests import oracle_eval as E
 from tests.conftest import maxabs
 from tests.harness import NAMES4, T, rel_err
 
 pytestmark = pytest.mark.gpu
-SUB_LIMIT = 8000          # the fixture's strided samples (make_golden_eval.py)
+SUB_LIMIT = 8000          # the fixture's strided samples (make_golden.py eval)
 TOL_SUMSQ_REL = 1e-4      # full-array check: relative deviation of the sum of squared probabilities
 TOL_FIRST = 1e-4
 TOL_DEPTH_MM = 1.0
@@ -51,7 +50,7 @@ def _coeffs(rng, C):
 
 
 def _affine_ref(y, g, b, rm, rv, res, relu):
-    out = E.batch_norm_eval(y, g, b, rm, rv)
+    out = N.batch_norm_eval(y, g, b, rm, rv)
     if res is not None:
         out = out + res
     return N.relu(out) if relu else out
@@ -122,7 +121,7 @@ def _case(name):
 
 
 def _eval_sd(c, gold, name):
-    """The case's weights with the running statistics the reference produced (make_golden_eval.py)."""
+    """The case's weights with the running statistics the reference produced (make_golden.py eval)."""
     sd = {k: np.asarray(v) for k, v in c['sd'].items()}
     pre = 'eval/%s/rs/' % name
     sd.update({k[len(pre):]: np.asarray(gold[k]) for k in gold.files if k.startswith(pre)})
@@ -204,7 +203,7 @@ def test_engine_eval_train_eval_on_one_engine():
     sd2 = m.state_dict()
     assert all(torch.equal(sd1[k].cpu(), sd2[k].cpu()) for k in sd1)
     ref_f, src_f, poses = cases.window(c, c['t_win_r'] + 1)
-    o = E.kvnet_forward({k: v.cpu().numpy() for k, v in sd1.items()}, ref_f, src_f, poses, cam, c['d'], c['sigma'],
+    o = N.kvnet_forward({k: v.cpu().numpy() for k, v in sd1.items()}, ref_f, src_f, poses, cam, c['d'], c['sigma'],
                         BV_predict=prior_eval, training=False)
     sub = lambda a: cases.subsample_to(a, SUB_LIMIT)     # noqa: E731  (sampled as every other comparison here)
     row = {nm: maxabs(np.exp(sub(a.cpu().numpy())), np.exp(sub(b))) for nm, a, b in zip(NAMES4, e2, o)}

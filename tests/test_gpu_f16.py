@@ -5,7 +5,7 @@
    (relative to the output scale). Also the BatchNorm sums, a pair output with y_lo = NULL (hi = RN_f16 of the fp32
    result, pad channels zero), the affine epilogue with a 22-bit pair residual, and the K-Net volume, the BatchNorm pass and
    the split pass with a NULL lo.
- * Engine against the reference with its convolutions' operands rounded to fp16 (tests/golden/make_golden_f16.py): first
+ * Engine against the reference with its convolutions' operands rounded to fp16 (tests/golden/make_golden.py f16): first
    windows and re-seeded steps within max(f16x3's gate, 2 F), free-running stream steps within max(f16x3's gate, 4 F), F the
    pinned deviation of the f16 oracle (tests/oracle_f16.py) from that reference, on probabilities and expected depth (for a
    steady step the largest of the case's steady steps). Against

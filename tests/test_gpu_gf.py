@@ -3,7 +3,7 @@
  * Forwards against tests/oracle_gf.py bit for bit on every case, which also holds the parallel scans' fp32 prefixes
    to the sequential double accumulation; BoxFilter on x, y, x*y and x*x of every case, bit for bit.
  * Backwards against the oracle's float64 backward and against the unmodified reference's torch autograd
-   (tests/golden/make_golden_gf.py), gated from the oracle-vs-reference floor pinned in PINNING_gf.json.
+   (tests/golden/make_golden.py gf), gated from the oracle-vs-reference floor pinned in PINNING_gf.json.
  * Plain inputs, inputs that require grad and torch.no_grad() give the same launches and bit-identical values; two
    runs give identical results; the reference's asserts are kept.
  * The reference's own models.KVNET.KVNET(refineNet_name='DGF') trained under train_utils/train_KVNet.py's L1 loss with
@@ -14,7 +14,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests import cases_gf as CG, oracle_gf as OG, harness
+from tests import cases, cases_gf as CG, oracle_gf as OG, harness
 from tests.test_oracle_gf import sumsq_allowance
 
 pytestmark = pytest.mark.gpu
@@ -39,7 +39,7 @@ def _gate(gold, pin, key, mine, orc):
     allow = FLOOR_X * p['maxabs_oracle'] + REL * p['max_ref']
     e_orc = float(np.abs(mine.astype(np.float64) - orc).max())
     e_ref = float(np.abs(CG.sub(mine).astype(np.float64) - gold[key]).max())
-    s, want = CG.summary(mine), gold[key + '/stats']
+    s, want = cases.summary(mine), gold[key + '/stats']
     harness.parity_dump('gf', key, {'vs_oracle': e_orc, 'vs_reference_sample': e_ref, 'floor': p['maxabs_oracle'], 'max_ref': p['max_ref'],
                 'gate': allow, 'rel_vs_oracle': e_orc / p['max_ref']})
     assert list(mine.shape) == p['shape']

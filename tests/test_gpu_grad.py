@@ -1,7 +1,7 @@
 """f-5 on the device: autograd through the warp_img_feats_v3 / _mgpu, resample_vol_cuda and depth_val_regression mirrors.
 
  * Each backward kernel against tests/oracle_grad.py (float64 sums) and against torch autograd through the unmodified
-   reference (tests/golden/make_golden_grad.py), gated from the oracle-vs-reference floor pinned in PINNING_grad.json.
+   reference (tests/golden/make_golden.py grad), gated from the oracle-vs-reference floor pinned in PINNING_grad.json.
  * The no-grad path: the same launches and bit-identical outputs whether or not the inputs require grad, under
    torch.no_grad() or not; the autograd path's forward value is the no-grad one, bit for bit.
  * The reference's own models.KVNET.KVNET (refineNet_name='DGF') trained for one step with the mirrors patched into
@@ -48,7 +48,7 @@ def _gate(gold, pin, key, mine, orc):
     allow = REL[op] * p['max_ref']
     e_orc = float(np.abs(mine.astype(np.float64) - orc).max())
     e_ref = float(np.abs(CG.sub(mine).astype(np.float64) - gold[key + '/g']).max())
-    s, want = CG.summary(mine), gold[key + '/stats']
+    s, want = cases.summary(mine), gold[key + '/stats']
     harness.parity_dump('grad', key, {'vs_oracle': e_orc, 'vs_reference_sample': e_ref, 'floor': p['maxabs_oracle'], 'max_ref': p['max_ref'],
                 'gate': allow})
     assert list(mine.shape) == p['shape']

@@ -1,6 +1,6 @@
 """GPU parity of the LBA depth-map back-warp and its gradients (SURVEY 8 f-3): warping.homography.back_warp_th_Rt(_msrc)
 mirrors against (i) the outputs of the unmodified reference and of torch autograd through it (tests/golden/lba_outputs.npz,
-tests/golden/make_golden_lba.py) and (ii) the numpy oracle; plus the optimiser-facing behaviour: autograd through the mirror
+tests/golden/make_golden.py lba) and (ii) the numpy oracle; plus the optimiser-facing behaviour: autograd through the mirror
 gives the pose gradients ICP/opt_pose_numerical.py:99-160 steps on, and a few Adam steps reduce a photometric loss."""
 import numpy as np
 import pytest

@@ -3,7 +3,7 @@
  * Op level: nrgbd_guided_filter_refine against tests/oracle_refine.py, bit for bit, on ragged sizes, a textured guide and a
    guide that is flat over whole regions (var_x = 0 there: A = cov / 1e-8), against the reference's RefineNet_DGF within its
    pinned floor, and bit-identical from run to run.
- * Engine against tests/golden/make_golden_refine.py (unmodified reference, re-seeded steady steps) in all three conv_math
+ * Engine against tests/golden/make_golden.py refine (unmodified reference, re-seeded steady steps) in all three conv_math
    modes. if_refined=False: -1 for both refined outputs, probabilities at 1e-4 on first windows and the train-mode K-Net gate
    on steady steps. DGF: depth maps in metres at GATE_MULT times the larger pinned oracle-vs-reference deviation of the step
    (the fp32-vs-fp32 floor of the ill-conditioned filter), and bit-close to the oracle's filter fed the engine's own DPV.

@@ -1,7 +1,7 @@
 """The depth_var and dpv_statistics mirrors on the device (mutils/misc.py:550-608).
 
  * Each kernel against tests/oracle_stats.py and against the unmodified reference's forward and torch autograd
-   (tests/golden/make_golden_stats.py), gated from the oracle-vs-reference floor pinned in PINNING_stats.json.
+   (tests/golden/make_golden.py stats), gated from the oracle-vs-reference floor pinned in PINNING_stats.json.
  * The plane indices of 'max' / 'min' equal the reference's on the tie case; E_mean inside dpv_statistics is
    depth_val_regression's, bit for bit.
  * Plain inputs, inputs that require grad and torch.no_grad() give the same launches and bit-identical values.
@@ -14,7 +14,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests import cases_stats as CS, oracle_stats as OS, harness
+from tests import cases, cases_stats as CS, oracle_stats as OS, harness
 
 pytestmark = pytest.mark.gpu
 T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()     # noqa: E731
@@ -38,7 +38,7 @@ def _gate(gold, pin, key, mine, orc):
     allow = REL[kind] * p['max_ref']
     e_orc = float(np.abs(mine.astype(np.float64) - orc).max())
     e_ref = float(np.abs(CS.sub(mine).astype(np.float64) - gold[key]).max())
-    s, want = CS.summary(mine), gold[key + '/stats']
+    s, want = cases.summary(mine), gold[key + '/stats']
     harness.parity_dump('stats', key, {'vs_oracle': e_orc, 'vs_reference_sample': e_ref, 'floor': p['maxabs_oracle'], 'max_ref': p['max_ref'],
                 'gate': allow})
     assert list(mine.shape) == p['shape']

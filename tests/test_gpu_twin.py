@@ -1,6 +1,6 @@
 """KVNET at temporal window radii 1 and 3 (V = 2 and 6 source views; K-Net input volumes of 10 and 22 channels) on the GPU.
 
- * Engine against tests/golden/make_golden_twin.py (unmodified reference, re-seeded steady steps) in all three conv_math
+ * Engine against tests/golden/make_golden.py twin (unmodified reference, re-seeded steady steps) in all three conv_math
    modes, train mode and .eval(): first windows at 1e-4 on probabilities and 1 mm on depth; a steady step at 640x480 D64 at
    train mode's K-Net gate for that arithmetic (test_gpu_configs.py: 1.5e-4 in f16x3, 5e-4 otherwise); the 16-plane steady
    steps at twice the pinned oracle-vs-reference floor (PINNING_twin.json, the largest of the case's steady steps); every
@@ -25,7 +25,7 @@ from tests.conftest import maxabs
 from tests.harness import NAMES4
 
 pytestmark = pytest.mark.gpu
-SUB_LIMIT = 8000          # the fixture's strided samples (make_golden_twin.py)
+SUB_LIMIT = 8000          # the fixture's strided samples (make_golden.py twin)
 TOL_SUMSQ_REL = 1e-4
 TOL_FIRST = 1e-4
 TOL_DEPTH_MM = 1.0

@@ -1,12 +1,11 @@
-"""CPU checks of the eval-mode oracle (tests/oracle_eval.py) against the eval fixtures of the unmodified reference
-(tests/golden/make_golden_eval.py), and of which layers eval mode touches."""
+"""CPU checks of the eval-mode oracle (oracle/kvnet_oracle.py, training=False) against the eval fixtures of the unmodified
+reference (tests/golden/make_golden.py eval), and of which layers eval mode touches."""
 import numpy as np
 import pytest
 
 from oracle import kvnet_oracle as N
 from oracle import planesweep_oracle as O
 from tests import cases, harness
-from tests import oracle_eval as E
 from tests.conftest import maxabs
 
 NAME = 'kvnet_256_d16'
@@ -41,7 +40,7 @@ def test_eval_oracle_vs_reference_fixture(step):
     ref_f, src_f, poses = cases.window(c, 2 + step)
     ref_gold = harness.golden('reference_outputs.npz')
     prior = ref_gold['kvnet/%s/step%d/BV_predict_next_full' % (NAME, step - 1)] if step else None      # as recorded
-    o = E.kvnet_forward(_sd(c, gold), ref_f, src_f, poses, cam, c['d'], c['sigma'], BV_predict=prior, training=False)
+    o = N.kvnet_forward(_sd(c, gold), ref_f, src_f, poses, cam, c['d'], c['sigma'], BV_predict=prior, training=False)
     key = 'eval/%s/step%d' % (NAME, step)
     for nm, a in zip(NAMES4, o):
         if '%s/%s' % (key, nm) not in gold.files:          # first window: the filtered outputs equal the stored ones
@@ -59,24 +58,24 @@ def test_untracked_layers_keep_batch_statistics_in_eval_mode():
     P = N.Params(_sd(c, gold))
     pre = 'feature_extractor.feature_extraction'
     x = c['frames'][2][None].astype(np.float32)
-    a = E._convbn(P, pre + '.firstconv.0', x, 2, 1, 1, True)
-    b = E._convbn(P, pre + '.firstconv.0', x, 2, 1, 1, False)
+    a = N._convbn(P, pre + '.firstconv.0', x, 2, 1, 1, True)
+    b = N._convbn(P, pre + '.firstconv.0', x, 2, 1, 1, False)
     assert np.array_equal(a, b)
-    assert np.array_equal(a, N._convbn(P, pre + '.firstconv.0', x, 2, 1, 1))
-    l1_t = E._layer(P, pre + '.layer1', N.relu(a), 3, 1, 1, False, True)
-    l1_e = E._layer(P, pre + '.layer1', N.relu(b), 3, 1, 1, False, False)
+    l1_t = N._layer(P, pre + '.layer1', N.relu(a), 3, 1, 1, False, True)
+    l1_e = N._layer(P, pre + '.layer1', N.relu(b), 3, 1, 1, False, False)
     assert np.array_equal(l1_t, l1_e)
-    blk_t = E._basic_block(P, pre + '.layer2.1', l1_t[:, :, ::2, ::2].repeat(2, axis=1), 1, 1, False, True)
-    blk_e = E._basic_block(P, pre + '.layer2.1', l1_t[:, :, ::2, ::2].repeat(2, axis=1), 1, 1, False, False)
+    blk_t = N._basic_block(P, pre + '.layer2.1', l1_t[:, :, ::2, ::2].repeat(2, axis=1), 1, 1, 1, False, True)
+    blk_e = N._basic_block(P, pre + '.layer2.1', l1_t[:, :, ::2, ::2].repeat(2, axis=1), 1, 1, 1, False, False)
     assert np.array_equal(blk_t, blk_e)                    # a block without a downsample: nothing tracked
-    d_t = E._basic_block(P, pre + '.layer2.0', l1_t, 2, 1, True, True)
-    d_e = E._basic_block(P, pre + '.layer2.0', l1_t, 2, 1, True, False)
+    d_t = N._basic_block(P, pre + '.layer2.0', l1_t, 2, 1, 1, True, True)
+    d_e = N._basic_block(P, pre + '.layer2.0', l1_t, 2, 1, 1, True, False)
     assert not np.array_equal(d_t, d_e)
-    assert E.tracked(P, pre + '.layer2.0.downsample.1') and not E.tracked(P, pre + '.layer2.0.conv1.0.1')
+    assert N.tracked(P, pre + '.layer2.0.downsample.1') and not N.tracked(P, pre + '.layer2.0.conv1.0.1')
     n_tracked = sum(1 for k in P.sd if k.endswith('.running_mean') and not k.startswith('d_net.'))
     assert n_tracked == 13
-    # training=True restates the train-mode oracle exactly
+    # K-Net: eval mode reads the running buffers; without them every layer falls back to batch statistics
     rng = np.random.RandomState(0)
     vol = rng.standard_normal((1, 16, 4, 8, 8)).astype(np.float32)
-    assert np.array_equal(E.kv_net(P, vol, True), N.kv_net(P, vol))
-    assert not np.array_equal(E.kv_net(P, vol, False), N.kv_net(P, vol))
+    untracked = N.Params({k: v for k, v in P.sd.items() if '.running_' not in k})
+    assert np.array_equal(N.kv_net(untracked, vol, training=False), N.kv_net(untracked, vol, training=True))
+    assert not np.array_equal(N.kv_net(P, vol, training=False), N.kv_net(P, vol, training=True))

@@ -1,4 +1,4 @@
-"""conv_math='f16' fixtures and oracle on the CPU (tests/golden/make_golden_f16.py, tests/oracle_f16.py).
+"""conv_math='f16' fixtures and oracle on the CPU (tests/golden/make_golden.py f16, tests/oracle_f16.py).
 
  * The convolutions whose operands the fixtures round are exactly the ones the engine runs on tensor cores: every
    convolution of the architecture except the 3-input-channel first layer (from arch.kvnet_param_specs).

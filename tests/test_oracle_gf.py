@@ -1,6 +1,6 @@
 """CPU checks of tests/oracle_gf.py, the numpy restatement of the reference's models/GF GuidedFilter and BoxFilter, and of
 the host side of their mirrors in neuralrgbd_b200.models.GF:
- * the oracle against the unmodified reference's forward and torch autograd (tests/golden/make_golden_gf.py) at the
+ * the oracle against the unmodified reference's forward and torch autograd (tests/golden/make_golden.py gf) at the
    pinned floor; the forwards are bit-exact;
  * torch.autograd.gradcheck (float64 central differences) of the oracle backwards against their float64 forwards;
  * the mirrors' constructor, attributes, asserts and CPU-tensor error, and the install / uninstall round trip of the
@@ -13,7 +13,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests import cases_gf as CG, oracle_gf as OG, harness
+from tests import cases, cases_gf as CG, oracle_gf as OG, harness
 from tests.conftest import ROOT
 
 
@@ -26,7 +26,7 @@ def _check(gold, pin, key, mine):
     assert list(mine.shape) == p['shape']
     # the oracle is deterministic: it reproduces the deviation it was pinned at
     assert np.abs(CG.sub(mine).astype(np.float64) - gold[key]).max() <= p['maxabs_oracle']
-    s, want = CG.summary(mine), gold[key + '/stats']
+    s, want = cases.summary(mine), gold[key + '/stats']
     assert s[2] == want[2] and abs(s[3] - want[3]) <= p['maxabs_oracle']
     assert abs(s[1] - want[1]) <= 1e-5 * want[1] + sumsq_allowance(want, p['maxabs_oracle'])
     assert abs(s[0] - want[0]) <= p['maxabs_oracle'] * want[2] + 1e-9 * abs(want[0])

@@ -1,5 +1,5 @@
 """CPU checks of tests/oracle_grad.py, the numpy backward of the geometry mirrors (f-5):
- * against torch autograd through the unmodified reference (tests/golden/make_golden_grad.py), at the pinned floor;
+ * against torch autograd through the unmodified reference (tests/golden/make_golden.py grad), at the pinned floor;
  * torch.autograd.gradcheck (float64 central differences) of each oracle backward against its float64 forward over the
    same taps, and the taps against the pinned fp32 forward of oracle/planesweep_oracle.py;
  * the properties the kernels rely on: the six faces of a resampled volume get zero gradient, the clamp mask is the one
@@ -25,7 +25,7 @@ def _check(gold, pin, key, mine):
     assert list(mine.shape) == p['shape']
     # the oracle is deterministic: it reproduces the deviation it was pinned at (float64 sums vs the reference's fp32)
     assert np.abs(CG.sub(mine).astype(np.float64) - gold[key + '/g']).max() <= p['maxabs_oracle']
-    s, want = CG.summary(mine), gold[key + '/stats']
+    s, want = cases.summary(mine), gold[key + '/stats']
     assert s[2] == want[2] and abs(s[3] - want[3]) <= p['maxabs_oracle']
     assert abs(s[1] - want[1]) <= 1e-5 * want[1]
     assert abs(s[0] - want[0]) <= p['maxabs_oracle'] * want[2]

@@ -1,5 +1,5 @@
 """The LBA pose optimiser, oracle first (CPU): oracle/lba_opt_oracle.py against the unmodified reference's
-ICP/opt_pose_numerical.py local_BA_direct(_parallel) (tests/golden/lba_opt_outputs.npz, make_golden_lba_opt.py), its
+ICP/opt_pose_numerical.py local_BA_direct(_parallel) (tests/golden/lba_opt_outputs.npz, make_golden.py lba_opt), its
 Adam against torch.optim.Adam, the initial-pose conversion, and the drop-in patch of ICP.opt_pose_numerical."""
 import json
 import os

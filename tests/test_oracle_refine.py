@@ -1,5 +1,5 @@
 """KVNET's refinement configurations on the host: the guided-filter oracle (tests/oracle_refine.py) against the unmodified
-reference's RefineNet_DGF (tests/golden/make_golden_refine.py), and the mirror's constructor surface - module tree,
+reference's RefineNet_DGF (tests/golden/make_golden.py refine), and the mirror's constructor surface - module tree,
 state_dict keys / shapes / order, strict checkpoint loading and printed lines - for refineNet_name='DGF', if_refined=False
 and the depth-upsampled DPV R-Net (if_upsample_d=True) against the reference's own lists."""
 import contextlib

@@ -1,6 +1,6 @@
 """CPU checks of tests/oracle_stats.py, the numpy restatement of the reference's depth_var and dpv_statistics, and of the
 host-side logic of their mirrors in neuralrgbd_b200.mutils.misc:
- * the oracle against the unmodified reference's forward and torch autograd (tests/golden/make_golden_stats.py), at the
+ * the oracle against the unmodified reference's forward and torch autograd (tests/golden/make_golden.py stats), at the
    pinned floor, and the max / min plane indices exactly, the tie case's border pixels included;
  * torch.autograd.gradcheck (float64 central differences) of each oracle backward against its float64 forward;
  * the reference's behaviour the mirror keeps: names selected by identity, 'variance' before 'E_mean', 'min' without
@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests import cases_stats as CS, oracle_stats as OS, harness
+from tests import cases, cases_stats as CS, oracle_stats as OS, harness
 
 
 gold = harness.golden_fixture('stats_outputs.npz')
@@ -21,7 +21,7 @@ def _check(gold, pin, key, mine):
     assert list(mine.shape) == p['shape']
     # the oracle is deterministic: it reproduces the deviation it was pinned at
     assert np.abs(CS.sub(mine).astype(np.float64) - gold[key]).max() <= p['maxabs_oracle']
-    s, want = CS.summary(mine), gold[key + '/stats']
+    s, want = cases.summary(mine), gold[key + '/stats']
     assert s[2] == want[2] and abs(s[3] - want[3]) <= p['maxabs_oracle']
     assert abs(s[1] - want[1]) <= 1e-5 * want[1]
     assert abs(s[0] - want[0]) <= p['maxabs_oracle'] * want[2]

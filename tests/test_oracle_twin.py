@@ -1,5 +1,5 @@
 """CPU checks at temporal window radii other than 2: the numpy oracle against the fixtures of the unmodified reference
-(tests/golden/make_golden_twin.py) at r = 1 and 3, and KVNET(t_win_r=r)'s state_dict against the reference's for r = 1..4."""
+(tests/golden/make_golden.py twin) at r = 1 and 3, and KVNET(t_win_r=r)'s state_dict against the reference's for r = 1..4."""
 import contextlib
 import io
 import json
@@ -8,10 +8,10 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import kvnet_oracle as N
 from oracle import planesweep_oracle as O
 from tests import cases, harness
 from tests import cases_twin as CT
-from tests import oracle_eval as E
 from tests.conftest import maxabs
 
 NAMES4 = ['dmap_cur_refined', 'dmap_refined', 'BV_cur', 'DPV']
@@ -47,7 +47,7 @@ def test_oracle_vs_reference_fixture(name, step, mode):
         sd.update({k[len(pre):]: np.asarray(gold[k]) for k in gold.files if k.startswith(pre)})
     ref_f, src_f, poses = cases.window(c, c['t_win_r'] + step)
     assert src_f.shape[1] == 2 * c['t_win_r']
-    o = E.kvnet_forward(sd, ref_f, src_f, poses, cam, c['d'], c['sigma'], BV_predict=CT.prior(name, step) if step else None,
+    o = N.kvnet_forward(sd, ref_f, src_f, poses, cam, c['d'], c['sigma'], BV_predict=CT.prior(name, step) if step else None,
                         training=mode == 'train')
     key = 'twin/%s/%s/step%d' % (mode, name, step)
     checked = 0
