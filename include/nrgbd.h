@@ -401,8 +401,9 @@ int nrgbd_copy_channels(const float* x, long long P, int Cs_in, int c_off_in, in
  * models/GF/guided_filter.py GuidedFilter(r, eps) (KVNET(refineNet_name='DGF') uses r = 1, eps = 1e-8).
  * dmap [h][w] low-resolution depth; img: channel c (0..2) of pixel p at img[c * img_sc + p * img_sp], [H][W];
  * w0 [64][3], b0 [64], w1 [64], b1 [1] = r_net.feature_ext.{0,2}.{weight,bias}; out [H][W].
- * H / h == W / w > 1. ws: nrgbd_guided_filter_workspace_floats(H, W) floats. Box sums use the reference's
- * cumulative-sum form (double-accumulated prefixes rounded to fp32); no atomics, identical from run to run. */
+ * H / h == W / w > 1; H, W > 2r + 1. ws: nrgbd_guided_filter_workspace_floats(H, W) floats. One pass forms the guide
+ * (the 1x1 MLP of img) and the align-corners upsampled depth map, then nrgbd_guided_filter below filters the depth map
+ * guided by it (N = C_x = C_y = 1), with the same box sums and arithmetic; identical from run to run. */
 long long nrgbd_guided_filter_workspace_floats(int H, int W);
 int nrgbd_guided_filter_refine(const float* dmap, int h, int w, const float* img, long long img_sc, long long img_sp,
                                int H, int W, const float* w0, const float* b0, const float* w1, const float* b1,

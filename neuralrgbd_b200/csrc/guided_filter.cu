@@ -1,5 +1,6 @@
-// Guided-filter depth refinement: RefineNet_DGF.forward (models/Refine.py:620-641) with GuidedFilter(r, eps)
-// (models/GF/guided_filter.py) and its BoxFilter (models/GF/box_filter.py), for KVNET(refineNet_name='DGF').
+// Guided filter: GuidedFilter(r, eps) (models/GF/guided_filter.py) and its BoxFilter (models/GF/box_filter.py) on
+// N x C x H x W planes, forward and backward (the autograd mirrors in neuralrgbd_b200/models/GF), and the depth refinement
+// of KVNET(refineNet_name='DGF'), RefineNet_DGF.forward (models/Refine.py:620-641), which runs the same forward on one plane:
 //
 //   y = F.upsample(dmap, scale_factor=H/h, mode='bilinear', align_corners=True)
 //   x = Conv2d(64 -> 1, 1x1)(ReLU(Conv2d(3 -> 64, 1x1)(img)))
@@ -11,13 +12,26 @@
 // wherever the guide is locally flat, so a more accurate window sum would not reproduce the reference. Every other step is
 // one IEEE-rounded fp32 operation in the reference's order (no contraction), the bilinear taps and the 1x1 convolutions
 // in the FMA order of ATen's CPU kernels. No atomics: the output is identical from run to run.
+//
+// Parallel scans. A column pass (lines along H) gives a block 32 adjacent columns of one plane and cuts each column into
+// GF_COL_SEG segments, one per threadIdx.y: loads stay coalesced across the 32 columns. A row pass (lines along W) gives
+// each row a warp and each lane a contiguous segment. Every thread sums its segment in double, the segment totals are
+// scanned in double (shared memory across threadIdx.y, shuffles across lanes), and the thread re-walks its segment from
+// that offset, rounding each prefix to fp32. Only the double sums are reassociated; the fp32 prefixes are those of the
+// sequential double accumulation unless a reassociated double lands on the other side of an fp32 rounding boundary.
+//
+// Forward pass (ADJ = false): prefix sums cs (ATen's cumsum), then box_diff into dst. dst may be the source plane.
+// Adjoint pass (ADJ = true), autograd's order through box_filter.py: first the adjoint of box_diff (the slice / cat
+// backward: d cs[i] = g[i - r] - g[i + r + 1], and at i = n-1 the broadcast `right` slice's sum g[n-r..n-1] added to
+// g[n-1-r]), then cumsum's backward, a reverse prefix sum in double rounded per position. dst must not be the source.
+#include "../../include/nrgbd.h"
 #include "common.cuh"
 
 namespace {
 
 constexpr int GF_HID = 64;      // RefineNet_DGF.feature_ext: Conv2d(3, 64, 1) -> ReLU -> Conv2d(64, 1, 1)
 
-// planes [x | y | x*y | x*x], each [H][W]: the upsampled depth, the 1x1 MLP of the guide image and the two products
+// planes [x | y], each [H][W]: the 1x1 MLP of the guide image and the upsampled depth
 __global__ void __launch_bounds__(256)
 gf_prep_kernel(const float* __restrict__ dmap, int h, int w, const float* __restrict__ img, long long img_sc, long long img_sp,
                int H, int W, float sy, float sx, const float* __restrict__ w0, const float* __restrict__ b0,
@@ -52,8 +66,6 @@ gf_prep_kernel(const float* __restrict__ dmap, int h, int w, const float* __rest
   }
   planes[p] = xv;
   planes[HW + p] = yv;
-  planes[2 * HW + p] = __fmul_rn(xv, yv);
-  planes[3 * HW + p] = __fmul_rn(xv, xv);
 }
 
 // box_filter.py's diff_x / diff_y of the rounded prefix sums cs of one line of length n (element i at cs[i * step]):
@@ -61,23 +73,6 @@ gf_prep_kernel(const float* __restrict__ dmap, int h, int w, const float* __rest
 __device__ __forceinline__ float box_diff(const float* cs, long long step, int i, int n, int r) {
   const float hi = cs[min(i + r, n - 1) * step];
   return i > r ? __fsub_rn(hi, cs[(i - r - 1) * step]) : hi;
-}
-
-// One thread per (plane, line): prefix sums along the line in double, each rounded to fp32 (ATen's float cumsum),
-// then box_diff. Lines run along H (columns, `step` = W, consecutive threads on consecutive columns) or along W (rows,
-// `step` = 1). src may equal dst (each thread reads its whole line before writing it).
-__global__ void __launch_bounds__(128)
-gf_scan_diff_kernel(const float* src, float* __restrict__ cs, float* dst, int planes, int lines,
-                    long long line_stride, int n, long long step, int r, long long plane_stride) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= planes * lines) return;
-  const long long base = (long long)(t / lines) * plane_stride + (long long)(t % lines) * line_stride;
-  double s = 0.0;
-  for (int i = 0; i < n; ++i) {
-    s += (double)src[base + i * step];
-    cs[base + i * step] = (float)s;
-  }
-  for (int i = 0; i < n; ++i) dst[base + i * step] = box_diff(cs + base, step, i, n, r);
 }
 
 // N of guided_filter.py: the box filter of ones, i.e. the number of pixels of the (2r+1)^2 window inside the image
@@ -103,49 +98,6 @@ struct GfCoef {
 __device__ __forceinline__ float gf_out(float bA, float bb, float x, float N) {
   return __fadd_rn(__fmul_rn(__fdiv_rn(bA, N), x), __fdiv_rn(bb, N));
 }
-
-// box sums of [x | y | xy | xx] -> A, b (guided_filter.py: N, mean_x, mean_y, cov_xy, var_x, A, b)
-__global__ void __launch_bounds__(256)
-gf_coef_kernel(const float* __restrict__ box, int H, int W, int r, float eps, float* __restrict__ A, float* __restrict__ b) {
-  const long long HW = (long long)H * W;
-  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= HW) return;
-  const float N = box_count((int)(p / W), (int)(p % W), H, W, r);
-  const GfCoef k(box[p], box[HW + p], box[2 * HW + p], box[3 * HW + p], N, eps);
-  A[p] = k.A;
-  b[p] = k.b;
-}
-
-// out = box(A)/N * x + box(b)/N
-__global__ void __launch_bounds__(256)
-gf_out_kernel(const float* __restrict__ box_ab, const float* __restrict__ x, int H, int W, int r, float* __restrict__ out) {
-  const long long HW = (long long)H * W;
-  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= HW) return;
-  const float N = box_count((int)(p / W), (int)(p % W), H, W, r);
-  out[p] = gf_out(box_ab[p], box_ab[HW + p], x[p], N);
-}
-
-// box filter of `np` planes of src (plane stride HW) into dst, cs as scratch: column pass src -> dst, row pass dst -> dst
-void box_filter(const float* src, float* cs, float* dst, int np, int H, int W, int r, cudaStream_t st) {
-  const long long HW = (long long)H * W;
-  gf_scan_diff_kernel<<<ceil_div((long long)np * W, 128), 128, 0, st>>>(src, cs, dst, np, W, 1, H, W, r, HW);
-  gf_scan_diff_kernel<<<ceil_div((long long)np * H, 128), 128, 0, st>>>(dst, cs, dst, np, H, W, W, 1, r, HW);
-}
-
-// ---- models/GF GuidedFilter / BoxFilter on N x C x H x W planes, forward and backward (the autograd mirrors) ---------
-//
-// Parallel scans. A column pass (lines along H) gives a block 32 adjacent columns of one plane and cuts each column into
-// GF_COL_SEG segments, one per threadIdx.y: loads stay coalesced across the 32 columns. A row pass (lines along W) gives
-// each row a warp and each lane a contiguous segment. Every thread sums its segment in double, the segment totals are
-// scanned in double (shared memory across threadIdx.y, shuffles across lanes), and the thread re-walks its segment from
-// that offset, rounding each prefix to fp32. Only the double sums are reassociated; the fp32 prefixes are those of the
-// sequential double accumulation unless a reassociated double lands on the other side of an fp32 rounding boundary.
-//
-// Forward pass (ADJ = false): prefix sums cs (ATen's cumsum), then box_diff into dst. dst may be the source plane.
-// Adjoint pass (ADJ = true), autograd's order through box_filter.py: first the adjoint of box_diff (the slice / cat
-// backward: d cs[i] = g[i - r] - g[i + r + 1], and at i = n-1 the broadcast `right` slice's sum g[n-r..n-1] added to
-// g[n-1-r]), then cumsum's backward, a reverse prefix sum in double rounded per position. dst must not be the source.
 
 constexpr int GF_COL_SEG = 16;   // column pass: 32 columns x 16 segments per block
 constexpr int GF_ROW_WARPS = 4;  // row pass: one warp per row, 4 rows per block
@@ -433,29 +385,24 @@ int check_gf_dims(int N, int Cx, int Cy, int H, int W, int r) {
 
 extern "C" {
 
-long long nrgbd_guided_filter_workspace_floats(int H, int W) { return 12LL * H * W; }
+// workspace [x | y | the GuidedFilter forward's workspace for one plane]
+long long nrgbd_guided_filter_workspace_floats(int H, int W) {
+  return 2LL * H * W + nrgbd_gf_workspace_floats(1, 1, 1, H, W, 0);
+}
 
+// gf_prep_kernel writes the guide x and the upsampled depth y, then nrgbd_guided_filter filters y guided by x
 int nrgbd_guided_filter_refine(const float* dmap, int h, int w, const float* img, long long img_sc, long long img_sp, int H,
                                int W, const float* w0, const float* b0, const float* w1, const float* b1, int r, float eps,
                                float* ws, float* out, cudaStream_t st) {
   NRGBD_REQUIRE(dmap && img && w0 && b0 && w1 && b1 && ws && out, "null pointer");
   NRGBD_REQUIRE(h > 0 && w > 0 && H % h == 0 && W % w == 0 && H / h == W / w && H / h > 1,
                 "the guide must be an integer multiple > 1 of the depth map's size, the same in both axes (Refine.py:633-637)");
-  NRGBD_REQUIRE(r >= 0 && H > 2 * r + 1 && W > 2 * r + 1, "guide smaller than the box (guided_filter.py:73)");
+  if (int rc = check_gf_dims(1, 1, 1, H, W, r)) return rc;
   const long long HW = (long long)H * W;
-  float* planes = ws;             // [x | y | xy | xx], then [x | A | b]
-  float* cs = ws + 4 * HW;        // prefix sums
-  float* box = ws + 8 * HW;       // box sums
-  const unsigned grid = (unsigned)ceil_div(HW, 256);
   const float sy = h > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f, sx = w > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
-  gf_prep_kernel<<<grid, 256, 0, st>>>(dmap, h, w, img, img_sc, img_sp, H, W, sy, sx, w0, b0, w1, b1, planes);
-  box_filter(planes, cs, box, 4, H, W, r, st);
-  gf_coef_kernel<<<grid, 256, 0, st>>>(box, H, W, r, eps, planes + HW, planes + 2 * HW);
-  box_filter(planes + HW, cs, box, 2, H, W, r, st);
-  gf_out_kernel<<<grid, 256, 0, st>>>(box, planes, H, W, r, out);
-  NRGBD_COUNT(7);
-  NRGBD_LAUNCH_CHECK();
-  return NRGBD_OK;
+  gf_prep_kernel<<<ceil_div(HW, 256), 256, 0, st>>>(dmap, h, w, img, img_sc, img_sp, H, W, sy, sx, w0, b0, w1, b1, ws);
+  NRGBD_COUNT(1);
+  return nrgbd_guided_filter(ws, ws + HW, 1, 1, 1, H, W, r, eps, ws + 2 * HW, out, st);
 }
 
 long long nrgbd_box_filter_workspace_floats(int N, int C, int H, int W) { return (long long)N * C * H * W; }

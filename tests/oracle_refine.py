@@ -102,13 +102,15 @@ def dgf_refine(dmap, img, sd, pre='r_net.'):
 
 # ---- seeded inputs of the guided filter alone (tests/golden/make_golden.py refine, tests/test_gpu_refine.py) -----------
 GF_CASES = ['gf_ragged_13x17_x4', 'gf_ragged_37x53_x2', 'gf_textured_120x160_x4', 'gf_flat_120x160_x4']
+GF_ENGINE_CASES = ['gf_textured_256x256_x4', 'gf_textured_480x640_x4']     # the engine's sizes, checked against the oracle only
 
 
 def gf_case(name):
     """-> dict(dmap [h][w], img [3][H][W], sd {r_net.feature_ext.*}) in float32."""
     from neuralrgbd_b200 import synth
     h, w, ratio, seed = {'gf_ragged_13x17_x4': (13, 17, 4, 71), 'gf_ragged_37x53_x2': (37, 53, 2, 72),
-                         'gf_textured_120x160_x4': (30, 40, 4, 73), 'gf_flat_120x160_x4': (30, 40, 4, 74)}[name]
+                         'gf_textured_120x160_x4': (30, 40, 4, 73), 'gf_flat_120x160_x4': (30, 40, 4, 74),
+                         'gf_textured_256x256_x4': (64, 64, 4, 75), 'gf_textured_480x640_x4': (120, 160, 4, 76)}[name]
     rng = np.random.RandomState(seed)
     H, W = h * ratio, w * ratio
     dmap = (2.5 + synth.smooth_image(rng, 1, h, w)[0]).astype(f32)

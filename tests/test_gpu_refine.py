@@ -2,7 +2,7 @@
 
  * Op level: nrgbd_guided_filter_refine against tests/oracle_refine.py, bit for bit, on ragged sizes, a textured guide and a
    guide that is flat over whole regions (var_x = 0 there: A = cov / 1e-8), against the reference's RefineNet_DGF within its
-   pinned floor, and bit-identical from run to run.
+   pinned floor, and bit-identical from run to run; bit for bit against the oracle at the engine's 256x256 and 480x640.
  * Engine against tests/golden/make_golden.py refine (unmodified reference, re-seeded steady steps) in all three conv_math
    modes. if_refined=False: -1 for both refined outputs, probabilities at 1e-4 on first windows and the train-mode K-Net gate
    on steady steps. DGF: depth maps in metres at GATE_MULT times the larger pinned oracle-vs-reference deviation of the step
@@ -36,15 +36,17 @@ STEPS = {'kvnet_256_d16': 3, 'c23_640x480_d64_v4_stream30': 2}
 
 
 # ---- op level ----------------------------------------------------------------------------------------------------------
+def _gf_refine(g):
+    from neuralrgbd_b200 import convops
+    sd = {k: T(v) for k, v in g['sd'].items()}
+    return convops.guided_filter_refine(T(g['dmap']), T(g['img']), sd['r_net.feature_ext.0.weight'], sd['r_net.feature_ext.0.bias'],
+                                        sd['r_net.feature_ext.2.weight'], sd['r_net.feature_ext.2.bias'])
+
+
 @pytest.mark.parametrize('name', R.GF_CASES)
 def test_guided_filter_kernel_vs_oracle(name):
-    from neuralrgbd_b200 import convops
     g = R.gf_case(name)
-    sd = {k: T(v) for k, v in g['sd'].items()}
-    run = lambda: convops.guided_filter_refine(T(g['dmap']), T(g['img']), sd['r_net.feature_ext.0.weight'],   # noqa: E731
-                                               sd['r_net.feature_ext.0.bias'], sd['r_net.feature_ext.2.weight'],
-                                               sd['r_net.feature_ext.2.bias'])
-    y = run()
+    y = _gf_refine(g)
     got = y.cpu().numpy()
     want = R.dgf_refine(g['dmap'], g['img'], g['sd'])
     ref = harness.golden('refine_outputs.npz')['refine/gf/%s/out' % name]
@@ -52,7 +54,17 @@ def test_guided_filter_kernel_vs_oracle(name):
     harness.parity_dump('refine', 'gf/%s' % name, row)
     assert np.array_equal(got, want), row
     assert row['reference_m'] <= harness.pinning('PINNING_refine.json')['gf/%s' % name]['oracle_m'], row
-    assert torch.equal(run(), y), 'not bit-identical from run to run'
+    assert torch.equal(_gf_refine(g), y), 'not bit-identical from run to run'
+
+
+@pytest.mark.parametrize('name', R.GF_ENGINE_CASES)
+def test_guided_filter_kernel_vs_oracle_at_engine_sizes(name):
+    """256x256 (kvnet_256_d16) and 480x640 (c23), where the column pass's segments and the row pass's lane segments are
+    long: bit for bit against the oracle."""
+    g = R.gf_case(name)
+    got, want = _gf_refine(g).cpu().numpy(), R.dgf_refine(g['dmap'], g['img'], g['sd'])
+    assert np.array_equal(got, want), {'oracle_m': maxabs(got, want), 'differing': int((got != want).sum()),
+                                       'first': np.argwhere(got != want)[:4].tolist()}
 
 
 # ---- engine ------------------------------------------------------------------------------------------------------------

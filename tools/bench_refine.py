@@ -109,9 +109,11 @@ def gf_kernel(H=480, W=640, iters=200):
     torch.cuda.synchronize()
     ms = a.elapsed_time(b) / iters
     HW, hw = H * W, H * W // 16
-    # prep: dmap + rgb in, 4 planes out; each box filter: 2 passes x (read plane, write prefix, read prefix, write diff) over
-    # 4 then 2 planes; coefficients: 4 in, 2 out; output: 2 box planes + x in, 1 out
-    floats = (hw + 3 * HW + 4 * HW) + 8 * 4 * HW + 6 * HW + 8 * 2 * HW + 4 * HW
+    # prep: dmap + rgb in, x and y out; each scan pass reads its source planes twice (segment totals, then the prefix walk)
+    # and writes prefix, reads prefix, writes diff per output plane: column pass to [x | y | x*y | x*x] (5 source planes:
+    # the products formed from x and y while loading), row pass over those 4, column pass to [A | b] (each from the 4 box
+    # planes), row pass over those 2; output: 2 box planes + x in, 1 out
+    floats = (hw + 3 * HW + 2 * HW) + (2 * 5 + 3 * 4) * HW + (2 + 3) * 4 * HW + (2 * 8 + 3 * 2) * HW + (2 + 3) * 2 * HW + 4 * HW
     return {'ms': ms, 'bytes': 4.0 * floats, 'GB_per_s': 4.0 * floats / (ms * 1e-3) / 1e9, 'shape': [H, W]}
 
 
